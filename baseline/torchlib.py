@@ -1,6 +1,6 @@
 """BENCH COMPARISON ARM ONLY — the reference's op chain on the PyTorch *library* path, on the GPU, in bf16.
 
-SURVEY.md §2.2 / §8(d): the reference has no hand-written kernel on the hot path; what it launches on a B200 is
+SURVEY.md §2.2 / §8(d): the reference has no hand-written kernel on the hot path; what it launches on an H100 is
 `F.linear` (cuBLASLt), `F.layer_norm`, `F.scaled_dot_product_attention` (flash / cuDNN), `F.gelu`, elementwise torch ops,
 and cuDNN `conv3d` for the VAE.  The UNMODIFIED reference cannot travel to the GPU box (no /root/reference there, and it
 needs deepspeed / omegaconf / pytorch_lightning), so `bench.py --impl torchlib` and the `library_baseline` key time THIS

@@ -1,6 +1,6 @@
 """bench.py — SCAIL-14B denoising steps/sec at 512p/81f (config A of BASELINE.json / SURVEY §8d).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one sampler step of the reference (sgm/modules/diffusionmodules/sampling.py:950-963): the
 CFG-duplicated batch-2 DiT forward over the ref || noise || pose sequence (N = 27 904 tokens, 40 blocks,
@@ -8,6 +8,10 @@ hidden 5120), CFG combine and the Euler update.  `value` = steps/s with inputs r
 same step through scail_b200.sampler.HostStep (pinned host -> device inputs, device -> host latent) timed
 inside the region; `fwd_per_s` (extra key) = value * 2 is the b=1-forward rate BASELINE.md's targets are
 quoted on (SURVEY F3).  Random-init weights of the 14B architecture, synthetic inputs (no network).
+
+--dump-outputs DIR: after the timed steps, DIR/x.npy holds the fp32 latent the last timed step returned (what a caller of
+sampler_step receives).  Weights and inputs are seeded, so two builds run with the same arguments can be compared output
+for output.
 
 N > 1: one process per GPU (torchrun); strong scaling (the step is fixed).  Default layout for even N
 (`--parallel auto`): the two CFG branches on the two halves of the ranks, context parallel over the token dimension
@@ -42,7 +46,6 @@ import torch  # noqa: E402
 D, F, HEADS, LAYERS, TEXT_DIM = 5120, 13824, 40, 40, 4096
 T_LAT, H_LAT, W_LAT = 21, 64, 64  # 512x512, 81 frames
 N_TEXT, N_CLIP = 512, 257
-NCU_ATTN_DRAM_BYTES = 1.723713e9 + 0.555318e9  # per self-attention launch (b=2, 40 heads, N=27904), profiles/r02_ncu_summary.md
 
 
 def seq_len(t=None, h=None, w=None):
@@ -65,7 +68,7 @@ def measured_peaks():
     if os.path.isfile(p):
         d = json.load(open(p))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "NVIDIA H100 SXM data sheet (dense, 700 W)"
 
 
 class ClockSampler:
@@ -363,6 +366,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip library_baseline / kernel_compare / vae_decode (profiling runs)")
     ap.add_argument("--layers", type=int, default=LAYERS, help=argparse.SUPPRESS)  # debugging only; default = full model
     ap.add_argument("--no-cpu-baseline", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the fp32 latent returned by the last timed step to DIR/x.npy")
     ap.add_argument("--latent", default=None, help="TxHxW latent override, e.g. 21x64x112 (the reference's default 512x896); "
                     "the default 21x64x64 is the BASELINE.json config")
     args = ap.parse_args()
@@ -441,6 +446,7 @@ def main():
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1) / args.steps
+        x_last = x.float().cpu() if args.dump_outputs else None
         launches = (ops.LAUNCHES - launches0) // args.steps
         attn_ms = [a.elapsed_time(b) for a, b in ops.ATTN_EVENTS]
         ops.ATTN_EVENTS = None
@@ -485,9 +491,8 @@ def main():
                         "achieved": attn_flops / attn_avg / 1e9 if attn_avg else None,
                         "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
                         "frac": attn_flops / attn_avg / 1e9 / peaks["bf16_tflops_sustained"] if attn_avg else None,
-                        "traffic": NCU_ATTN_DRAM_BYTES if (world == 1 and args.latent is None) else None,
-                        "traffic_source": "dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` capture of this "
-                                          "launch shape (profiles/r02_ncu_summary.md); algorithmic Q+K+V+O bytes = 2.286e9",
+                        "traffic": 4 * 2 * (n / world) * D * 2 if world == 1 else None,
+                        "traffic_source": "algorithmic Q+K+V+O bytes of one launch, computed from the shapes",
                         "peak_source": peak_src + ", sustained figure (kernel timed inside a long step)",
                         "algorithmic_flops_per_launch": attn_flops, "avg_launch_ms": attn_avg,
                         "share_of_step": sum(attn_ms) / args.steps / ms if attn_ms else None}}
@@ -546,6 +551,10 @@ def main():
             torch.cuda.empty_cache()
     if not args.no_cpu_baseline and world >= 1 and not lib_arm:
         out["cpu_baseline"] = cpu_baseline()
+    if x_last is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "x.npy"), x_last.numpy())
     print(json.dumps(out))
 
 

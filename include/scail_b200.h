@@ -1,4 +1,4 @@
-/* scail_b200 — C ABI of the Blackwell-native SCAIL denoising path (libscail_b200.so).
+/* scail_b200 — C ABI of the Hopper-native (sm_90a) SCAIL denoising path (libscail_b200.so).
  *
  * Boundary contract (SURVEY.md §8b):
  *  - every buffer is caller-owned device memory (a PyTorch tensor's data_ptr); the library never
@@ -27,8 +27,6 @@ const char* scail_last_error(void);
 int scail_version(void);
 /* device properties the host side sizes grids with; returns <0 when no CUDA device is usable */
 int scail_device_sm_count(int device);
-/* perf experiments only: int64[64*8] device buffer receiving clock64 stamps of attention CTA (0,0,0); NULL disables */
-int scail_debug_set_attention_trace(void* buf);
 
 /* GEMM epilogues */
 enum {
@@ -43,8 +41,7 @@ enum {
 /* C[M,N] = epilogue(A[M,K] @ W[N,K]^T); A, W, C bf16 row-major with leading dims lda/ldw/ldc
  * (elements, multiples of 8; ldc % 4 for a float32 C).  bias [N] bf16 or NULL; gate [B, gate_stride] bf16 indexed by
  * row / rows_per_batch; residual [M, ldr] bf16.  c_fp32 != 0 writes float32 C instead.  C, bias, gate and residual must be
- * 16-byte aligned (-1 otherwise).  Shapes with >= one 256x256 tile pair per SM pair run on the CTA-pair kernel
- * (tcgen05 cta_group::2, cluster of 2 CTAs), the others on the single-CTA kernel; same numerics.
+ * 16-byte aligned (-1 otherwise).
  * Replaces ColumnParallelLinear.forward / RowParallelLinear.forward (sat/mpu/layers.py:230-243,
  * :425-444) and nn.Linear / nn.Conv3d-as-GEMM call sites of the DiT. */
 int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
@@ -129,7 +126,7 @@ int scail_cast_f32_bf16(const float* x, void* out, int64_t n, scail_stream_t str
 /* ---- Wan2.1 VAE decode (sgm/models/wan_vae.py); activations channels-last bf16 [T, H, W, C] ---- */
 enum { SCAIL_CONV_EPI_BIAS = 0, SCAIL_CONV_EPI_BIAS_RES = 1, SCAIL_CONV_EPI_HEAD_CLAMP = 2 };
 
-/* Causal 3-D convolution as an implicit GEMM on tcgen05 (CausalConv3d.forward, wan_vae.py:17-36; also the
+/* Causal 3-D convolution as an implicit GEMM on wgmma (CausalConv3d.forward, wan_vae.py:17-36; also the
  * per-frame Conv2d 3x3 of Resample with KT = 1, :77-83).  x [T,H,W,Cin]; w2 = weight repacked to
  * [Cout, KT*KH*KW*Cin] (tap-major, channel-minor); stride 1, "same" spatial zero padding, causal temporal
  * padding (KT-1 zero frames on the left).  Output column c is written to frame t*fmul + c/ocols, channel

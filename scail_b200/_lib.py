@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _VARIANT = os.environ.get("SCAIL_LIB_VARIANT", "")
 LIB_PATH = os.path.join(_HERE, f"libscail_b200_{_VARIANT}.so" if _VARIANT else "libscail_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
 c_p, c_i64, c_int, c_f = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_float
@@ -22,7 +22,6 @@ c_p, c_i64, c_int, c_f = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c
 SIGNATURES = {
     "scail_version": [],
     "scail_device_sm_count": [c_int],
-    "scail_debug_set_attention_trace": [c_p],
     "scail_gemm_bf16": [c_p, c_i64, c_p, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_p, c_i64, c_i64, c_p,
                         c_i64, c_int, c_p],
     "scail_ln_modulate": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
@@ -70,10 +69,10 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """Compile the CUDA extension in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA extension in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     if not force and not needs_build():
         return LIB_PATH
-    extra = os.environ.get("SCAIL_NVCC_EXTRA", "").split()  # e.g. -DSCAIL_ATTN_EXPERIMENTS for scripts/trace_attn.py
+    extra = os.environ.get("SCAIL_NVCC_EXTRA", "").split()  # extra nvcc flags for experiments, e.g. -DSCAIL_MBAR_DEBUG
     cmd = ["nvcc", *NVCC_FLAGS, *extra, "-o", LIB_PATH, os.path.join(CSRC, "api.cu"), "-lcudart", "-ldl"]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")

@@ -161,7 +161,6 @@ int make_tmap_cl4d(const void* ptr, uint64_t T, uint64_t H, uint64_t W, uint64_t
     return 0;
 }
 
-long long* g_attn_trace = nullptr;  // perf experiments only
 constexpr int MAX_DEVICES = 64;
 int g_sm_count[MAX_DEVICES] = {0};  // per device: a process may drive several GPUs
 int sm_count() {
@@ -236,11 +235,6 @@ extern "C" {
 const char* scail_last_error(void) { return g_err; }
 int scail_version(void) { return 100; }
 
-int scail_debug_set_attention_trace(void* buf) {
-    g_attn_trace = static_cast<long long*>(buf);
-    return 0;
-}
-
 int scail_device_sm_count(int device) {
     int n = 0;
     cudaError_t e = cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device);
@@ -275,27 +269,11 @@ int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, cons
     p.rows_per_batch = rows_per_batch > 0 ? (int)rows_per_batch : (int)M;
     p.epilogue = epilogue;
     static const int gm_env = getenv("SCAIL_GEMM_GROUP_M") ? atoi(getenv("SCAIL_GEMM_GROUP_M")) : 0;
-    static const int cg_env = getenv("SCAIL_GEMM_CG") ? atoi(getenv("SCAIL_GEMM_CG")) : 0;  // experiments: force 1 or 2
-    static const int hint_env = getenv("SCAIL_GEMM_L2_HINTS") ? atoi(getenv("SCAIL_GEMM_L2_HINTS")) : 1;
-    p.l2_hints = hint_env;
     const int sms = sm_count();
     SCAIL_REQUIRE(sms > 0, "gemm: no CUDA device");
-    // CTA-pair kernel for the big GEMMs (>= one 256-row tile pair per cluster); the 1-CTA kernel for short / skinny ones
-    const int64_t pair_tiles = blocks_for(M, 2 * GEMM_BM) * (int64_t)blocks_for(N, GEMM_BN);
-    const bool use_cg2 = cg_env ? cg_env == 2 : (M >= 2 * GEMM_BM && pair_tiles >= sms / 2);
-    if (use_cg2) {
-        if ((rc = make_tmap_2d(A, M, K, lda, 128, GEMM_BK, &ta))) return rc;
-        if ((rc = make_tmap_2d(W, N, K, ldw, 128, GEMM_BK, &tw))) return rc;
-        p.group_m = gm_env > 0 ? gm_env : 16;  // in 256-row pairs (sweep: profiles/r02_gemm_l2.md)
-        if ((rc = set_smem(gemm_bf16_cg2_kernel, GEMM2_SMEM_BYTES))) return rc;
-        int grid = (int)(2 * pair_tiles < sms ? 2 * pair_tiles : (sms & ~1));
-        gemm_bf16_cg2_kernel<<<grid, GEMM_THREADS, GEMM2_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(ta, tw, p);
-        SCAIL_CHECK_CUDA(cudaGetLastError());
-        return 0;
-    }
     if ((rc = make_tmap_2d(A, M, K, lda, GEMM_BM, GEMM_BK, &ta))) return rc;
     if ((rc = make_tmap_2d(W, N, K, ldw, GEMM_BN, GEMM_BK, &tw))) return rc;
-    p.group_m = gm_env > 0 ? gm_env : 24;
+    p.group_m = gm_env > 0 ? gm_env : 16;
     if ((rc = set_smem(gemm_bf16_kernel, GEMM_SMEM_BYTES))) return rc;
     const int num_tiles = blocks_for(M, GEMM_BM) * blocks_for(N, GEMM_BN);
     const int grid = num_tiles < sms ? num_tiles : sms;
@@ -371,11 +349,8 @@ static int attention_impl(const void* Q, int64_t ldq, const void* K, int64_t ldk
     p.o32 = o32; p.ldo32 = ldo32; p.state = static_cast<float2*>(state); p.heads = (int)H;
     p.scale_log2 = scale * 1.4426950408889634f;
     p.accumulate = accumulate;
-    p.trace = g_attn_trace;
-    static const int dbg = getenv("SCAIL_ATTN_DEBUG") ? atoi(getenv("SCAIL_ATTN_DEBUG")) : 0;  // honoured only by -DSCAIL_ATTN_EXPERIMENTS builds
-    p.debug = dbg;
     if ((rc = set_smem(attention_fwd_kernel, ATT_SMEM_BYTES))) return rc;
-    dim3 grid(blocks_for(q_len, 2 * ATT_BQ), (unsigned)H, (unsigned)B);
+    dim3 grid(blocks_for(q_len, ATT_BQ), (unsigned)H, (unsigned)B);
     attention_fwd_kernel<<<grid, ATT_THREADS, ATT_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(tq, tk, tv, p);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -1,70 +1,30 @@
-// Warp-specialised flash attention forward for sm_100a (head_dim 128, bf16, non-causal).
+// Warp-specialised flash attention forward for sm_90a (head_dim 128, bf16, non-causal).
 // Replaces F.scaled_dot_product_attention in sat/transformer_defaults.py:67-72 for both the
 // spatiotemporal self-attention (dit_video_crossattn_sc_xc.py:1092-1094) and the two short-KV
 // cross-attention calls (:1159-1197).
 //
-// One CTA owns 256 query rows of one (batch, head): two 128-row Q tiles that ping-pong on the
-// tensor core.  Roles (12 warps = 3 warpgroups, registers re-split with setmaxnreg):
-//   warps 0-3  softmax warpgroup for Q tile 0      warps 4-7  softmax warpgroup for Q tile 1
-//   warp  8    TMA producer (Q once, K/V rings)     warp  9    tcgen05.mma issuer + TMEM owner   (10, 11 idle)
-// The MMA warp keeps its control flow warp-uniform (all lanes wait on the mbarriers; descriptors are computed in
-// uniform registers) and only the tcgen05 instructions are issued by the elected lane.
-//
-// TMEM (512 columns): S0 | S1 | O0 | O1, 128 fp32 columns each; P (bf16) aliases the first 64 columns of its S buffer and
-// feeds the PV product as the TMEM A operand (no smem round trip).
-//   S = Q K^T : UMMA 128x128x16, A/B K-major from smem (TMA SWIZZLE_128B) -- measured (scripts/umma_microbench.cu): this shape
-//               reads 8 KB of operands per 64-cycle UMMA = exactly the 128 B/clk/SM shared-memory operand bandwidth; the
-//               N = 64 variant is operand-bound at 48 instead of 32 cycles, which is why S is NOT split into halves.
-//   O += P V  : UMMA 128x128x16, A from TMEM, B = V tile read MN-major straight from its [kv, d] layout (full rate).
-// Because P aliases S, one Q tile's loop-carried chain is  S -> softmax -> P -> PV -> next QK^T -> S, and the step time is
-// max(2048 cycles of UMMA, softmax latency + the part of PV + QK^T that cannot start before the last P column exists).
-// Two things shorten that chain:
-//   * P is handed over in ATT_P_SPLIT column groups with one mbarrier each, so the PV UMMAs of the first groups run while
-//     the later exponentials are still being computed (only the last group's k-steps stay on the chain);
-//   * a fraction of the exponentials (ATT_POLY_MASK) runs as a Cody-Waite + cubic polynomial on the FMA pipe: MUFU.EX2
-//     (16/clk/SM) alone needs 1024 cycles per 128x128 tile.
-// Online softmax keeps a (possibly stale) running max; O is rescaled only when the max grew by > 2^8 (S full implies the
-// previous PV of that tile has completed, so the read-modify-write of O cannot race the tensor core).
+// One CTA owns 128 query rows of one (batch, head).  Roles (12 warps = 3 warpgroups, registers re-split with setmaxnreg):
+//   warpgroup 0: one TMA producer warp (Q once, K and V rings);  warpgroups 1, 2: 64 query rows each.
+// Per 128-key tile a consumer warpgroup computes
+//   S = Q K^T : wgmma m64n128k16 x 8, Q and K K-major from shared memory (TMA SWIZZLE_128B), S in registers,
+//   online softmax on the S fragments (a row lives in the 4 lanes of a quad), P rounded to bf16 in registers,
+//   O += P V  : wgmma m64n128k16 x 8 with A = P straight from registers (the S accumulator fragment IS the A-operand
+//               fragment of the next MMA) and B = the V tile read MN-major from its [kv, d] layout.
+// The two warpgroups run independently, so one's softmax overlaps the other's tensor-core work.
 #pragma once
-#include "sm100.cuh"
-
-#ifdef SCAIL_ATTN_EXPERIMENTS
-#define SCAIL_ATTN_TRACE(IDX) if (tr) p.trace[IDX] = clock64()
-#define SCAIL_ATTN_TRACE_DECL_MMA
-#else
-#define SCAIL_ATTN_TRACE(IDX)
-#define SCAIL_ATTN_TRACE_DECL_MMA
-#endif
-
-#ifndef SCAIL_ATT_POLY_MASK
-#define SCAIL_ATT_POLY_MASK 0x8888u  // bit c set: column pair c of every 16-pair chunk uses the FMA-pipe exp2 (25 %)
-#endif
-#ifndef SCAIL_ATT_K_STAGES
-#define SCAIL_ATT_K_STAGES 3
-#endif
-#ifndef SCAIL_ATT_P_SPLIT
-#define SCAIL_ATT_P_SPLIT 4  // P hand-over groups per tile: 1, 2, 4 = equal groups of 128 / SPLIT keys; 3 = two groups of 96 + 32 keys
-#endif
+#include "sm90.cuh"
 
 namespace scail {
 
 constexpr int ATT_D = 128;
-constexpr int ATT_BQ = 128;   // rows per Q tile (2 tiles per CTA)
+constexpr int ATT_BQ = 128;   // query rows per CTA (64 per consumer warpgroup)
 constexpr int ATT_BKV = 128;  // keys per K/V tile
-constexpr int ATT_K_STAGES = SCAIL_ATT_K_STAGES;
-constexpr int ATT_V_STAGES = 2;
-constexpr int ATT_P_MODE = SCAIL_ATT_P_SPLIT;
-constexpr int ATT_P_SPLIT = ATT_P_MODE == 3 ? 2 : ATT_P_MODE;  // number of hand-over groups (mbarriers) per tile
-// last 32-key chunk (0..3) of hand-over group g, and the group a chunk belongs to
-__host__ __device__ constexpr int att_group_last_chunk(int g) { return ATT_P_MODE == 3 ? (g == 0 ? 2 : 3) : (g + 1) * (4 / ATT_P_SPLIT) - 1; }
-__host__ __device__ constexpr int att_chunk_group(int ch) { return ATT_P_MODE == 3 ? (ch < 3 ? 0 : 1) : ch / (4 / ATT_P_SPLIT); }
+constexpr int ATT_STAGES = 2;
 constexpr int ATT_TILE_BYTES = 128 * 128 * 2;  // 32 KB: one 128x128 bf16 tile (two 64-column halves)
 constexpr int ATT_HALF_BYTES = ATT_TILE_BYTES / 2;
-constexpr int ATT_THREADS = 384;  // 3 warpgroups: softmax0, softmax1, {TMA, MMA, 2 idle warps}
-constexpr uint32_t ATT_POLY_MASK = SCAIL_ATT_POLY_MASK;
-constexpr int ATT_SMEM_BYTES = (2 + ATT_K_STAGES + ATT_V_STAGES) * ATT_TILE_BYTES + 1024 + 256;
+constexpr int ATT_THREADS = 384;
+constexpr int ATT_SMEM_BYTES = (1 + 2 * ATT_STAGES) * ATT_TILE_BYTES + 1024 + 256;
 static_assert(ATT_SMEM_BYTES <= 232448, "attention: shared memory budget");
-static_assert(ATT_P_MODE >= 1 && ATT_P_MODE <= 4, "attention: P split");
 
 struct AttnParams {
     __nv_bfloat16* out;  // [B*q_rows_per_batch, ldo]; head h written at columns [h*128, h*128+128)
@@ -81,400 +41,196 @@ struct AttnParams {
     int kv_batch_rows;   // row stride between batches in the K/V matrices
     float scale_log2;    // softmax scale * log2(e)
     int accumulate;      // out += result (second cross-attention pass, dit_video_crossattn_sc_xc.py:1197)
-    long long* trace;    // perf experiments only: per-step clock64 stamps of CTA (0,0,0), or null
-    int debug;           // perf experiments only (SCAIL_ATTN_DEBUG): 1 = softmax skips its math, 5 = no QK^T UMMAs, 6 = no PV UMMAs
 };
 
-// exp2 of one 32-column chunk (16 packed pairs) -> 16 packed bf16x2 words of P; pairs selected by ATT_POLY_MASK use the
-// FMA-pipe polynomial, the others MUFU.EX2.  Row sums accumulate in two packed fp32 pairs.
-__device__ __forceinline__ void exp_chunk(const uint32_t (&src)[32], uint64_t sc2, uint64_t nm2, uint64_t& sum_a, uint64_t& sum_b,
-                                          uint32_t (&pk)[16]) {
-#pragma unroll
-    for (int c = 0; c < 16; ++c) {
-        const uint64_t y2 = fma_f32x2(pack_f32x2(__uint_as_float(src[2 * c]), __uint_as_float(src[2 * c + 1])), sc2, nm2);
-        uint64_t e2;
-        if ((ATT_POLY_MASK >> c) & 1u) {
-            e2 = poly_exp2_x2(y2);
-        } else {
-            float y0, y1;
-            unpack_f32x2(y2, y0, y1);
-            e2 = pack_f32x2(fast_exp2(y0), fast_exp2(y1));
-        }
-        if (c & 1) sum_b = add_f32x2(sum_b, e2);
-        else sum_a = add_f32x2(sum_a, e2);
-        float e0, e1;
-        unpack_f32x2(e2, e0, e1);
-        pk[c] = pack_bf16(e0, e1);
-    }
-}
-
-// One 128x128 score tile of one softmax warp (thread = row): TMEM S -> running max (lazy O rescale) -> exp2 ->
-// bf16 P back into TMEM, handed to the MMA warp in ATT_P_SPLIT groups.  MASK = this is the partial last KV tile.
-template <bool MASK>
-__device__ __forceinline__ void softmax_tile(uint32_t s_tmem, uint32_t o_tmem, float scale_log2, int valid, int j,
-                                             float& m_run, float& l_run, uint32_t bar_pfull0) {
-    uint32_t s0[32], s1[32], s2[32], s3[32];
-    tmem_ld_32x32(s_tmem + 0, s0);
-    tmem_ld_32x32(s_tmem + 32, s1);
-    tmem_ld_32x32(s_tmem + 64, s2);
-    tmem_ld_32x32(s_tmem + 96, s3);
-    tmem_ld_wait();
-    if constexpr (MASK) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-            if (c >= valid) s0[c] = 0xff800000u;
-            if (c + 32 >= valid) s1[c] = 0xff800000u;
-            if (c + 64 >= valid) s2[c] = 0xff800000u;
-            if (c + 96 >= valid) s3[c] = 0xff800000u;
-        }
-    }
-    float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-    for (int c = 0; c < 32; c += 2) {
-        mx0 = fmax3(mx0, __uint_as_float(s0[c]), __uint_as_float(s0[c + 1]));
-        mx1 = fmax3(mx1, __uint_as_float(s1[c]), __uint_as_float(s1[c + 1]));
-        mx2 = fmax3(mx2, __uint_as_float(s2[c]), __uint_as_float(s2[c + 1]));
-        mx3 = fmax3(mx3, __uint_as_float(s3[c]), __uint_as_float(s3[c + 1]));
-    }
-    const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-    const float m_new = fmaxf(m_run, mx * scale_log2);
-    const bool need = (m_new - m_run) > 8.0f;  // also true on the first tile (m_run = -inf)
-    if (__any_sync(0xffffffffu, need)) {
-        const float alpha = fast_exp2(m_run - m_new);  // 0 on the first tile
-        m_run = m_new;
-        l_run *= alpha;
-        if (j > 0) {
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                uint32_t o[32];
-                tmem_ld_32x32(o_tmem + c * 32, o);
-                tmem_ld_wait();
-#pragma unroll
-                for (int k = 0; k < 32; ++k) o[k] = __float_as_uint(__uint_as_float(o[k]) * alpha);
-                tmem_st_32x32(o_tmem + c * 32, o);
-            }
-        }
-    }
-    const float neg_m = -m_run;
-    const uint64_t sc2 = pack_f32x2(scale_log2, scale_log2), nm2 = pack_f32x2(neg_m, neg_m);
-    uint64_t sum_a = 0ull, sum_b = 0ull;  // packed (0.f, 0.f)
-    const bool lane0 = (threadIdx.x & 31) == 0;
-    // chunk CH = 32 keys = 16 packed P columns; after the last chunk of hand-over group g the warp arrives on bar_pfull0 + 8 * g
-#define SCAIL_ATT_P_CHUNK(SRC, CH)                                             \
-    {                                                                          \
-        uint32_t pk[16];                                                       \
-        exp_chunk(SRC, sc2, nm2, sum_a, sum_b, pk);                            \
-        tmem_st_32x16(s_tmem + (CH) * 16, pk);                                 \
-        if (att_group_last_chunk(att_chunk_group(CH)) == (CH)) {                \
-            tmem_st_wait();                                                    \
-            tc_fence_before();                                                 \
-            __syncwarp();                                                      \
-            if (lane0) mbar_arrive(bar_pfull0 + 8u * att_chunk_group(CH));    \
-        }                                                                      \
-    }
-    SCAIL_ATT_P_CHUNK(s0, 0)
-    SCAIL_ATT_P_CHUNK(s1, 1)
-    SCAIL_ATT_P_CHUNK(s2, 2)
-    SCAIL_ATT_P_CHUNK(s3, 3)
-#undef SCAIL_ATT_P_CHUNK
-    float la, lb, lc, ld;
-    unpack_f32x2(sum_a, la, lb);
-    unpack_f32x2(sum_b, lc, ld);
-    l_run += (la + lb) + (lc + ld);
-}
 
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                      const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t q_smem = smem_base;                                     // 2 tiles
-    const uint32_t k_smem = smem_base + 2 * ATT_TILE_BYTES;                // ATT_K_STAGES tiles
-    const uint32_t v_smem = k_smem + ATT_K_STAGES * ATT_TILE_BYTES;        // ATT_V_STAGES tiles
-    const uint32_t bar_base = v_smem + ATT_V_STAGES * ATT_TILE_BYTES;
+    const uint32_t q_smem = smem_base;                                // 1 tile
+    const uint32_t k_smem = smem_base + ATT_TILE_BYTES;               // ATT_STAGES tiles
+    const uint32_t v_smem = k_smem + ATT_STAGES * ATT_TILE_BYTES;     // ATT_STAGES tiles
+    const uint32_t bar_base = v_smem + ATT_STAGES * ATT_TILE_BYTES;
     enum {
         B_QFULL = 0,
-        B_KFULL = 1,                        // [ATT_K_STAGES]
-        B_KEMPTY = B_KFULL + ATT_K_STAGES,  // [ATT_K_STAGES]
-        B_VFULL = B_KEMPTY + ATT_K_STAGES,  // [ATT_V_STAGES]
-        B_VEMPTY = B_VFULL + ATT_V_STAGES,  // [ATT_V_STAGES]
-        B_SFULL = B_VEMPTY + ATT_V_STAGES,  // [tile]
-        B_OFULL = B_SFULL + 2,              // [tile]
-        B_PFULL = B_OFULL + 2,              // [tile * ATT_P_SPLIT + group]
-        B_COUNT = B_PFULL + 2 * ATT_P_SPLIT
+        B_KFULL = 1,                      // [ATT_STAGES]
+        B_KEMPTY = B_KFULL + ATT_STAGES,  // [ATT_STAGES]
+        B_VFULL = B_KEMPTY + ATT_STAGES,  // [ATT_STAGES]
+        B_VEMPTY = B_VFULL + ATT_STAGES,  // [ATT_STAGES]
+        B_COUNT = B_VEMPTY + ATT_STAGES
     };
-    static_assert(8 * B_COUNT + 8 <= 256, "attention: barrier area");
+    static_assert(8 * B_COUNT <= 256, "attention: barrier area");
     auto bar = [&](int i) { return bar_base + 8u * i; };
-    const uint32_t tmem_slot = bar_base + 8u * B_COUNT;
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int head = blockIdx.y;
     const int batch = blockIdx.z;
-    const int q0 = blockIdx.x * (2 * ATT_BQ);
+    const int q0 = blockIdx.x * ATT_BQ;
+    const int n_kv0 = (p.kv_len + ATT_BKV - 1) / ATT_BKV;
+    const int n_kv = n_kv0 + (p.kv_len1 + ATT_BKV - 1) / ATT_BKV;
 
-    if (warp == 8 && lane == 0) {
+    if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_q);
         tma_prefetch_desc(&tmap_k);
         tma_prefetch_desc(&tmap_v);
         mbar_init(bar(B_QFULL), 1);
-        for (int s = 0; s < ATT_K_STAGES; ++s) {
+        for (int s = 0; s < ATT_STAGES; ++s) {
             mbar_init(bar(B_KFULL + s), 1);
-            mbar_init(bar(B_KEMPTY + s), 1);
-        }
-        for (int s = 0; s < ATT_V_STAGES; ++s) {
+            mbar_init(bar(B_KEMPTY + s), 2);  // one arrive per consumer warpgroup
             mbar_init(bar(B_VFULL + s), 1);
-            mbar_init(bar(B_VEMPTY + s), 1);
+            mbar_init(bar(B_VEMPTY + s), 2);
         }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(bar(B_SFULL + i), 1);
-            mbar_init(bar(B_OFULL + i), 1);
-        }
-        for (int i = 0; i < 2 * ATT_P_SPLIT; ++i) mbar_init(bar(B_PFULL + i), 4);  // one arrive per softmax warp
         fence_barrier_init();
     }
-    if (warp == 9) {
-        tmem_alloc<1>(tmem_slot, 512);
-        tmem_relinquish<1>();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp >= 8) setmaxnreg_dec<88>();
-    if (warp == 8) {
+    if (warp < 4) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             const int col = head * ATT_D;
-            const int qrow = batch * p.q_batch_rows + q0;
-            mbar_expect_tx(bar(B_QFULL), 2 * ATT_TILE_BYTES);
-            for (int t = 0; t < 2; ++t)
-                for (int h = 0; h < 2; ++h)
-                    tma_load_2d(q_smem + t * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmap_q, bar(B_QFULL), col + h * 64,
-                                qrow + t * ATT_BQ);
+            mbar_expect_tx(bar(B_QFULL), ATT_TILE_BYTES);
+            for (int h = 0; h < 2; ++h)
+                tma_load_2d(q_smem + h * ATT_HALF_BYTES, &tmap_q, bar(B_QFULL), col + h * 64, batch * p.q_batch_rows + q0);
             const int kvbase = batch * p.kv_batch_rows;
-            const int n_kv0 = (p.kv_len + ATT_BKV - 1) / ATT_BKV;
-            const int n_kv = n_kv0 + (p.kv_len1 + ATT_BKV - 1) / ATT_BKV;
             // tile j of the concatenated key ranges starts at this row (a range's last tile may run past its end: masked)
             auto kv_row = [&](int j) { return kvbase + (j < n_kv0 ? p.kv_off + j * ATT_BKV : p.kv_off1 + (j - n_kv0) * ATT_BKV); };
-            auto load_k = [&](int j) {
-                const int s = j % ATT_K_STAGES;
-                mbar_wait(bar(B_KEMPTY + s), ((j / ATT_K_STAGES) & 1) ^ 1, 10);
-#ifdef SCAIL_ATTN_EXPERIMENTS
-                if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && j < 64) p.trace[j * 8 + 7] = clock64();
-#endif
+            for (int j = 0; j < n_kv; ++j) {
+                const int s = j % ATT_STAGES;
+                const uint32_t par = ((j / ATT_STAGES) & 1) ^ 1;
+                mbar_wait(bar(B_KEMPTY + s), par, 10);
                 mbar_expect_tx(bar(B_KFULL + s), ATT_TILE_BYTES);
                 for (int h = 0; h < 2; ++h)
                     tma_load_2d(k_smem + s * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmap_k, bar(B_KFULL + s), col + h * 64, kv_row(j));
-            };
-            auto load_v = [&](int j) {
-                const int s = j % ATT_V_STAGES;
-                mbar_wait(bar(B_VEMPTY + s), ((j / ATT_V_STAGES) & 1) ^ 1, 11);
+                mbar_wait(bar(B_VEMPTY + s), par, 11);
                 mbar_expect_tx(bar(B_VFULL + s), ATT_TILE_BYTES);
                 for (int h = 0; h < 2; ++h)
                     tma_load_2d(v_smem + s * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmap_v, bar(B_VFULL + s), col + h * 64, kv_row(j));
-            };
-            // K runs one tile ahead of V (QK^T of tile j+1 is issued during the PV work of tile j)
-            load_k(0);
-            for (int j = 0; j < n_kv; ++j) {
-                if (j + 1 < n_kv) load_k(j + 1);
-                load_v(j);
             }
         }
-    } else if (warp == 9) {
-        // ===================== MMA issuer =====================
-        // The whole warp runs the control flow (waits, descriptor arithmetic stay warp-uniform => uniform
-        // datapath); only the tcgen05 instructions themselves are issued by the elected lane.
-        const bool leader = elect_one_sync();
-        const int n_kv = (p.kv_len + ATT_BKV - 1) / ATT_BKV + (p.kv_len1 + ATT_BKV - 1) / ATT_BKV;
-        constexpr uint32_t idesc_qk = umma_idesc_bf16(128, 128, 0, 0);
-        constexpr uint32_t idesc_pv = umma_idesc_bf16(128, 128, 0, 1);  // B (=V) is MN-major
-        const uint64_t q_desc0 = umma_desc_kmajor_sw128(q_smem), q_desc1 = umma_desc_kmajor_sw128(q_smem + ATT_TILE_BYTES);
-        const uint64_t k_desc0 = umma_desc_kmajor_sw128(k_smem);
-        const uint64_t v_desc0 = umma_desc_mnmajor_sw128(v_smem, ATT_HALF_BYTES);
-        constexpr uint64_t STAGE_STEP = ATT_TILE_BYTES >> 4;  // descriptor address units are 16 B
-        auto issue_qk = [&](int tile, int ks) {
-#ifdef SCAIL_ATTN_EXPERIMENTS
-            if (p.debug == 5) return;
-#endif
-            const uint32_t d = tmem_base + tile * 128;
-            const uint64_t qa = tile ? q_desc1 : q_desc0, kb = k_desc0 + ks * STAGE_STEP;
-            if (leader) {
+    } else {
+        // ===================== consumer warpgroups: QK^T, softmax, PV, epilogue =====================
+        setmaxnreg_inc<232>();
+        const int wg = (warp >> 2) - 1;  // rows [64 wg, 64 wg + 64) of the CTA's 128
+        const int t = threadIdx.x & 127;
+        const bool releaser = t == 0;
+        const int quad = t & 3;
+        float m_run[2] = {-INFINITY, -INFINITY};  // running max of rows r, r + 8 (already multiplied by scale_log2)
+        float l_run[2] = {0.f, 0.f};               // this thread's partial row sums (reduced over the quad at the end)
+        float o[ATT_D / 2];
 #pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const uint64_t off = ((k >> 2) * ATT_HALF_BYTES + (k & 3) * 32) >> 4;
-                    umma_ss<1>(d, qa + off, kb + off, idesc_qk, k != 0);
-                }
-            }
-        };
-        // PV of one tile: group g's k-steps are issued as soon as the softmax warpgroup has handed that group of P over
-        auto issue_pv = [&](int tile, int vs, uint32_t parity, bool acc) {
-            const uint32_t d = tmem_base + 256 + tile * 128;
-            const uint32_t a = tmem_base + tile * 128;  // P aliases S columns [0,64)
-            const uint64_t vb = v_desc0 + vs * STAGE_STEP;
-#pragma unroll
-            for (int g = 0; g < ATT_P_SPLIT; ++g) {
-                mbar_wait(bar(B_PFULL + tile * ATT_P_SPLIT + g), parity, 23 + tile);
-                tc_fence_after();
-#ifdef SCAIL_ATTN_EXPERIMENTS
-                if (p.debug == 6) continue;
-#endif
-                if (leader) {
-                    // group g feeds the 16-key UMMA k-steps of its 32-key chunks (2 per chunk)
-                    const int k_lo = g == 0 ? 0 : 2 * (att_group_last_chunk(g - 1) + 1), k_hi = 2 * (att_group_last_chunk(g) + 1);
-#pragma unroll
-                    for (int k = k_lo; k < k_hi; ++k) {
-                        // 16 kv rows per step = 2048 B inside each 64-column half; halves are 16 KB apart (LBO)
-                        umma_ts(d, a + k * 8, vb + k * (2048 >> 4), idesc_pv, acc || k != 0);
-                    }
-                }
-            }
-        };
-        auto commit = [&](int b) {
-            if (leader) umma_commit(bar(b));
-        };
+        for (int i = 0; i < ATT_D / 2; ++i) o[i] = 0.f;
+        const uint64_t q_desc = wgmma_desc_kmajor_sw128(q_smem + wg * (64 * 128));
         mbar_wait(bar(B_QFULL), 0, 20);
-        mbar_wait(bar(B_KFULL + 0), 0, 21);
-        tc_fence_after();
-        issue_qk(0, 0);
-        commit(B_SFULL + 0);
-        issue_qk(1, 0);
-        commit(B_SFULL + 1);
-        commit(B_KEMPTY + 0);
+#pragma unroll 1
         for (int j = 0; j < n_kv; ++j) {
-            const int vs = j % ATT_V_STAGES;
-            const bool more = j + 1 < n_kv;
-            const int ks = (j + 1) % ATT_K_STAGES;
-            mbar_wait(bar(B_VFULL + vs), (j / ATT_V_STAGES) & 1, 22);
-#ifdef SCAIL_ATTN_EXPERIMENTS
-            const bool tr = p.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && j < 64 && leader;
-#endif
-            SCAIL_ATTN_TRACE(j * 8 + 0);
-            issue_pv(0, vs, j & 1, j > 0);
-            SCAIL_ATTN_TRACE(j * 8 + 1);
-            if (more) {
-                mbar_wait(bar(B_KFULL + ks), ((j + 1) / ATT_K_STAGES) & 1, 24);
-                tc_fence_after();
-                issue_qk(0, ks);
-                commit(B_SFULL + 0);
-            } else {
-                commit(B_OFULL + 0);
-            }
-            SCAIL_ATTN_TRACE(j * 8 + 2);
-            issue_pv(1, vs, j & 1, j > 0);
-            SCAIL_ATTN_TRACE(j * 8 + 3);
-            commit(B_VEMPTY + vs);
-            if (more) {
-                issue_qk(1, ks);
-                commit(B_SFULL + 1);
-                commit(B_KEMPTY + ks);
-            } else {
-                commit(B_OFULL + 1);
-            }
-        }
-    } else if (warp < 8) {
-        // ===================== softmax warpgroups (+ O rescale + epilogue) =====================
-        setmaxnreg_inc<208>();
-        const int tile = warp >> 2;  // 0 or 1
-        const int sub = warp & 3;
-        const uint32_t lane_off = static_cast<uint32_t>(sub * 32) << 16;
-        const uint32_t s_tmem = tmem_base + lane_off + tile * 128;
-        const uint32_t o_tmem = tmem_base + lane_off + 256 + tile * 128;
-        const uint32_t bar_p0 = bar(B_PFULL + tile * ATT_P_SPLIT);
-        float m_run = -INFINITY;  // running max, already multiplied by scale_log2
-        float l_run = 0.f;
-        int j = 0;  // tile counter over both key ranges (mbarrier parity, "first tile" test)
-#pragma unroll 1
-        for (int r = 0; r < 2; ++r) {
-            const int len = r == 0 ? p.kv_len : p.kv_len1;
-            const int j_end = j + len / ATT_BKV;  // full tiles of this range; an optional partial tile follows (peeled)
-            for (; j < j_end; ++j) {
-#ifdef SCAIL_ATTN_EXPERIMENTS
-                const bool tr = p.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && j < 64 && warp == 0 && lane == 0;
-#endif
-                SCAIL_ATTN_TRACE(j * 8 + 4);
-                mbar_wait(bar(B_SFULL + tile), j & 1, 30 + tile);
-                SCAIL_ATTN_TRACE(j * 8 + 5);
-                tc_fence_after();
-#ifdef SCAIL_ATTN_EXPERIMENTS
-                if (p.debug == 1 || p.debug >= 5) {  // pipeline only: no TMEM reads, no math
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0)
-                        for (int g = 0; g < ATT_P_SPLIT; ++g) mbar_arrive(bar_p0 + 8u * g);
-                    l_run = 1.f;
-                    continue;
-                }
-#endif
-                softmax_tile<false>(s_tmem, o_tmem, p.scale_log2, ATT_BKV, j, m_run, l_run, bar_p0);
-                SCAIL_ATTN_TRACE(j * 8 + 6);
-            }
-            if (len % ATT_BKV) {  // partial last tile of the range: masked instantiation
-                mbar_wait(bar(B_SFULL + tile), j & 1, 32 + tile);
-                tc_fence_after();
-                softmax_tile<true>(s_tmem, o_tmem, p.scale_log2, len % ATT_BKV, j, m_run, l_run, bar_p0);
-                ++j;
-            }
-        }
-        // ---- epilogue: O / l -> bf16 -> global ----
-        mbar_wait(bar(B_OFULL + tile), 0, 40 + tile);
-        tc_fence_after();
-        const int qi = q0 + tile * ATT_BQ + sub * 32 + lane;
-        const bool row_ok = qi < p.q_len;
-        const float inv_l = 1.0f / l_run;
-        const int64_t grow = static_cast<int64_t>(batch) * p.q_batch_rows + qi;
-        __nv_bfloat16* orow = p.out + grow * p.ldo + head * ATT_D;
-        if (p.o32 != nullptr && row_ok) p.state[grow * p.heads + head] = make_float2(m_run, l_run);
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-            uint32_t o[32];
-            tmem_ld_32x32(o_tmem + c * 32, o);
-            tmem_ld_wait();
-            if (p.o32 != nullptr) {  // partial result over a subset of the keys: fp32, merged later (attn_merge_kernel)
-                if (row_ok) {
-                    float4* dst = reinterpret_cast<float4*>(p.o32 + grow * p.ldo32 + head * ATT_D + c * 32);
+            const int s = j % ATT_STAGES;
+            const uint32_t par = (j / ATT_STAGES) & 1;
+            const int valid = j < n_kv0 ? min(ATT_BKV, p.kv_len - j * ATT_BKV) : min(ATT_BKV, p.kv_len1 - (j - n_kv0) * ATT_BKV);
+            // ---- S = Q K^T ----
+            float sc[ATT_BKV / 2];
+            mbar_wait(bar(B_KFULL + s), par, 21);
+            const uint64_t k_desc = wgmma_desc_kmajor_sw128(k_smem + s * ATT_TILE_BYTES);
+            wgmma_fence();
 #pragma unroll
-                    for (int g = 0; g < 8; ++g)
-                        dst[g] = make_float4(__uint_as_float(o[4 * g]) * inv_l, __uint_as_float(o[4 * g + 1]) * inv_l,
-                                             __uint_as_float(o[4 * g + 2]) * inv_l, __uint_as_float(o[4 * g + 3]) * inv_l);
+            for (int k = 0; k < 8; ++k) {
+                const uint64_t off = ((k >> 2) * ATT_HALF_BYTES + (k & 3) * 32) >> 4;
+                wgmma_ss<ATT_BKV>(sc, q_desc + off, k_desc + off, k != 0);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(sc);
+            if (releaser) mbar_arrive(bar(B_KEMPTY + s));
+            // ---- online softmax (thread: rows r = sc[4c + 0/1], r + 8 = sc[4c + 2/3], columns 8c + 2 quad + 0/1) ----
+            if (valid < ATT_BKV) {
+#pragma unroll
+                for (int c = 0; c < ATT_BKV / 8; ++c) {
+                    const int col = 8 * c + 2 * quad;
+                    if (col >= valid) { sc[4 * c] = -INFINITY; sc[4 * c + 2] = -INFINITY; }
+                    if (col + 1 >= valid) { sc[4 * c + 1] = -INFINITY; sc[4 * c + 3] = -INFINITY; }
                 }
+            }
+            float alpha[2], neg_m[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int c = 0; c < ATT_BKV / 8; ++c) mx = fmaxf(mx, fmaxf(sc[4 * c + 2 * h], sc[4 * c + 2 * h + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                const float m_new = fmaxf(m_run[h], mx * p.scale_log2);
+                alpha[h] = fast_exp2(m_run[h] - m_new);  // 0 on the first tile (m_run = -inf)
+                m_run[h] = m_new;
+                l_run[h] *= alpha[h];
+                neg_m[h] = -m_new;
+            }
+#pragma unroll
+            for (int c = 0; c < ATT_D / 8; ++c) {
+                o[4 * c] *= alpha[0];
+                o[4 * c + 1] *= alpha[0];
+                o[4 * c + 2] *= alpha[1];
+                o[4 * c + 3] *= alpha[1];
+            }
+            uint32_t pa[ATT_BKV / 16][4];  // P as bf16 A fragments, one set of 4 registers per 16-key MMA step
+#pragma unroll
+            for (int c = 0; c < ATT_BKV / 8; ++c) {
+                float e[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    e[i] = fast_exp2(fmaf(sc[4 * c + i], p.scale_log2, neg_m[i >> 1]));
+                    l_run[i >> 1] += e[i];
+                }
+                pa[c >> 1][(c & 1) * 2] = pack_bf16(e[0], e[1]);
+                pa[c >> 1][(c & 1) * 2 + 1] = pack_bf16(e[2], e[3]);
+            }
+            // ---- O += P V ----
+            mbar_wait(bar(B_VFULL + s), par, 22);
+            const uint64_t v_desc = wgmma_desc_mnmajor_sw128(v_smem + s * ATT_TILE_BYTES, ATT_HALF_BYTES);
+            fence_regs(o);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < ATT_BKV / 16; ++k) wgmma_rs_tb<ATT_D>(o, pa[k], v_desc + k * (2048 >> 4));  // 16 kv rows = 2048 B
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(o);
+            if (releaser) mbar_arrive(bar(B_VEMPTY + s));
+        }
+        // ---- epilogue: O / l -> bf16 (or normalised fp32 partial + (m, l)) -> global ----
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+            l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int qi = q0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + 8 * h;
+            if (qi >= p.q_len) continue;
+            const float inv_l = 1.0f / l_run[h];
+            const int64_t grow = static_cast<int64_t>(batch) * p.q_batch_rows + qi;
+            if (p.o32 != nullptr) {  // partial result over a subset of the keys: fp32, merged later (attn_merge_kernel)
+                if (quad == 0) p.state[grow * p.heads + head] = make_float2(m_run[h], l_run[h]);
+                float* dst = p.o32 + grow * p.ldo32 + head * ATT_D + 2 * quad;
+#pragma unroll
+                for (int c = 0; c < ATT_D / 8; ++c)
+                    *reinterpret_cast<float2*>(dst + 8 * c) = make_float2(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
                 continue;
             }
-            if (row_ok) {
+            __nv_bfloat16* dst = p.out + grow * p.ldo + head * ATT_D + 2 * quad;
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    float f[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) f[k] = __uint_as_float(o[g * 8 + k]) * inv_l;
-                    uint4* dst = reinterpret_cast<uint4*>(orow + c * 32 + g * 8);
-                    if (p.accumulate) {
-                        uint4 prev = *dst;
-                        const uint32_t pw[4] = {prev.x, prev.y, prev.z, prev.w};
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            float2 t = unpack_bf16(pw[k]);
-                            f[2 * k] += t.x;
-                            f[2 * k + 1] += t.y;
-                        }
-                    }
-                    uint4 ov;
-                    ov.x = pack_bf16(f[0], f[1]);
-                    ov.y = pack_bf16(f[2], f[3]);
-                    ov.z = pack_bf16(f[4], f[5]);
-                    ov.w = pack_bf16(f[6], f[7]);
-                    *dst = ov;
+            for (int c = 0; c < ATT_D / 8; ++c) {
+                float f0 = o[4 * c + 2 * h] * inv_l, f1 = o[4 * c + 2 * h + 1] * inv_l;
+                uint32_t* d32 = reinterpret_cast<uint32_t*>(dst + 8 * c);
+                if (p.accumulate) {
+                    const float2 prev = unpack_bf16(*d32);
+                    f0 += prev.x;
+                    f1 += prev.y;
                 }
+                *d32 = pack_bf16(f0, f1);
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) {
-        tc_fence_after();
-        tmem_dealloc<1>(tmem_base, 512);
     }
 }
 

@@ -1,4 +1,4 @@
-// Implicit-GEMM causal 3-D convolution on tcgen05 for the Wan2.1 VAE decoder (sgm/models/wan_vae.py:17-36,
+// Implicit-GEMM causal 3-D convolution on wgmma for the Wan2.1 VAE decoder (sgm/models/wan_vae.py:17-36,
 // CausalConv3d; :186-220 ResidualBlock; :101-160 Resample).
 //
 // Activations are channels-last bf16 [T, H, W, C].  One M tile = an 8x16 patch of output pixels of one frame.
@@ -6,9 +6,9 @@
 // (4-D tensor map; out-of-bounds coordinates — spatial zero padding and the causal t < 0 frames — are
 // zero-filled by the hardware), which lands in shared memory exactly like a 128 x 64 K-major GEMM A tile.
 // B = weights repacked to [Cout, taps * Cin] (tap-major, channel-minor).  The rest is the GEMM pipeline of
-// gemm.cuh: 1 TMA warp, 1 MMA thread (UMMA 128 x BN x 16), double-buffered TMEM, 4 epilogue warps.
+// gemm.cuh: one TMA producer warp, two consumer warpgroups (wgmma m64 x BN x 16 each, fp32 accumulators in registers).
 #pragma once
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace scail {
 
@@ -37,7 +37,7 @@ struct ConvParams {
 
 constexpr int CONV_BM = 128, CONV_BK = 64, CONV_PH = 8, CONV_PW = 16;
 constexpr int CONV_A_BYTES = CONV_BM * CONV_BK * 2;
-constexpr int CONV_THREADS = 256;
+constexpr int CONV_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: consumers
 
 template <int BN>
 struct ConvCfg {
@@ -45,7 +45,35 @@ struct ConvCfg {
     static constexpr int STAGE_BYTES = CONV_A_BYTES + B_BYTES;
     static constexpr int STAGES = (BN <= 128) ? 6 : 4;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
+    static_assert(SMEM_BYTES <= 232448, "conv: shared memory budget");
 };
+
+// Epilogue of one channel pair (col, col + 1) of output pixel (t, h, w); the caller checks the pixel.
+__device__ __forceinline__ void conv_store_pair(const ConvParams& p, int t, int h, int w, int col, float f0, float f1) {
+    if (p.epilogue == CONV_EPI_HEAD_CLAMP) {  // fp32 planes [Cout, T, H, W], clamp(-1, 1), first 3 channels
+        float* o = static_cast<float*>(p.out);
+        const int64_t plane = static_cast<int64_t>(p.T) * p.H * p.W;
+        const int64_t pix = (static_cast<int64_t>(t) * p.H + h) * p.W + w;
+        if (col < 3 && col < p.Cout) o[col * plane + pix] = fminf(fmaxf(f0 + __bfloat162float(p.bias[col]), -1.0f), 1.0f);
+        if (col + 1 < 3 && col + 1 < p.Cout)
+            o[(col + 1) * plane + pix] = fminf(fmaxf(f1 + __bfloat162float(p.bias[col + 1]), -1.0f), 1.0f);
+        return;
+    }
+    if (col >= p.Cout) return;
+    const int fr = t * p.fmul + col / p.ocols;
+    const int64_t pix = (static_cast<int64_t>(fr) * p.H + h) * p.W + w;
+    if (p.bias) {
+        const float2 b2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
+        f0 += b2.x;
+        f1 += b2.y;
+    }
+    if (p.epilogue == CONV_EPI_BIAS_RES) {
+        const float2 r2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.residual + pix * p.ldr + col % p.ocols));
+        f0 += r2.x;
+        f1 += r2.y;
+    }
+    *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix * p.ldo + col % p.ocols) = pack_bf16(f0, f1);
+}
 
 template <int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
@@ -57,10 +85,6 @@ conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant_
     const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_h = (p.H + CONV_PH - 1) / CONV_PH, tiles_w = (p.W + CONV_PW - 1) / CONV_PW;
@@ -74,26 +98,13 @@ conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant_
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_x);
         tma_prefetch_desc(&tmap_w);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar(s), 1);
-            mbar_init(tempty_bar(s), 4);
+            mbar_init(empty_bar(s), 2);
         }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc<1>(tmem_slot, 512);
-        tmem_relinquish<1>();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     auto tile_coords = [&](int tile, int& t, int& h0, int& w0, int& n_blk) {
         n_blk = tile % num_n;
@@ -104,8 +115,9 @@ conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant_
         t = m / tiles_h;
     };
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -125,138 +137,60 @@ conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        {   // whole warp runs the warp-uniform control flow; the elected lane issues tcgen05.mma / commit
-            const bool leader = elect_one_sync();
-            constexpr uint32_t idesc = umma_idesc_bf16(CONV_BM, BN, 0, 0);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                mbar_wait(tempty_bar(acc), acc_phase ^ 1, 52);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * 256;
-                for (int kb = 0; kb < num_k; ++kb) {
-                    mbar_wait(full_bar(stage), phase, 53);
-                    tc_fence_after();
-                    const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-                    const uint64_t da = umma_desc_kmajor_sw128(sa);
-                    const uint64_t db = umma_desc_kmajor_sw128(sa + CONV_A_BYTES);
-                    if (leader) {
-#pragma unroll
-                        for (int k = 0; k < CONV_BK / 16; ++k) umma_ss<1>(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                        umma_commit(empty_bar(stage));
-                    }
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (leader) umma_commit(tfull_bar(acc));
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp >= 4) {
-        const int sub = warp & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
+    } else {
+        setmaxnreg_inc<232>();
+        const int wg = (warp >> 2) - 1;  // pixel rows [64 wg, 64 wg + 64) of the 128-pixel tile
+        const int tid = threadIdx.x & 127;
+        const bool releaser = tid == 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc[BN / 2];
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             int t, h0, w0, n_blk;
             tile_coords(tile, t, h0, w0, n_blk);
-            mbar_wait(tfull_bar(acc), acc_phase, 54);
-            tc_fence_after();
-            const int r = sub * 32 + lane;
-            const int h = h0 + r / CONV_PW, w = w0 + r % CONV_PW;
-            const bool pix_ok = h < p.H && w < p.W;
-            const uint32_t t_row = tmem_base + (static_cast<uint32_t>(sub * 32) << 16) + acc * 256;
-            constexpr int NCH = (BN + 31) / 32;
-#pragma unroll 1
-            for (int c = 0; c < NCH; ++c) {
-                const int col0 = n_blk * BN + c * 32;
-                if (col0 >= p.Cout) break;
-                uint32_t v[32];
-                if (BN % 32 == 0 || c * 32 + 32 <= BN) {
-                    tmem_ld_32x32(t_row + c * 32, v);
-                } else {  // BN = 16: only 16 accumulator columns exist
-                    uint32_t v16[16];
-                    tmem_ld_32x16(t_row + c * 32, v16);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) { v[j] = v16[j]; v[j + 16] = 0; }
-                }
-                tmem_ld_wait();
-                if (!pix_ok) continue;
-                if (p.epilogue == CONV_EPI_HEAD_CLAMP) {
-                    float* o = static_cast<float*>(p.out);
-                    const int64_t plane = static_cast<int64_t>(p.T) * p.H * p.W;
-                    const int64_t pix = (static_cast<int64_t>(t) * p.H + h) * p.W + w;
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            int prev_stage = -1;
+            for (int kb = 0; kb < num_k; ++kb) {
+                mbar_wait(full_bar(stage), phase, 53);
+                const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+                const uint64_t da = wgmma_desc_kmajor_sw128(sa + wg * (64 * 128));
+                const uint64_t db = wgmma_desc_kmajor_sw128(sa + CONV_A_BYTES);
+                fence_regs(acc);
+                wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 3; ++j) {
-                        if (col0 + j < p.Cout) {
-                            float f = __uint_as_float(v[j]) + __bfloat162float(p.bias[col0 + j]);
-                            o[(col0 + j) * plane + pix] = fminf(fmaxf(f, -1.0f), 1.0f);
-                        }
-                    }
-                    continue;
-                }
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const int col = col0 + g * 8;
-                    if (col < p.Cout) {
-                        const int fr = t * p.fmul + col / p.ocols;
-                        const int64_t pix = (static_cast<int64_t>(fr) * p.H + h) * p.W + w;
-                        __nv_bfloat16* orow = static_cast<__nv_bfloat16*>(p.out) + pix * p.ldo + col % p.ocols;
-                        float f[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[g * 8 + j]);
-                        if (p.bias) {
-                            uint4 bv = *reinterpret_cast<const uint4*>(p.bias + col);
-                            const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                float2 b2 = unpack_bf16(bw[j]);
-                                f[2 * j] += b2.x;
-                                f[2 * j + 1] += b2.y;
-                            }
-                        }
-                        if (p.epilogue == CONV_EPI_BIAS_RES) {
-                            uint4 rv = *reinterpret_cast<const uint4*>(p.residual + pix * p.ldr + col % p.ocols);
-                            const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                float2 r2 = unpack_bf16(rw[j]);
-                                f[2 * j] += r2.x;
-                                f[2 * j + 1] += r2.y;
-                            }
-                        }
-                        uint4 ov;
-                        ov.x = pack_bf16(f[0], f[1]);
-                        ov.y = pack_bf16(f[2], f[3]);
-                        ov.z = pack_bf16(f[4], f[5]);
-                        ov.w = pack_bf16(f[6], f[7]);
-                        *reinterpret_cast<uint4*>(orow) = ov;
-                    }
-                }
+                for (int k = 0; k < CONV_BK / 16; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, 1);
+                wgmma_commit();
+                wgmma_wait<1>();
+                fence_regs(acc);
+                if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
+                prev_stage = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
+            const int colb = n_blk * BN + 2 * (tid & 3);
+#pragma unroll
+            for (int h8 = 0; h8 < 2; ++h8) {
+                const int r = wg * 64 + (tid >> 5) * 16 + ((tid & 31) >> 2) + 8 * h8;
+                const int h = h0 + r / CONV_PW, w = w0 + r % CONV_PW;
+                if (h >= p.H || w >= p.W) continue;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) conv_store_pair(p, t, h, w, colb + 8 * j, acc[4 * j + 2 * h8], acc[4 * j + 2 * h8 + 1]);
+            }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<1>(tmem_base, 512);
     }
 }
 
 // ------------------------------------------------------------------ row-tile variant (3x3 spatial taps, W >= 128)
 // The generic kernel above re-fetches the input patch from L2 for each of the 27 taps and the weight slice for every
-// 128-pixel tile; with 96 output channels that is ~146 B/clk/SM of L2->SM traffic and the kernel is L2-bound.
-// Here one CTA iteration produces TWO output rows (h0, h0+1) x 128 pixels x 96 channels.  Per (dt, dh, 64-channel
-// slice) ONE TMA box [2 rows x 130 pixels x 64 ch] is staged (input rows h0+dh-1, h0+dh with a one-pixel halo on both
-// sides); the three dw taps of both output rows are row-shifted views of it: the UMMA descriptor start address is
-// simply advanced by whole 128-byte rows (measured on B200: the 128B swizzle is a function of the absolute shared
-// memory address, exactly as TMA wrote it, so no descriptor base_offset is needed), and the three weight slices
-// of the stage are shared by both rows: 70 KB feed 24 UMMAs (1152 cycles) = 62 B/clk/SM.
+// 128-pixel tile; with 96 output channels that makes it L2-bound.
+// Here one CTA iteration produces TWO output rows (h0, h0+1) x 128 pixels x 96 channels (consumer warpgroup i owns row h0+i).
+// Per (dt, dh, 64-channel slice) ONE TMA box [2 rows x 130 pixels x 64 ch] is staged (input rows h0+dh-1, h0+dh with a
+// one-pixel halo on both sides); the three dw taps of both output rows are row-shifted views of it: the wgmma descriptor
+// start address is simply advanced by whole 128-byte rows (the 128B swizzle is a function of the absolute shared memory
+// address, exactly as TMA wrote it), and the three weight slices of the stage are shared by both rows.
 constexpr int CROW_PW = 128;
 constexpr int CROW_A_ROWS = CROW_PW + 2;                                       // 130 pixels per input row
 constexpr int CROW_A_BYTES = ((2 * CROW_A_ROWS * 128 + 1023) / 1024) * 1024;   // 33280 -> 33792
@@ -267,6 +201,7 @@ struct ConvRowCfg {  // BN = 96 (residual / resample convs) or 16 (head conv 96 
     static constexpr int STAGES = BN > 16 ? 3 : 5;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
     static constexpr uint32_t TX_BYTES = 2 * CROW_A_ROWS * 128 + 3 * B_BYTES;      // bytes the TMA engine reports per stage
+    static_assert(SMEM_BYTES <= 232448, "conv row kernel: shared memory budget");
 };
 
 template <int BN>
@@ -275,16 +210,11 @@ conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     using Cfg = ConvRowCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int CROW_STAGE_BYTES = Cfg::STAGE_BYTES, CROW_B_BYTES = Cfg::B_BYTES;
-    constexpr uint32_t CROW_TX_BYTES = Cfg::TX_BYTES;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t bar_base = smem_base + STAGES * CROW_STAGE_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_h = (p.H + 1) / 2, tiles_w = (p.W + CROW_PW - 1) / CROW_PW;
@@ -297,26 +227,13 @@ conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_x);
         tma_prefetch_desc(&tmap_w);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar(s), 1);
-            mbar_init(tempty_bar(s), 4);
+            mbar_init(empty_bar(s), 2);
         }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc<1>(tmem_slot, 512);
-        tmem_relinquish<1>();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     auto tile_coords = [&](int tile, int& t, int& h0, int& w0, int& n_blk) {
         n_blk = tile % num_n;
@@ -327,8 +244,9 @@ conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         t = m / tiles_h;
     };
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -339,7 +257,7 @@ conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                         for (int kc = 0; kc < kc_per_tap; ++kc) {
                             mbar_wait(empty_bar(stage), phase ^ 1, 61);
                             const uint32_t sa = smem_base + stage * CROW_STAGE_BYTES;
-                            mbar_expect_tx(full_bar(stage), CROW_TX_BYTES);
+                            mbar_expect_tx(full_bar(stage), Cfg::TX_BYTES);
                             tma_load_4d(sa, &tmap_x, full_bar(stage), kc * CONV_BK, w0 - 1, h0 + dh - 1, t + dt + p.toff);
                             const int tap0 = (dt * 3 + dh) * 3;
 #pragma unroll
@@ -350,206 +268,107 @@ conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                         }
             }
         }
-    } else if (warp == 1) {
-        const bool leader = elect_one_sync();
-        constexpr uint32_t idesc = umma_idesc_bf16(CONV_BM, BN, 0, 0);
-        int stage = 0, acc = 0;
-        uint32_t phase = 0, acc_phase = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            mbar_wait(tempty_bar(acc), acc_phase ^ 1, 62);
-            tc_fence_after();
-            for (int kb = 0; kb < num_k; ++kb) {
-                mbar_wait(full_bar(stage), phase, 63);
-                tc_fence_after();
-                const uint32_t sa = smem_base + stage * CROW_STAGE_BYTES;
-                if (leader) {
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {       // output row h0 + i reads input row slot i of the box
-                        const uint32_t d_tmem = tmem_base + acc * 256 + i * 128;
-#pragma unroll
-                        for (int dw = 0; dw < 3; ++dw) {
-                            const uint64_t da = umma_desc_kmajor_sw128(sa + (i * CROW_A_ROWS + dw) * 128);
-                            const uint64_t db = umma_desc_kmajor_sw128(sa + CROW_A_BYTES + dw * CROW_B_BYTES);
-#pragma unroll
-                            for (int k = 0; k < CONV_BK / 16; ++k)
-                                umma_ss<1>(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | dw | k) != 0);
-                        }
-                    }
-                    umma_commit(empty_bar(stage));
-                }
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-            if (leader) umma_commit(tfull_bar(acc));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-    } else if (warp >= 4) {
-        const int sub = warp & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
+    } else {
+        setmaxnreg_inc<232>();
+        const int i = (warp >> 2) - 1;  // output row h0 + i reads input row slot i of the box
+        const int tid = threadIdx.x & 127;
+        const bool releaser = tid == 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc[2][BN / 2];  // pixels [0, 64) and [64, 128) of the row
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             int t, h0, w0, n_blk;
             tile_coords(tile, t, h0, w0, n_blk);
-            mbar_wait(tfull_bar(acc), acc_phase, 64);
-            tc_fence_after();
-            const int w = w0 + sub * 32 + lane;
-#pragma unroll 1
-            for (int i = 0; i < 2; ++i) {
-                const int h = h0 + i;
-                const bool pix_ok = h < p.H && w < p.W;
-                const uint32_t t_row = tmem_base + (static_cast<uint32_t>(sub * 32) << 16) + acc * 256 + i * 128;
-                const int64_t pix = (static_cast<int64_t>(t) * p.H + h) * p.W + w;
-                if constexpr (BN == 96) {
-                    if (p.norm_gamma != nullptr) {
-                        // Fused RMS_norm + SiLU of the NEXT conv's input: this thread holds all 96 channels of its pixel.
-                        uint32_t v[3][32];
 #pragma unroll
-                        for (int c = 0; c < 3; ++c) tmem_ld_32x32(t_row + c * 32, v[c]);
-                        tmem_ld_wait();
-                        if (!pix_ok) continue;
-                        float ss = 0.f;
+            for (int half = 0; half < 2; ++half)
 #pragma unroll
-                        for (int c = 0; c < 3; ++c) {
+                for (int k = 0; k < BN / 2; ++k) acc[half][k] = 0.f;
+            int prev_stage = -1;
+            for (int kb = 0; kb < num_k; ++kb) {
+                mbar_wait(full_bar(stage), phase, 63);
+                const uint32_t sa = smem_base + stage * CROW_STAGE_BYTES;
+                fence_regs(acc[0]);
+                fence_regs(acc[1]);
+                wgmma_fence();
 #pragma unroll
-                            for (int g = 0; g < 4; ++g) {
-                                const int col = c * 32 + g * 8;
-                                float f[8];
+                for (int dw = 0; dw < 3; ++dw) {
+                    const uint64_t db = wgmma_desc_kmajor_sw128(sa + CROW_A_BYTES + dw * CROW_B_BYTES);
 #pragma unroll
-                                for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[c][g * 8 + j]);
-                                if (p.bias) {
-                                    uint4 bv = *reinterpret_cast<const uint4*>(p.bias + col);
-                                    const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
+                    for (int half = 0; half < 2; ++half) {
+                        const uint64_t da = wgmma_desc_kmajor_sw128(sa + (i * CROW_A_ROWS + dw + 64 * half) * 128);
 #pragma unroll
-                                    for (int j = 0; j < 4; ++j) {
-                                        float2 b2 = unpack_bf16(bw[j]);
-                                        f[2 * j] += b2.x;
-                                        f[2 * j + 1] += b2.y;
-                                    }
-                                }
-                                if (p.epilogue == CONV_EPI_BIAS_RES) {
-                                    uint4 rv = *reinterpret_cast<const uint4*>(p.residual + pix * p.ldr + col);
-                                    const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) {
-                                        float2 r2 = unpack_bf16(rw[j]);
-                                        f[2 * j] += r2.x;
-                                        f[2 * j + 1] += r2.y;
-                                    }
-                                }
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) {
-                                    ss += f[j] * f[j];
-                                    v[c][g * 8 + j] = __float_as_uint(f[j]);
-                                }
-                                if (p.out) {
-                                    uint4 ov;
-                                    ov.x = pack_bf16(f[0], f[1]);
-                                    ov.y = pack_bf16(f[2], f[3]);
-                                    ov.z = pack_bf16(f[4], f[5]);
-                                    ov.w = pack_bf16(f[6], f[7]);
-                                    *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out) + pix * p.ldo + col) = ov;
-                                }
-                            }
-                        }
-                        const float inv = 9.797958971132712f / fmaxf(sqrtf(ss), 1e-12f);  // sqrt(96) / max(||x||, eps)
-#pragma unroll
-                        for (int c = 0; c < 3; ++c) {
-#pragma unroll
-                            for (int g = 0; g < 4; ++g) {
-                                const int col = c * 32 + g * 8;
-                                uint4 gv = *reinterpret_cast<const uint4*>(p.norm_gamma + col);
-                                const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w};
-                                uint32_t r[4];
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    float2 g2 = unpack_bf16(gw[j]);
-                                    float a = __uint_as_float(v[c][g * 8 + 2 * j]) * inv * g2.x;
-                                    float b = __uint_as_float(v[c][g * 8 + 2 * j + 1]) * inv * g2.y;
-                                    a = a / (1.0f + __expf(-a));
-                                    b = b / (1.0f + __expf(-b));
-                                    r[j] = pack_bf16(a, b);
-                                }
-                                *reinterpret_cast<uint4*>(p.out2 + pix * 96 + col) = make_uint4(r[0], r[1], r[2], r[3]);
-                            }
-                        }
-                        continue;
+                        for (int k = 0; k < CONV_BK / 16; ++k) wgmma_ss<BN>(acc[half], da + 2 * k, db + 2 * k, 1);
                     }
                 }
-#pragma unroll 1
-                for (int c = 0; c < (BN + 31) / 32; ++c) {
-                    const int col0 = n_blk * BN + c * 32;
-                    if (col0 >= p.Cout) break;
-                    uint32_t v[32];
-                    if constexpr (BN % 32 == 0) {
-                        tmem_ld_32x32(t_row + c * 32, v);
-                    } else {  // BN = 16
-                        uint32_t v16[16];
-                        tmem_ld_32x16(t_row + c * 32, v16);
+                wgmma_commit();
+                wgmma_wait<1>();
+                fence_regs(acc[0]);
+                fence_regs(acc[1]);
+                if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
+                prev_stage = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_regs(acc[0]);
+            fence_regs(acc[1]);
+            if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
+            const int h = h0 + i;
+            const int quad = tid & 3;
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) { v[j] = v16[j]; v[j + 16] = 0; }
+            for (int half = 0; half < 2; ++half) {
+#pragma unroll
+                for (int h8 = 0; h8 < 2; ++h8) {
+                    const int w = w0 + half * 64 + (tid >> 5) * 16 + ((tid & 31) >> 2) + 8 * h8;
+                    const bool pix_ok = h < p.H && w < p.W;
+                    if constexpr (BN == 96) {
+                        if (p.norm_gamma != nullptr) {
+                            // Fused RMS_norm + SiLU of the NEXT conv's input: the quad of lanes holds all 96 channels of the pixel.
+                            const int64_t pix = (static_cast<int64_t>(t) * p.H + h) * p.W + w;
+                            float v[BN / 4];
+                            float ss = 0.f;
+#pragma unroll
+                            for (int j = 0; j < BN / 8; ++j) {
+                                const int col = 8 * j + 2 * quad;
+                                float f0 = acc[half][4 * j + 2 * h8], f1 = acc[half][4 * j + 2 * h8 + 1];
+                                if (p.bias) {
+                                    const float2 b2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
+                                    f0 += b2.x;
+                                    f1 += b2.y;
+                                }
+                                if (p.epilogue == CONV_EPI_BIAS_RES && pix_ok) {
+                                    const float2 r2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.residual + pix * p.ldr + col));
+                                    f0 += r2.x;
+                                    f1 += r2.y;
+                                }
+                                v[2 * j] = f0;
+                                v[2 * j + 1] = f1;
+                                ss += f0 * f0 + f1 * f1;
+                                if (p.out && pix_ok)
+                                    *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix * p.ldo + col) = pack_bf16(f0, f1);
+                            }
+                            ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+                            ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+                            if (!pix_ok) continue;
+                            const float inv = 9.797958971132712f / fmaxf(sqrtf(ss), 1e-12f);  // sqrt(96) / max(||x||, eps)
+#pragma unroll
+                            for (int j = 0; j < BN / 8; ++j) {
+                                const int col = 8 * j + 2 * quad;
+                                const float2 g2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.norm_gamma + col));
+                                float a = v[2 * j] * inv * g2.x, b = v[2 * j + 1] * inv * g2.y;
+                                a = a / (1.0f + __expf(-a));
+                                b = b / (1.0f + __expf(-b));
+                                *reinterpret_cast<uint32_t*>(p.out2 + pix * 96 + col) = pack_bf16(a, b);
+                            }
+                            continue;
+                        }
                     }
-                    tmem_ld_wait();
                     if (!pix_ok) continue;
-                    if (p.epilogue == CONV_EPI_HEAD_CLAMP) {  // fp32 planes [Cout, T, H, W], clamp(-1, 1)
-                        float* o = static_cast<float*>(p.out);
-                        const int64_t plane = static_cast<int64_t>(p.T) * p.H * p.W;
 #pragma unroll
-                        for (int j = 0; j < 3; ++j) {
-                            if (col0 + j < p.Cout) {
-                                const float f = __uint_as_float(v[j]) + __bfloat162float(p.bias[col0 + j]);
-                                o[(col0 + j) * plane + pix] = fminf(fmaxf(f, -1.0f), 1.0f);
-                            }
-                        }
-                        continue;
-                    }
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int col = col0 + g * 8;
-                        if (col < p.Cout) {
-                            float f[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[g * 8 + j]);
-                            if (p.bias) {
-                                uint4 bv = *reinterpret_cast<const uint4*>(p.bias + col);
-                                const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    float2 b2 = unpack_bf16(bw[j]);
-                                    f[2 * j] += b2.x;
-                                    f[2 * j + 1] += b2.y;
-                                }
-                            }
-                            if (p.epilogue == CONV_EPI_BIAS_RES) {
-                                uint4 rv = *reinterpret_cast<const uint4*>(p.residual + pix * p.ldr + col);
-                                const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    float2 r2 = unpack_bf16(rw[j]);
-                                    f[2 * j] += r2.x;
-                                    f[2 * j + 1] += r2.y;
-                                }
-                            }
-                            uint4 ov;
-                            ov.x = pack_bf16(f[0], f[1]);
-                            ov.y = pack_bf16(f[2], f[3]);
-                            ov.z = pack_bf16(f[4], f[5]);
-                            ov.w = pack_bf16(f[6], f[7]);
-                            *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out) + pix * p.ldo + col) = ov;
-                        }
-                    }
+                    for (int j = 0; j < BN / 8; ++j)
+                        conv_store_pair(p, t, h, w, n_blk * BN + 8 * j + 2 * quad, acc[half][4 * j + 2 * h8], acc[half][4 * j + 2 * h8 + 1]);
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<1>(tmem_base, 512);
     }
 }
 

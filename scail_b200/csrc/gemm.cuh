@@ -1,17 +1,13 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:  C[M,N] = epi(A[M,K] * W[N,K]^T)
-//   * TMA (SWIZZLE_128B) stages A/W tiles into a 4-deep shared-memory ring,
-//   * one elected thread issues tcgen05.mma (UMMA 128x256x16, fp32 accumulators in TMEM),
-//   * TMEM accumulators are double-buffered (2 x 256 columns) so the epilogue of tile i
-//     overlaps the main loop of tile i+1,
-//   * 4 epilogue warps read TMEM (tcgen05.ld 32x32b: thread = row), apply bias / activation / gate in registers, then
-//     transpose 32x32 fp32 chunks through a swizzled shared-memory staging tile so that the residual read and the bf16
-//     store are row-contiguous (8 rows x 64 B per warp instruction instead of 32 rows x 16 B: every 32-byte sector is
-//     touched once and completely; the per-thread-row accesses of round 1 made the out-projection epilogue as long as its
-//     mainloop).
+// Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = epi(A[M,K] * W[N,K]^T)
+//   * one producer warp streams A/W tiles with TMA (SWIZZLE_128B) into a 4-deep shared-memory ring,
+//   * two consumer warpgroups each own 64 rows of the 128 x 256 tile: wgmma m64n256k16 with fp32 accumulators in registers,
+//     one wgmma group kept in flight so that a ring stage is released as soon as the MMAs that read it have retired,
+//   * the epilogue (bias / activation / gate / residual, one bf16 rounding) runs on the accumulator registers while the
+//     producer already fills the ring with the next tile's operands.
 // Replaces the reference's F.linear calls (sat/mpu/layers.py:230-243, :425-444) together with
 // the elementwise ops that follow them (bias, GELU-tanh, gate*out + residual).
 #pragma once
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace scail {
 
@@ -35,7 +31,6 @@ struct GemmParams {
     int rows_per_batch;
     int epilogue;
     int group_m;  // rasterisation: m-blocks per L2 group
-    int l2_hints; // CTA-pair kernel: 0 = none, 1 = A evict_last, 2 = A evict_last + W evict_first
 };
 
 constexpr int GEMM_BM = 128;
@@ -45,9 +40,9 @@ constexpr int GEMM_STAGES = 4;
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;  // 16 KB
 constexpr int GEMM_B_BYTES = GEMM_BN * GEMM_BK * 2;  // 32 KB
 constexpr int GEMM_STAGE_BYTES = GEMM_A_BYTES + GEMM_B_BYTES;
-constexpr int GEMM_EPI_STAGE_BYTES = 32 * 32 * 4;  // one 32x32 fp32 chunk per epilogue warp
-constexpr int GEMM_SMEM_BYTES = GEMM_STAGES * GEMM_STAGE_BYTES + 4 * GEMM_EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-constexpr int GEMM_THREADS = 256;
+constexpr int GEMM_SMEM_BYTES = GEMM_STAGES * GEMM_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int GEMM_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: consumers
+static_assert(GEMM_SMEM_BYTES <= 232448, "gemm: shared memory budget");
 
 __device__ __forceinline__ void gemm_tile_coords(int tile, int num_m, int num_n, int group_m, int& m_blk, int& n_blk) {
     int per_group = group_m * num_n;
@@ -66,101 +61,31 @@ __device__ __forceinline__ float epi_act(float v, int epilogue) {
     return v;
 }
 
-// Epilogue of one 128 x 256 accumulator tile for one epilogue warp (`sub` = TMEM sub-partition = rows [32 sub, 32 sub + 32)):
-// m0 = first global row of the tile, t_acc = TMEM address of the accumulator (lane 0, first column).
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, int m0, int n_blk, uint32_t t_acc, uint32_t epi_base,
-                                                   int sub, int lane) {
-    const int row = m0 + sub * 32 + lane;  // phase 1: this thread's accumulator row
-    const int bidx = row < p.M ? row / p.rows_per_batch : 0;
-    const uint32_t t_row = t_acc + (static_cast<uint32_t>(sub * 32) << 16);
-    const uint32_t stage = epi_base + sub * GEMM_EPI_STAGE_BYTES;
-    // phase 2 mapping: 4 lanes per row (8 columns each), 8 rows per instruction
-    const int r2 = lane >> 2, cg = lane & 3;
-#pragma unroll 1
-    for (int c = 0; c < GEMM_BN / 32; ++c) {
-        const int col0 = n_blk * GEMM_BN + c * 32;
-        if (col0 >= p.N) break;  // warp-uniform
-        uint32_t v[32];
-        tmem_ld_32x32(t_row + c * 32, v);
-        tmem_ld_wait();
-        // ---- phase 1 (thread = row): bias, activation, gate in fp32; park the chunk in the staging tile ----
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {  // groups of 8 columns
-            const int col = col0 + g * 8;
-            float f[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[g * 8 + j]);
-            if (col < p.N) {
-                if (p.bias) {
-                    uint4 bv = *reinterpret_cast<const uint4*>(p.bias + col);  // warp-uniform address: broadcast
-                    const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float2 b2 = unpack_bf16(bw[j]);
-                        f[2 * j] += b2.x;
-                        f[2 * j + 1] += b2.y;
-                    }
-                }
-                if (p.epilogue == EPI_BIAS_GELU || p.epilogue == EPI_BIAS_SILU || p.epilogue == EPI_BIAS_GELU_ERF) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) f[j] = epi_act(f[j], p.epilogue);
-                }
-                if (p.epilogue == EPI_BIAS_GATE_RES) {
-                    uint4 gv = *reinterpret_cast<const uint4*>(p.gate + bidx * p.gate_stride + col);
-                    const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w};
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float2 g2 = unpack_bf16(gw[j]);
-                        f[2 * j] *= g2.x;
-                        f[2 * j + 1] *= g2.y;
-                    }
-                }
-            }
-            // row `lane` = 128 B = 8 chunks of 16 B; chunk q lives at position q ^ (lane & 7): conflict-free both ways
-            const uint32_t a0 = stage + lane * 128 + (((2 * g) ^ (lane & 7)) << 4);
-            const uint32_t a1 = stage + lane * 128 + (((2 * g + 1) ^ (lane & 7)) << 4);
-            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a0), "f"(f[0]), "f"(f[1]), "f"(f[2]), "f"(f[3]) : "memory");
-            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a1), "f"(f[4]), "f"(f[5]), "f"(f[6]), "f"(f[7]) : "memory");
-        }
-        __syncwarp();
-        // ---- phase 2 (4 lanes per row): residual add, one bf16 rounding, row-contiguous stores ----
-        const int col = col0 + cg * 8;
-#pragma unroll
-        for (int it = 0; it < 4; ++it) {
-            const int rr = it * 8 + r2;
-            const int grow = m0 + sub * 32 + rr;
-            float f[8];
-            const uint32_t a0 = stage + rr * 128 + (((2 * cg) ^ (rr & 7)) << 4);
-            const uint32_t a1 = stage + rr * 128 + (((2 * cg + 1) ^ (rr & 7)) << 4);
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]) : "r"(a0) : "memory");
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7]) : "r"(a1) : "memory");
-            if (grow < p.M && col < p.N) {
-                if (p.epilogue == EPI_BIAS_GATE_RES || p.epilogue == EPI_BIAS_RES) {
-                    uint4 rv = *reinterpret_cast<const uint4*>(p.residual + static_cast<int64_t>(grow) * p.ldr + col);
-                    const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float2 r2f = unpack_bf16(rw[j]);
-                        f[2 * j] += r2f.x;
-                        f[2 * j + 1] += r2f.y;
-                    }
-                }
-                if (p.C32) {
-                    float4* o = reinterpret_cast<float4*>(p.C32 + static_cast<int64_t>(grow) * p.ldc + col);
-                    o[0] = make_float4(f[0], f[1], f[2], f[3]);
-                    o[1] = make_float4(f[4], f[5], f[6], f[7]);
-                } else {
-                    uint4 o;
-                    o.x = pack_bf16(f[0], f[1]);
-                    o.y = pack_bf16(f[2], f[3]);
-                    o.z = pack_bf16(f[4], f[5]);
-                    o.w = pack_bf16(f[6], f[7]);
-                    *reinterpret_cast<uint4*>(p.C + static_cast<int64_t>(grow) * p.ldc + col) = o;
-                }
-            }
-        }
-        __syncwarp();  // the staging tile is rewritten by the next chunk
+// Epilogue of one column pair (col, col + 1) of one row: bias, activation, gate, residual in fp32, one rounding.
+__device__ __forceinline__ void gemm_epilogue_pair(const GemmParams& p, int row, int col, float f0, float f1) {
+    if (row >= p.M || col >= p.N) return;
+    if (p.bias) {
+        const float2 b2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
+        f0 += b2.x;
+        f1 += b2.y;
     }
+    if (p.epilogue == EPI_BIAS_GELU || p.epilogue == EPI_BIAS_SILU || p.epilogue == EPI_BIAS_GELU_ERF) {
+        f0 = epi_act(f0, p.epilogue);
+        f1 = epi_act(f1, p.epilogue);
+    }
+    if (p.epilogue == EPI_BIAS_GATE_RES) {
+        const int bidx = row / p.rows_per_batch;
+        const float2 g2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.gate + bidx * p.gate_stride + col));
+        f0 *= g2.x;
+        f1 *= g2.y;
+    }
+    if (p.epilogue == EPI_BIAS_GATE_RES || p.epilogue == EPI_BIAS_RES) {
+        const float2 r2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.residual + static_cast<int64_t>(row) * p.ldr + col));
+        f0 += r2.x;
+        f1 += r2.y;
+    }
+    if (p.C32) *reinterpret_cast<float2*>(p.C32 + static_cast<int64_t>(row) * p.ldc + col) = make_float2(f0, f1);
+    else *reinterpret_cast<uint32_t*>(p.C + static_cast<int64_t>(row) * p.ldc + col) = pack_bf16(f0, f1);
 }
 
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -168,15 +93,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                  const GemmParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t epi_base = smem_base + GEMM_STAGES * GEMM_STAGE_BYTES;
-    const uint32_t bar_base = epi_base + 4 * GEMM_EPI_STAGE_BYTES;
-    // barrier layout (8 B each): full[S], empty[S], tmem_full[2], tmem_empty[2], then tmem ptr slot
+    const uint32_t bar_base = smem_base + GEMM_STAGES * GEMM_STAGE_BYTES;
+    // barrier layout (8 B each): full[S], empty[S]
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (GEMM_STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * GEMM_STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * GEMM_STAGES + 2 + s); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * GEMM_STAGES + 4);
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -188,30 +108,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_w);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < GEMM_STAGES; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar(s), 1);
-            mbar_init(tempty_bar(s), 4);  // one arrive per epilogue warp
+            mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
         }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc<1>(tmem_slot, 512);
-        tmem_relinquish<1>();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -227,247 +135,49 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // whole warp runs the (warp-uniform) control flow; the elected lane issues tcgen05.mma / commit
-        {
-            const bool leader = elect_one_sync();
-            constexpr uint32_t idesc = umma_idesc_bf16(GEMM_BM, GEMM_BN, 0, 0);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                mbar_wait(tempty_bar(acc), acc_phase ^ 1, 2);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * GEMM_BN;
-                for (int kb = 0; kb < num_k; ++kb) {
-                    mbar_wait(full_bar(stage), phase, 3);
-                    tc_fence_after();
-                    const uint32_t sa = smem_base + stage * GEMM_STAGE_BYTES;
-                    const uint64_t da = umma_desc_kmajor_sw128(sa);
-                    const uint64_t db = umma_desc_kmajor_sw128(sa + GEMM_A_BYTES);
-                    if (leader) {
-#pragma unroll
-                        for (int k = 0; k < GEMM_BK / 16; ++k) {
-                            // +32 B per K=16 step inside the 128-B swizzle atom (descriptor units of 16 B)
-                            umma_ss<1>(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                        }
-                        umma_commit(empty_bar(stage));  // frees the smem stage when these MMAs have read it
-                    }
-                    if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (leader) umma_commit(tfull_bar(acc));  // accumulator complete -> epilogue
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue warps =====================
-        const int sub = warp & 3;  // TMEM sub-partition this warp may access: lanes [32*sub, 32*sub+32)
-        int acc = 0;
-        uint32_t acc_phase = 0;
+    } else {
+        // ===================== consumer warpgroups =====================
+        setmaxnreg_inc<232>();
+        const int wg = (warp >> 2) - 1;  // 0 or 1: rows [64 wg, 64 wg + 64) of the tile
+        const int t = threadIdx.x & 127;
+        const bool releaser = t == 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc[GEMM_BN / 2];
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             int m_blk, n_blk;
             gemm_tile_coords(tile, num_m, num_n, p.group_m, m_blk, n_blk);
-            mbar_wait(tfull_bar(acc), acc_phase, 4);
-            tc_fence_after();
-            gemm_epilogue_tile(p, m_blk * GEMM_BM, n_blk, tmem_base + acc * GEMM_BN, epi_base, sub, lane);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<1>(tmem_base, 512);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): two CTAs of a cluster (the two SMs of a TPC) compute one 256 x 256 tile.
-// Each CTA stages ITS 128 rows of A and ITS 128-row half of the W tile (32 KB per k-block instead of 48 KB: the other half
-// of B is read by the pair's UMMA from the peer's shared memory), so L2->SM fill traffic and shared-memory operand reads
-// drop by a third per FLOP -- the 1-CTA kernel already keeps the tensor pipe >93 % busy and is limited by the 1 kW power
-// cap (SM clock ~1.3-1.4 GHz under GEMM load), so fewer bytes moved per FLOP is what buys clock.
-//   * TMA loads of both CTAs complete on the LEADER's (cluster rank 0) full barrier (`.cta_group::2` TMA form; the leader
-//     alone posts expect_tx for the 64 KB of the pair),
-//   * the leader's MMA warp issues tcgen05.mma.cta_group::2 (M = 256: accumulator rows 0-127 in the leader's TMEM, 128-255
-//     in the peer's) and releases the smem stage / publishes the accumulator with MULTICAST commits to both CTAs,
-//   * each CTA's epilogue warps drain their own TMEM half and arrive on the leader's tmem-empty barrier (8 arrivals).
-constexpr int GEMM2_STAGES = 6;
-constexpr int GEMM2_A_BYTES = 128 * GEMM_BK * 2;  // this CTA's 128 rows of A
-constexpr int GEMM2_B_BYTES = 128 * GEMM_BK * 2;  // this CTA's half (128 of 256 rows) of the W tile
-constexpr int GEMM2_STAGE_BYTES = GEMM2_A_BYTES + GEMM2_B_BYTES;
-constexpr int GEMM2_SMEM_BYTES = GEMM2_STAGES * GEMM2_STAGE_BYTES + 4 * GEMM_EPI_STAGE_BYTES + 1024 + 256;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-// shared::cluster address of `local_addr` (a shared::cta address of this CTA) in the CTA with rank `cta_rank`
-__device__ __forceinline__ uint32_t cluster_map_addr(uint32_t local_addr, uint32_t cta_rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta_rank));
-    return r;
-}
-// 2-CTA TMA load: data lands in THIS CTA's shared memory, the bytes are signalled on `cluster_bar` (a shared::cluster address:
-// the leader CTA's full barrier)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* m, uint32_t cluster_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(cluster_bar), "r"(c0), "r"(c1) : "memory");
-}
-// same with an L2 eviction-priority hint (createpolicy encodings: evict_last keeps the operand block that is re-read by the
-// following waves resident while the other operand streams through L2)
-constexpr uint64_t TMA_L2_EVICT_NORMAL = 0x1000000000000000ull;
-constexpr uint64_t TMA_L2_EVICT_FIRST = 0x12F0000000000000ull;
-constexpr uint64_t TMA_L2_EVICT_LAST = 0x14F0000000000000ull;
-__device__ __forceinline__ void tma_load_2d_pair_hint(uint32_t dst, const CUtensorMap* m, uint32_t cluster_bar, int c0, int c1,
-                                                      uint64_t hint) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(cluster_bar), "r"(c0), "r"(c1), "l"(hint) : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_cg2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w, const GemmParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t epi_base = smem_base + GEMM2_STAGES * GEMM2_STAGE_BYTES;
-    const uint32_t bar_base = epi_base + 4 * GEMM_EPI_STAGE_BYTES;
-    auto full_bar = [&](int s) { return bar_base + 8u * s; };
-    auto empty_bar = [&](int s) { return bar_base + 8u * (GEMM2_STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * GEMM2_STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * GEMM2_STAGES + 2 + s); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * GEMM2_STAGES + 4);
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();  // 0 = leader
-    const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-    const int num_mp = (p.M + 2 * GEMM_BM - 1) / (2 * GEMM_BM);  // 256-row tile pairs
-    const int num_n = (p.N + GEMM_BN - 1) / GEMM_BN;
-    const int num_tiles = num_mp * num_n;
-    const int num_k = (p.K + GEMM_BK - 1) / GEMM_BK;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_a);
-        tma_prefetch_desc(&tmap_w);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < GEMM2_STAGES; ++s) {
-            mbar_init(full_bar(s), 1);   // leader: its own arrive.expect_tx (bytes of both CTAs)
-            mbar_init(empty_bar(s), 1);  // one multicast commit per phase
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar(s), 1);
-            mbar_init(tempty_bar(s), 8);  // 4 epilogue warps of each CTA (leader's barrier is the one that is waited on)
-        }
-        fence_barrier_init();
-    }
-    if (warp == 2) {
-        tmem_alloc<2>(tmem_slot, 512);
-        tmem_relinquish<2>();
-    }
-    tc_fence_before();
-    cluster_sync_all();  // barriers of both CTAs are initialised before any remote complete_tx / arrive / commit
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
-
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs) =====================
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-                int mp, n_blk;
-                gemm_tile_coords(tile, num_mp, num_n, p.group_m, mp, n_blk);
-                const int m_row = (2 * mp + static_cast<int>(rank)) * GEMM_BM;
-                const int n_row = n_blk * GEMM_BN + static_cast<int>(rank) * 128;
-                for (int kb = 0; kb < num_k; ++kb) {
-                    mbar_wait(empty_bar(stage), phase ^ 1, 1);
-                    const uint32_t sa = smem_base + stage * GEMM2_STAGE_BYTES;
-                    if (rank == 0) mbar_expect_tx(full_bar(stage), 2 * GEMM2_STAGE_BYTES);
-                    const uint32_t lead_full = cluster_map_addr(full_bar(stage), 0);  // the leader's barrier collects both CTAs' bytes
-                    if (p.l2_hints) {  // A rows of this m-group are re-read by every following wave of the group; W streams
-                        tma_load_2d_pair_hint(sa, &tmap_a, lead_full, kb * GEMM_BK, m_row, TMA_L2_EVICT_LAST);
-                        tma_load_2d_pair_hint(sa + GEMM2_A_BYTES, &tmap_w, lead_full, kb * GEMM_BK, n_row,
-                                              p.l2_hints == 2 ? TMA_L2_EVICT_FIRST : TMA_L2_EVICT_NORMAL);
-                    } else {
-                        tma_load_2d_pair(sa, &tmap_a, lead_full, kb * GEMM_BK, m_row);
-                        tma_load_2d_pair(sa + GEMM2_A_BYTES, &tmap_w, lead_full, kb * GEMM_BK, n_row);
-                    }
-                    if (++stage == GEMM2_STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        if (rank == 0) {
-            const bool leader = elect_one_sync();
-            constexpr uint32_t idesc = umma_idesc_bf16(2 * GEMM_BM, GEMM_BN, 0, 0);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-                mbar_wait(tempty_bar(acc), acc_phase ^ 1, 2);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * GEMM_BN;
-                for (int kb = 0; kb < num_k; ++kb) {
-                    mbar_wait(full_bar(stage), phase, 3);
-                    tc_fence_after();
-                    const uint32_t sa = smem_base + stage * GEMM2_STAGE_BYTES;
-                    const uint64_t da = umma_desc_kmajor_sw128(sa);
-                    const uint64_t db = umma_desc_kmajor_sw128(sa + GEMM2_A_BYTES);
-                    if (leader) {
 #pragma unroll
-                        for (int k = 0; k < GEMM_BK / 16; ++k) umma_ss<2>(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                        umma_commit_cg2(empty_bar(stage), 3);  // frees this smem stage in BOTH CTAs
-                    }
-                    if (++stage == GEMM2_STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (leader) umma_commit_cg2(tfull_bar(acc), 3);  // accumulator halves complete -> both epilogues
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+            for (int i = 0; i < GEMM_BN / 2; ++i) acc[i] = 0.f;
+            int prev_stage = -1;
+            for (int kb = 0; kb < num_k; ++kb) {
+                mbar_wait(full_bar(stage), phase, 3);
+                const uint32_t sa = smem_base + stage * GEMM_STAGE_BYTES;
+                const uint64_t da = wgmma_desc_kmajor_sw128(sa + wg * (64 * 128));
+                const uint64_t db = wgmma_desc_kmajor_sw128(sa + GEMM_A_BYTES);
+                fence_regs(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<GEMM_BN>(acc, da + 2 * k, db + 2 * k, 1);
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+                fence_regs(acc);
+                if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
+                prev_stage = stage;
+                if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
+            // ---- epilogue straight from the accumulator fragments ----
+            const int row0 = m_blk * GEMM_BM + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+            const int colb = n_blk * GEMM_BN + 2 * (t & 3);
+#pragma unroll
+            for (int j = 0; j < GEMM_BN / 8; ++j) {
+                gemm_epilogue_pair(p, row0, colb + 8 * j, acc[4 * j], acc[4 * j + 1]);
+                gemm_epilogue_pair(p, row0 + 8, colb + 8 * j, acc[4 * j + 2], acc[4 * j + 3]);
             }
         }
-    } else if (warp >= 4) {
-        // ===================== epilogue warps (both CTAs, own TMEM half) =====================
-        const int sub = warp & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-            int mp, n_blk;
-            gemm_tile_coords(tile, num_mp, num_n, p.group_m, mp, n_blk);
-            mbar_wait(tfull_bar(acc), acc_phase, 4);
-            tc_fence_after();
-            gemm_epilogue_tile(p, (2 * mp + static_cast<int>(rank)) * GEMM_BM, n_blk, tmem_base + acc * GEMM_BN, epi_base, sub, lane);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (rank == 0) mbar_arrive(tempty_bar(acc));
-                else mbar_arrive_cluster(tempty_bar(acc), 0);
-            }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-    }
-
-    tc_fence_before();
-    cluster_sync_all();  // neither CTA may exit (or free TMEM) while the pair's UMMAs / remote arrives can still touch it
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<2>(tmem_base, 512);
     }
 }
 

@@ -1,7 +1,7 @@
 // HBM-bound row / elementwise kernels of the SCAIL DiT step (everything that is not a GEMM or attention).
 // One warp per row, 16-byte vectorised loads, fp32 statistics, bf16 in/out.
 #pragma once
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace scail {
 
@@ -44,15 +44,15 @@ struct LnModParams {
     float eps;
 };
 
-// bf16x2 word -> packed f32x2 (two ALU ops), and the packed math below halve the instruction count of the row kernels, which
-// are otherwise ALU-bound on bf16 unpacking before they are HBM-bound.
+// bf16x2 word -> f32x2 pair (two ALU ops: shift and mask instead of two conversions).
 __device__ __forceinline__ uint64_t bf16x2_to_f32x2(uint32_t w) {
     return pack_f32x2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
 }
 __device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    float a0, a1, b0, b1;
+    unpack_f32x2(a, a0, a1);
+    unpack_f32x2(b, b0, b1);
+    return pack_f32x2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint32_t f32x2_to_bf16x2(uint64_t v) {
     float lo, hi;

@@ -1,4 +1,4 @@
-"""Blackwell-native SCAIL DiT: drop-in replacements for the reference's SAT mixins plus a standalone
+"""Hopper-native (sm_90a) SCAIL DiT: drop-in replacements for the reference's SAT mixins plus a standalone
 `DiffusionTransformer` with the reference's constructor kwargs, forward signature and state_dict names.
 
 Reference surface mirrored here (paths relative to /root/reference):
@@ -163,7 +163,7 @@ class Conditioning:
 
 def _need_cuda(t):
     if not t.is_cuda:
-        raise RuntimeError("scail_b200 has no CPU path: tensors must live on a CUDA (sm_100a) device")
+        raise RuntimeError("scail_b200 has no CPU path: tensors must live on a CUDA (sm_90a) device")
 
 
 # ------------------------------------------------------------------------------------------------

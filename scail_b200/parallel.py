@@ -46,10 +46,9 @@ class ContextParallel:
         self._q = {}
         self._streams = {}
         # Opt-in: attend to the local K/V shard first while the all-gathers are in flight, then to the remote shards, and merge
-        # the two partials (scail_attention_partial / scail_attention_merge).  Measured on 4 B200s it LOSES (cfg2 x cp2: 1.689 vs
-        # 1.778 steps/s; cp4: 1.602 vs 1.679): two launches + fp32 partials + merge cost ~10 % of the attention time, more than
-        # the exposed part of the gather that the Q projection does not already cover; outputs are then no longer bit-identical
-        # to one GPU (cp_check_rel 1.8e-2 on the x4-amplified guided velocity).  Kept for larger CP degrees / slower links.
+        # the two partials (scail_attention_partial / scail_attention_merge).  Two launches + fp32 partials + merge add work
+        # that only pays off when the gather is exposed, and outputs are then no longer bit-identical to one GPU.  Off by
+        # default; kept for larger CP degrees / slower links.
         self.local_first = False
 
     def _init_native(self):

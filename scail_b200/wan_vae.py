@@ -1,4 +1,4 @@
-"""Blackwell-native Wan2.1 VAE decode: drop-in for the reference's `sgm.models.wan_vae.WanVAE`
+"""Hopper-native (sm_90a) Wan2.1 VAE decode: drop-in for the reference's `sgm.models.wan_vae.WanVAE`
 (sgm/models/wan_vae.py:619-666).  The module path contains "wan_vae" and the wrapper exposes `.model`
 (an nn.Module), `.decode(list)` and `.encode(list)` exactly as SATVideoDiffusionEngine._init_first_stage /
 decode_first_stage expect (diffusion_video.py:225-236, :298-309; SURVEY F11).
@@ -8,7 +8,7 @@ decoder.upsamples.N.*, decoder.head.*, conv2.*), so `load_state_dict(torch.load(
 fills it (decoder.* / conv2.* for decode, encoder.* / conv1.* for encode).
 
 Compute path (all kernels of libscail_b200.so, activations channels-last bf16 [T,H,W,C]):
-  whole-sequence causal 3x3x3 convs as tcgen05 implicit GEMMs with fused bias / residual epilogues,
+  whole-sequence causal 3x3x3 convs as wgmma implicit GEMMs with fused bias / residual epilogues,
   RMS_norm+SiLU as one pass, nearest-2x upsample as a gather, the time_conv frame interleave folded into the
   conv epilogue (incl. the reference's first-frame 'Rep' rule, wan_vae.py:105-131), per-frame mid-block
   attention (d=384) as GEMM -> row softmax -> GEMM, head conv writing clamped fp32 NCTHW directly.
@@ -242,7 +242,7 @@ class WanVAE_(nn.Module):
     def decode(self, z, scale):
         """z [1,16,T,h,w]; scale = [mean, 1/std] (tensors).  Returns fp32 [1,3,1+4(T-1),8h,8w] in [-1,1]."""
         if not z.is_cuda:
-            raise RuntimeError("scail_b200 has no CPU path: the VAE decode needs a CUDA (sm_100a) device")
+            raise RuntimeError("scail_b200 has no CPU path: the VAE decode needs a CUDA (sm_90a) device")
         assert z.shape[0] == 1 and z.shape[1] == 16
         zb = z[0].to(torch.bfloat16).contiguous()
         mean = scale[0].to(device=z.device, dtype=torch.float32).contiguous()
@@ -258,7 +258,7 @@ class WanVAE_(nn.Module):
         (mu - mean) / std (wan_vae.py:516-542).  Whole-sequence causal convolutions; see Resample.run_down for the
         first-frame rule of the temporal downsampling."""
         if not x.is_cuda:
-            raise RuntimeError("scail_b200 has no CPU path: the VAE encode needs a CUDA (sm_100a) device")
+            raise RuntimeError("scail_b200 has no CPU path: the VAE encode needs a CUDA (sm_90a) device")
         assert x.shape[0] == 1 and x.shape[1] == 3
         _, _, T, H, W = x.shape
         x8 = torch.zeros(T, H, W, 8, device=x.device, dtype=torch.bfloat16)

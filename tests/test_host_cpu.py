@@ -1,7 +1,6 @@
 """CPU tests of the host side: the C-ABI library loads and exports every declared symbol, the product path
-refuses to run without CUDA (no CPU fallback), RoPE tables are bit-identical to the oracle, parameter names match
-the reference's, and — where /root/reference is present — the mixins are accepted by the reference's own
-DiffusionTransformer through the YAML `target:` plug-in mechanism."""
+refuses to run without CUDA (no CPU fallback), RoPE tables are bit-identical to the oracle, and parameter names match
+the reference's (stored golden data)."""
 import os
 import re
 import sys
@@ -98,29 +97,6 @@ def test_bench_flop_model():
     assert bench.seq_len() == 27904
     assert abs(bench.block_flops(27904) / 1e12 - 33.144) < 0.01          # BASELINE.md table
     assert abs(bench.forward_flops(27904) / 1e12 - 1325.8) < 0.1
-
-
-@pytest.mark.skipif(not os.path.isfile("/root/reference/dit_video_crossattn_sc_xc.py"), reason="reference not mounted")
-def test_mixins_plug_into_reference_model():
-    """instantiate_from_config resolves the YAML target strings to scail_b200.dit.*; the reference's
-    DiffusionTransformer._build_modules / BaseModel.collect_hooks_ accept them and the resulting model has
-    exactly the reference's parameter names and shapes."""
-    from oracle import ref_harness as H
-    H.setup()
-    import dit_video_crossattn_sc_xc as ref
-    import importlib
-    import scail_b200.dit as ours
-    importlib.reload(ours)  # pick up sat's BaseMixin now that SAT is importable
-    stock = ref.DiffusionTransformer(**H.dit_config())
-    mine = ref.DiffusionTransformer(**H.dit_config(mixin_module="scail_b200.dit"))
-    assert isinstance(mine.mixins["adaln_layer"], ours.AdaLNMixin)
-    a = {k: tuple(v.shape) for k, v in stock.state_dict().items()}
-    b = {k: tuple(v.shape) for k, v in mine.state_dict().items()}
-    assert a == b
-    for hook in ("word_embedding_forward", "layer_forward", "final_forward", "position_embedding_forward",
-                 "attention_forward", "cross_attention_forward"):
-        assert hook in mine.hooks, hook
-    importlib.reload(ours)
 
 
 def test_bench_reference_arm_json_contract():

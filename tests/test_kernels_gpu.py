@@ -1,4 +1,4 @@
-"""GPU parity tests of the individual sm_100a kernels, called through the C ABI (scail_b200.ops ->
+"""GPU parity tests of the individual sm_90a kernels, called through the C ABI (scail_b200.ops ->
 ctypes -> libscail_b200.so) and compared with the oracle restatement (oracle/dit_oracle.py, fp32) on the
 same seeded inputs.  Tolerances: bf16 outputs -> rel-L2 vs the fp32 oracle <= 4e-3 (one bf16 ulp is
 2^-8 = 3.9e-3; SURVEY §0 F10), stated per test."""

@@ -1,7 +1,7 @@
 """GPU parity of the Wan2.1 VAE decode path through the C ABI:
  (a) against the golden vector produced by the UNMODIFIED reference (tests/golden/vae_small.pt: dim=16 variant,
      latent [1,16,3,8,8] -> [1,3,9,64,64], fp32 chunked decode with the feature cache),
- (b) single-op checks of the tcgen05 implicit-GEMM causal conv against F.conv3d in fp32.
+ (b) single-op checks of the wgmma implicit-GEMM causal conv against F.conv3d in fp32.
 Tolerance: output is in [-1,1] after clamp; rel-L2 vs the fp32 reference <= 2e-2 over ~40 bf16 layers,
 per-op rel-L2 <= 4e-3 (one bf16 rounding)."""
 import os
