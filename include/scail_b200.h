@@ -146,6 +146,28 @@ int scail_conv3d_cl(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin,
 int scail_conv3d_strided_cl(const void* x, int64_t T_in, int64_t H_in, int64_t W_in, int64_t Cin, const void* w2, int64_t Cout,
                             int KT, int KH, int KW, const void* bias, void* out, int64_t ldo, int64_t T_out, int64_t H_out,
                             int64_t W_out, int sstride, int pad_h, int pad_w, int tstride, int toff, scail_stream_t stream);
+
+/* Temporally chunked VAE runs (CausalConv3d.forward(x, cache_x), wan_vae.py:28-36): the same convolutions with a causal
+ * HISTORY, hist [T_hist, H, W, Cin] bf16 channels-last (same H, W, Cin as x; for the strided call the input extent
+ * H_in, W_in), holding the frames that precede x[0] in the conv's input stream.  A tap whose input frame
+ * ct = t*tstride + dt + toff is < 0 reads hist frame ct + T_hist; when that is still < 0 it reads zeros (so a 1-frame
+ * history means "one real frame, then zero padding").  0 <= T_hist <= KT-1; T_hist == 0 ignores hist (may be NULL) and
+ * is exactly scail_conv3d_cl / scail_conv3d_strided_cl, which forward here.  hist must be 16-byte aligned (C % 8 == 0).
+ * The taps, channel slices and their summation order do not depend on where a frame comes from, so a conv over
+ * cat(hist, x) and this call agree bit for bit on the frames of x.
+ * Head epilogue only: out_plane_stride (elements per output channel plane; 0 = T*H*W) and out_frame_offset place the
+ * T output frames at frames [out_frame_offset, out_frame_offset + T) of a larger fp32 [Cout, T_total, H, W] output
+ * (out_plane_stride = T_total*H*W); both must be 0 for the bf16 epilogues.
+ * Strided variant: the downsample3d time_conv of a later chunk is tstride 2, toff -1 with the last input frame of the
+ * previous chunk as a 1-frame history (the reference's x[:, :, -1:] cache, wan_vae.py:151-157). */
+int scail_conv3d_cl_hist(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin, const void* w2, int64_t Cout, int KT,
+                         int KH, int KW, const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo,
+                         int64_t ocols, int fmul, int epilogue, const void* norm_gamma, void* out2, const void* hist,
+                         int64_t T_hist, int64_t out_plane_stride, int64_t out_frame_offset, scail_stream_t stream);
+int scail_conv3d_strided_cl_hist(const void* x, int64_t T_in, int64_t H_in, int64_t W_in, int64_t Cin, const void* w2,
+                                 int64_t Cout, int KT, int KH, int KW, const void* bias, void* out, int64_t ldo, int64_t T_out,
+                                 int64_t H_out, int64_t W_out, int sstride, int pad_h, int pad_w, int tstride, int toff,
+                                 const void* hist, int64_t T_hist, scail_stream_t stream);
 /* RMS_norm over channels (F.normalize * sqrt(C) * gamma, wan_vae.py:39-54), optional SiLU; [npix, C] bf16 */
 int scail_rmsnorm_cl(const void* x, const void* gamma, void* out, int64_t npix, int64_t C, int silu, scail_stream_t stream);
 /* nearest-exact 2x spatial upsample (wan_vae.py:57-63): [frames,H,W,C] -> [frames,2H,2W,C] */

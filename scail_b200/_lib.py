@@ -47,6 +47,10 @@ SIGNATURES = {
                         c_i64, c_int, c_int, c_p, c_p, c_p],
     "scail_conv3d_strided_cl": [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_i64, c_int, c_int, c_int, c_p, c_p, c_i64, c_i64,
                                 c_i64, c_i64, c_int, c_int, c_int, c_int, c_int, c_p],
+    "scail_conv3d_cl_hist": [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_i64, c_int, c_int, c_int, c_p, c_p, c_i64, c_p, c_i64,
+                             c_i64, c_int, c_int, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_p],
+    "scail_conv3d_strided_cl_hist": [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_i64, c_int, c_int, c_int, c_p, c_p, c_i64, c_i64,
+                                     c_i64, c_i64, c_int, c_int, c_int, c_int, c_int, c_p, c_i64, c_p],
     "scail_rmsnorm_cl": [c_p, c_p, c_p, c_i64, c_i64, c_int, c_p],
     "scail_upsample2x_cl": [c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_vae_latent_to_cl": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_p],

@@ -202,14 +202,15 @@ int set_smem(K kernel, int bytes) {
 inline int blocks_for(int64_t n, int per) { return static_cast<int>((n + per - 1) / per); }
 
 template <int BN>
-static int launch_conv(const CUtensorMap& tx, const CUtensorMap& tw, const scail::ConvParams& p, cudaStream_t st) {
+static int launch_conv(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& th, const scail::ConvParams& p,
+                       cudaStream_t st) {
     using namespace scail;
     int rc;
     if ((rc = set_smem(conv3d_kernel<BN>, ConvCfg<BN>::SMEM_BYTES))) return rc;
     const int tiles = p.T * blocks_for(p.H, CONV_PH) * blocks_for(p.W, CONV_PW) * blocks_for(p.Cout, BN);
     const int sms = sm_count();
     if (sms <= 0) return fail(-2, "conv3d: no CUDA device");
-    conv3d_kernel<BN><<<tiles < sms ? tiles : sms, CONV_THREADS, ConvCfg<BN>::SMEM_BYTES, st>>>(tx, tw, p);
+    conv3d_kernel<BN><<<tiles < sms ? tiles : sms, CONV_THREADS, ConvCfg<BN>::SMEM_BYTES, st>>>(tx, tw, th, p);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -454,6 +455,14 @@ int scail_cast_f32_bf16(const float* x, void* out, int64_t n, scail_stream_t str
 int scail_conv3d_cl(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin, const void* w2, int64_t Cout, int KT,
                     int KH, int KW, const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo,
                     int64_t ocols, int fmul, int epilogue, const void* norm_gamma, void* out2, scail_stream_t stream) {
+    return scail_conv3d_cl_hist(x, T, H, W, Cin, w2, Cout, KT, KH, KW, bias, residual, ldr, out, ldo, ocols, fmul, epilogue,
+                                norm_gamma, out2, nullptr, 0, 0, 0, stream);
+}
+
+int scail_conv3d_cl_hist(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin, const void* w2, int64_t Cout, int KT,
+                         int KH, int KW, const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo,
+                         int64_t ocols, int fmul, int epilogue, const void* norm_gamma, void* out2, const void* hist,
+                         int64_t T_hist, int64_t out_plane_stride, int64_t out_frame_offset, scail_stream_t stream) {
     using namespace scail;
     SCAIL_REQUIRE(x && w2 && (out || (norm_gamma && out2)), "conv3d: null operand");
     SCAIL_REQUIRE((norm_gamma == nullptr) == (out2 == nullptr), "conv3d: norm_gamma and out2 come together");
@@ -466,10 +475,20 @@ int scail_conv3d_cl(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin,
     SCAIL_REQUIRE(aligned16(out) && aligned16(bias) && aligned16(residual) && aligned16(out2), "conv3d: out, bias, residual must be 16-byte aligned");
     if (epilogue == CONV_EPI_HEAD_CLAMP) SCAIL_REQUIRE(bias && Cout <= 16, "conv3d: head epilogue needs bias and Cout <= 16");
     else SCAIL_REQUIRE(Cout % 8 == 0 && ldo % 8 == 0 && ocols > 0 && ocols % 8 == 0, "conv3d: Cout, ldo, ocols must be multiples of 8");
+    SCAIL_REQUIRE(T_hist >= 0 && T_hist <= KT - 1, "conv3d: T_hist=%lld must be in [0, KT-1=%d]", (long long)T_hist, KT - 1);
+    SCAIL_REQUIRE(T_hist == 0 || (hist && aligned16(hist)), "conv3d: a history of T_hist > 0 frames needs a 16-byte aligned hist");
+    const int64_t plane = out_plane_stride > 0 ? out_plane_stride : T * H * W;
+    if (epilogue == CONV_EPI_HEAD_CLAMP)
+        SCAIL_REQUIRE(out_frame_offset >= 0 && out_plane_stride >= 0 && plane >= (out_frame_offset + T) * H * W,
+                      "conv3d: head output planes of %lld elements cannot hold frames [%lld, %lld)", (long long)plane,
+                      (long long)out_frame_offset, (long long)(out_frame_offset + T));
+    else SCAIL_REQUIRE(out_plane_stride == 0 && out_frame_offset == 0, "conv3d: out_plane_stride / out_frame_offset are head-epilogue only");
     const int taps = KT * KH * KW;
-    CUtensorMap tx, tw;
+    CUtensorMap tx, tw, th;
     int rc;
     if ((rc = make_tmap_cl4d(x, T, H, W, Cin, &tx))) return rc;
+    th = tx;  // not read when T_hist == 0
+    if (T_hist > 0 && (rc = make_tmap_cl4d(hist, T_hist, H, W, Cin, &th))) return rc;
     const int BN = Cout <= 16 ? 16 : (Cout <= 96 ? 96 : 192);
     if ((rc = make_tmap_2d(w2, Cout, (uint64_t)taps * Cin, (uint64_t)taps * Cin, BN, 64, &tw))) return rc;
     ConvParams p;
@@ -479,6 +498,11 @@ int scail_conv3d_cl(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin,
     p.epilogue = epilogue;
     p.norm_gamma = static_cast<const __nv_bfloat16*>(norm_gamma); p.out2 = static_cast<__nv_bfloat16*>(out2);
     p.sstride = 1; p.pad_h = KH / 2; p.pad_w = KW / 2; p.tstride = 1; p.toff = -(KT - 1);
+    p.T_hist = (int)T_hist;
+    if (epilogue == CONV_EPI_HEAD_CLAMP) {  // plane stride in ldo; `out` starts at frame out_frame_offset of every plane
+        p.ldo = plane;
+        p.out = static_cast<float*>(out) + out_frame_offset * H * W;
+    }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     static const bool row_ok_env = !(getenv("SCAIL_CONV_ROW") && atoi(getenv("SCAIL_CONV_ROW")) == 0);
     const bool row_head = epilogue == CONV_EPI_HEAD_CLAMP && Cout <= 16;
@@ -486,40 +510,54 @@ int scail_conv3d_cl(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin,
     if (row_ok_env && KH == 3 && KW == 3 && W >= 128 && (Cout % 96 == 0 || row_head) && fmul <= 1 && (ocols <= 0 || ocols == Cout)) {
         // row-tile kernel: 2 output rows x 128 pixels x BN channels per iteration, taps as shifted smem views
         const int RBN = row_head ? 16 : 96;
-        CUtensorMap txr, twr;
+        CUtensorMap txr, twr, thr;
         if ((rc = make_tmap_cl4d(x, T, H, W, Cin, &txr, CROW_A_ROWS, 2))) return rc;
         if ((rc = make_tmap_2d(w2, Cout, (uint64_t)taps * Cin, (uint64_t)taps * Cin, RBN, 64, &twr))) return rc;
+        thr = txr;
+        if (T_hist > 0 && (rc = make_tmap_cl4d(hist, T_hist, H, W, Cin, &thr, CROW_A_ROWS, 2))) return rc;
         const int tiles = (int)(T * ((H + 1) / 2) * blocks_for(W, CROW_PW) * blocks_for(Cout, RBN));
         const int sms = sm_count();
         SCAIL_REQUIRE(sms > 0, "conv3d: no CUDA device");
         const int grid = tiles < sms ? tiles : sms;
         if (row_head) {
             if ((rc = set_smem(conv3d_row_kernel<16>, ConvRowCfg<16>::SMEM_BYTES))) return rc;
-            conv3d_row_kernel<16><<<grid, CONV_THREADS, ConvRowCfg<16>::SMEM_BYTES, st>>>(txr, twr, p);
+            conv3d_row_kernel<16><<<grid, CONV_THREADS, ConvRowCfg<16>::SMEM_BYTES, st>>>(txr, twr, thr, p);
         } else {
             if ((rc = set_smem(conv3d_row_kernel<96>, ConvRowCfg<96>::SMEM_BYTES))) return rc;
-            conv3d_row_kernel<96><<<grid, CONV_THREADS, ConvRowCfg<96>::SMEM_BYTES, st>>>(txr, twr, p);
+            conv3d_row_kernel<96><<<grid, CONV_THREADS, ConvRowCfg<96>::SMEM_BYTES, st>>>(txr, twr, thr, p);
         }
         SCAIL_CHECK_CUDA(cudaGetLastError());
         return 0;
     }
-    if (BN == 16) return launch_conv<16>(tx, tw, p, st);
-    if (BN == 96) return launch_conv<96>(tx, tw, p, st);
-    return launch_conv<192>(tx, tw, p, st);
+    if (BN == 16) return launch_conv<16>(tx, tw, th, p, st);
+    if (BN == 96) return launch_conv<96>(tx, tw, th, p, st);
+    return launch_conv<192>(tx, tw, th, p, st);
 }
 
 int scail_conv3d_strided_cl(const void* x, int64_t T_in, int64_t H_in, int64_t W_in, int64_t Cin, const void* w2, int64_t Cout,
                             int KT, int KH, int KW, const void* bias, void* out, int64_t ldo, int64_t T_out, int64_t H_out,
                             int64_t W_out, int sstride, int pad_h, int pad_w, int tstride, int toff, scail_stream_t stream) {
+    return scail_conv3d_strided_cl_hist(x, T_in, H_in, W_in, Cin, w2, Cout, KT, KH, KW, bias, out, ldo, T_out, H_out, W_out,
+                                        sstride, pad_h, pad_w, tstride, toff, nullptr, 0, stream);
+}
+
+int scail_conv3d_strided_cl_hist(const void* x, int64_t T_in, int64_t H_in, int64_t W_in, int64_t Cin, const void* w2,
+                                 int64_t Cout, int KT, int KH, int KW, const void* bias, void* out, int64_t ldo, int64_t T_out,
+                                 int64_t H_out, int64_t W_out, int sstride, int pad_h, int pad_w, int tstride, int toff,
+                                 const void* hist, int64_t T_hist, scail_stream_t stream) {
     using namespace scail;
     SCAIL_REQUIRE(x && w2 && out, "conv3d_strided: null operand");
     SCAIL_REQUIRE(Cin % 8 == 0 && Cout % 8 == 0 && ldo % 8 == 0, "conv3d_strided: channels must be multiples of 8");
     SCAIL_REQUIRE((sstride == 1 || sstride == 2) && (tstride == 1 || tstride == 2), "conv3d_strided: strides must be 1 or 2");
     SCAIL_REQUIRE(KT >= 1 && KT <= 3 && KH >= 1 && KH <= 3 && KW >= 1 && KW <= 3, "conv3d_strided: taps must be 1..3");
+    SCAIL_REQUIRE(T_hist >= 0 && T_hist <= KT - 1, "conv3d_strided: T_hist=%lld must be in [0, KT-1=%d]", (long long)T_hist, KT - 1);
+    SCAIL_REQUIRE(T_hist == 0 || (hist && aligned16(hist)), "conv3d_strided: a history of T_hist > 0 frames needs a 16-byte aligned hist");
     const int taps = KT * KH * KW;
-    CUtensorMap tx, tw;
+    CUtensorMap tx, tw, th;
     int rc;
     if ((rc = make_tmap_cl4d(x, T_in, H_in, W_in, Cin, &tx, 16 * sstride, 8 * sstride, sstride))) return rc;
+    th = tx;  // not read when T_hist == 0
+    if (T_hist > 0 && (rc = make_tmap_cl4d(hist, T_hist, H_in, W_in, Cin, &th, 16 * sstride, 8 * sstride, sstride))) return rc;
     const int BN = Cout <= 16 ? 16 : (Cout <= 96 ? 96 : 192);
     if ((rc = make_tmap_2d(w2, Cout, (uint64_t)taps * Cin, (uint64_t)taps * Cin, BN, 64, &tw))) return rc;
     ConvParams p;
@@ -527,10 +565,11 @@ int scail_conv3d_strided_cl(const void* x, int64_t T_in, int64_t H_in, int64_t W
     p.bias = static_cast<const __nv_bfloat16*>(bias); p.residual = nullptr; p.out = out; p.ldo = ldo; p.ldr = 0;
     p.ocols = (int)Cout; p.fmul = 1; p.epilogue = CONV_EPI_BIAS; p.norm_gamma = nullptr; p.out2 = nullptr;
     p.sstride = sstride; p.pad_h = pad_h; p.pad_w = pad_w; p.tstride = tstride; p.toff = toff;
+    p.T_hist = (int)T_hist;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (BN == 16) return launch_conv<16>(tx, tw, p, st);
-    if (BN == 96) return launch_conv<96>(tx, tw, p, st);
-    return launch_conv<192>(tx, tw, p, st);
+    if (BN == 16) return launch_conv<16>(tx, tw, th, p, st);
+    if (BN == 96) return launch_conv<96>(tx, tw, th, p, st);
+    return launch_conv<192>(tx, tw, th, p, st);
 }
 
 int scail_rmsnorm_cl(const void* x, const void* gamma, void* out, int64_t npix, int64_t C, int silu, scail_stream_t stream) {

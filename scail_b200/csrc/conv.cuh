@@ -7,10 +7,22 @@
 // zero-filled by the hardware), which lands in shared memory exactly like a 128 x 64 K-major GEMM A tile.
 // B = weights repacked to [Cout, taps * Cin] (tap-major, channel-minor).  The rest is the GEMM pipeline of
 // gemm.cuh: one TMA producer warp, two consumer warpgroups (wgmma m64 x BN x 16 each, fp32 accumulators in registers).
+//
+// Chunked (temporally tiled) VAE runs pass a second activation map, the causal history [T_hist, H, W, Cin]: the last
+// frames of the previous chunk's input.  A box whose frame ct is < 0 is then fetched from the history at frame
+// ct + T_hist instead (and is zero-filled as before when that is still < 0).  Same box shape and byte count, same
+// tap / channel-slice order, so a chunk computes exactly what the whole sequence computes for its frames.
 #pragma once
 #include "sm90.cuh"
 
 namespace scail {
+
+// TMA load of one activation box at frame t: from the history map when t < 0 and there is a history, else from x.
+__device__ __forceinline__ void conv_load_act(uint32_t dst, const CUtensorMap* tmap_x, const CUtensorMap* tmap_h, int T_hist,
+                                              uint32_t bar, int c, int w, int h, int t) {
+    if (t < 0 && T_hist > 0) tma_load_4d(dst, tmap_h, bar, c, w, h, t + T_hist);
+    else tma_load_4d(dst, tmap_x, bar, c, w, h, t);
+}
 
 enum ConvEpilogue : int {
     CONV_EPI_BIAS = 0,       // out = acc + bias
@@ -24,8 +36,8 @@ struct ConvParams {
     int KT, KH, KW;       // filter taps; temporal padding is causal (KT-1 on the left), spatial is "same"
     const __nv_bfloat16* bias;      // [Cout]
     const __nv_bfloat16* residual;  // channels-last [T, H, W, ldr]
-    void* out;                      // bf16 channels-last [*, H, W, ldo]  or  fp32 [3, T, H, W] (head)
-    int64_t ldo, ldr;
+    void* out;                      // bf16 channels-last [*, H, W, ldo]  or  fp32 [3, *, H, W] (head)
+    int64_t ldo, ldr;               // head: ldo = elements per output channel plane (the host may offset `out` by frames)
     int sstride, pad_h, pad_w;  // input coordinate of tap (dh,dw) for output (h,w): (h*sstride + dh - pad_h, w*sstride + dw - pad_w)
     int tstride, toff;          // input frame of tap dt for output frame t: t*tstride + dt + toff (causal stride 1: toff = -(KT-1))
     const __nv_bfloat16* norm_gamma;  // row-tile kernel, Cout == 96 only: also emit out2 = SiLU(RMS_norm(value) * gamma)
@@ -33,7 +45,12 @@ struct ConvParams {
     int ocols;            // output column c lands in frame t*fmul + c / ocols, channel c % ocols
     int fmul;             // (time_conv of upsample3d interleaves its two channel halves as two frames)
     int epilogue;
+    int T_hist;           // frames of the causal history map: a tap at input frame ct < 0 reads history frame ct + T_hist
+                          // (still < 0: zero-filled); 0 = no history, t < 0 is zero padding (CausalConv3d cache_x, wan_vae.py:28-36)
 };
+// 128 bytes: T_hist fills the tail padding.  A larger struct measurably changes the code nvcc generates for the
+// epilogues (more parameter reloads and branches; 9 % slower VAE decode on H100), so keep new fields out of it.
+static_assert(sizeof(ConvParams) == 128, "ConvParams: keep the kernel parameter struct at 128 bytes");
 
 constexpr int CONV_BM = 128, CONV_BK = 64, CONV_PH = 8, CONV_PW = 16;
 constexpr int CONV_A_BYTES = CONV_BM * CONV_BK * 2;
@@ -50,9 +67,9 @@ struct ConvCfg {
 
 // Epilogue of one channel pair (col, col + 1) of output pixel (t, h, w); the caller checks the pixel.
 __device__ __forceinline__ void conv_store_pair(const ConvParams& p, int t, int h, int w, int col, float f0, float f1) {
-    if (p.epilogue == CONV_EPI_HEAD_CLAMP) {  // fp32 planes [Cout, T, H, W], clamp(-1, 1), first 3 channels
+    if (p.epilogue == CONV_EPI_HEAD_CLAMP) {  // fp32 planes [Cout, *, H, W], clamp(-1, 1), first 3 channels
         float* o = static_cast<float*>(p.out);
-        const int64_t plane = static_cast<int64_t>(p.T) * p.H * p.W;
+        const int64_t plane = p.ldo;
         const int64_t pix = (static_cast<int64_t>(t) * p.H + h) * p.W + w;
         if (col < 3 && col < p.Cout) o[col * plane + pix] = fminf(fmaxf(f0 + __bfloat162float(p.bias[col]), -1.0f), 1.0f);
         if (col + 1 < 3 && col + 1 < p.Cout)
@@ -77,7 +94,8 @@ __device__ __forceinline__ void conv_store_pair(const ConvParams& p, int t, int 
 
 template <int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w, const ConvParams p) {
+conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+              const __grid_constant__ CUtensorMap tmap_h, const ConvParams p) {
     using Cfg = ConvCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -98,6 +116,7 @@ conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant_
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_x);
         tma_prefetch_desc(&tmap_w);
+        if (p.T_hist > 0) tma_prefetch_desc(&tmap_h);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_bar(s), 1);
             mbar_init(empty_bar(s), 2);
@@ -130,7 +149,7 @@ conv3d_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant_
                         mbar_wait(empty_bar(stage), phase ^ 1, 51);
                         const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
                         mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-                        tma_load_4d(sa, &tmap_x, full_bar(stage), kc * CONV_BK, cw, ch, ct);
+                        conv_load_act(sa, &tmap_x, &tmap_h, p.T_hist, full_bar(stage), kc * CONV_BK, cw, ch, ct);
                         tma_load_2d(sa + CONV_A_BYTES, &tmap_w, full_bar(stage), tap * p.Cin + kc * CONV_BK, n_blk * BN);
                         if (++stage == STAGES) { stage = 0; phase ^= 1; }
                     }
@@ -206,7 +225,8 @@ struct ConvRowCfg {  // BN = 96 (residual / resample convs) or 16 (head conv 96 
 
 template <int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w, const ConvParams p) {
+conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                  const __grid_constant__ CUtensorMap tmap_h, const ConvParams p) {
     using Cfg = ConvRowCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int CROW_STAGE_BYTES = Cfg::STAGE_BYTES, CROW_B_BYTES = Cfg::B_BYTES;
@@ -227,6 +247,7 @@ conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_x);
         tma_prefetch_desc(&tmap_w);
+        if (p.T_hist > 0) tma_prefetch_desc(&tmap_h);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_bar(s), 1);
             mbar_init(empty_bar(s), 2);
@@ -258,7 +279,8 @@ conv3d_row_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                             mbar_wait(empty_bar(stage), phase ^ 1, 61);
                             const uint32_t sa = smem_base + stage * CROW_STAGE_BYTES;
                             mbar_expect_tx(full_bar(stage), Cfg::TX_BYTES);
-                            tma_load_4d(sa, &tmap_x, full_bar(stage), kc * CONV_BK, w0 - 1, h0 + dh - 1, t + dt + p.toff);
+                            conv_load_act(sa, &tmap_x, &tmap_h, p.T_hist, full_bar(stage), kc * CONV_BK, w0 - 1, h0 + dh - 1,
+                                          t + dt + p.toff);
                             const int tap0 = (dt * 3 + dh) * 3;
 #pragma unroll
                             for (int dw = 0; dw < 3; ++dw)

@@ -218,21 +218,40 @@ def conv3d_fusable(x, kh, kw, cout):
     return kh == 3 and kw == 3 and x.shape[2] >= 128 and cout == 96
 
 
+def _hist_arg(hist, x, kt):
+    """(pointer, frames) of an optional causal history [T_hist, H, W, Cin] for the conv input x (scail_conv3d_cl_hist)."""
+    if hist is None or hist.shape[0] == 0:
+        return None, 0
+    _req(hist)
+    assert hist.is_contiguous() and hist.shape[1:] == x.shape[1:] and hist.shape[0] <= kt - 1, (tuple(hist.shape), tuple(x.shape), kt)
+    return _ptr(hist), hist.shape[0]
+
+
 def conv3d_cl(x, w2, bias, kt, kh, kw, cout, out=None, residual=None, fmul=1, ocols=None, head=False, norm_gamma=None,
-              want_raw=True):
+              want_raw=True, *, hist=None, out_frame_offset=0):
     """x [T,H,W,Cin] bf16 channels-last; w2 [cout, kt*kh*kw*Cin] bf16.  Returns out [T*fmul,H,W,ocols] bf16
     (or fp32 planes [cout,T,H,W] when head=True).  With norm_gamma (see conv3d_fusable) returns (out, out2) where
-    out2 = SiLU(RMS_norm(out) * gamma) comes from the same epilogue; want_raw=False skips writing `out` (returned None)."""
+    out2 = SiLU(RMS_norm(out) * gamma) comes from the same epilogue; want_raw=False skips writing `out` (returned None).
+    hist [T_hist <= kt-1, H, W, Cin]: the input frames preceding x[0] (causal history of a chunked run) instead of zero
+    padding.  head=True with out_frame_offset: write frames [out_frame_offset, out_frame_offset + T) of a given fp32
+    out [cout, T_total, H, W]."""
     _req(x), _req(w2)
     T, H, W, Cin = x.shape
     assert x.is_contiguous() and w2.is_contiguous() and w2.shape == (cout, kt * kh * kw * Cin)
+    hp, th = _hist_arg(hist, x, kt)
     ocols = cout if ocols is None else ocols
     out2 = None
+    plane = 0
     if head:
         if out is None:
+            assert out_frame_offset == 0, "out_frame_offset needs an output tensor"
             out = torch.empty(cout, T, H, W, device=x.device, dtype=torch.float32)
-        epi, ldo = CONV_EPI_HEAD_CLAMP, 0
+        _req(out, torch.float32)
+        assert out.is_contiguous() and out.shape[0] == cout and out.shape[2:] == (H, W)
+        assert 0 <= out_frame_offset and out_frame_offset + T <= out.shape[1]
+        epi, ldo, plane = CONV_EPI_HEAD_CLAMP, 0, out.stride(0)
     else:
+        assert out_frame_offset == 0, "out_frame_offset is for the head epilogue"
         if norm_gamma is not None:
             assert conv3d_fusable(x, kh, kw, cout) and fmul == 1
             out2 = torch.empty(T, H, W, cout, device=x.device, dtype=torch.bfloat16)
@@ -240,25 +259,29 @@ def conv3d_cl(x, w2, bias, kt, kh, kw, cout, out=None, residual=None, fmul=1, oc
             out = torch.empty(T * fmul, H, W, ocols, device=x.device, dtype=torch.bfloat16)
         epi, ldo = (CONV_EPI_BIAS_RES if residual is not None else CONV_EPI_BIAS), (out.shape[-1] if out is not None else cout)
         assert out is None or out.is_contiguous()
-    _lib.check(_lib.lib().scail_conv3d_cl(_ptr(x), T, H, W, Cin, _ptr(w2), cout, kt, kh, kw, _ptr(bias), _ptr(residual),
-                                          residual.shape[-1] if residual is not None else 0, _ptr(out), ldo, ocols, fmul,
-                                          epi, _ptr(norm_gamma), _ptr(out2), _stream()), "scail_conv3d_cl")
+    _lib.check(_lib.lib().scail_conv3d_cl_hist(_ptr(x), T, H, W, Cin, _ptr(w2), cout, kt, kh, kw, _ptr(bias), _ptr(residual),
+                                               residual.shape[-1] if residual is not None else 0, _ptr(out), ldo, ocols, fmul,
+                                               epi, _ptr(norm_gamma), _ptr(out2), hp, th, plane, out_frame_offset, _stream()),
+               "scail_conv3d_cl_hist")
     _count()
     return (out, out2) if norm_gamma is not None else out
 
 
-def conv3d_strided_cl(x, w2, bias, kt, kh, kw, cout, out_shape, sstride=1, pad_h=0, pad_w=0, tstride=1, toff=0, out=None):
-    """Strided conv for the VAE encoder: x [T,H,W,Cin] -> out [T_out,H_out,W_out,cout] (see scail_conv3d_strided_cl)."""
+def conv3d_strided_cl(x, w2, bias, kt, kh, kw, cout, out_shape, sstride=1, pad_h=0, pad_w=0, tstride=1, toff=0, out=None, *,
+                      hist=None):
+    """Strided conv for the VAE encoder: x [T,H,W,Cin] -> out [T_out,H_out,W_out,cout] (see scail_conv3d_strided_cl);
+    hist [T_hist <= kt-1, H, W, Cin]: input frames preceding x[0], read for the taps at frames < 0 (scail_conv3d_strided_cl_hist)."""
     _req(x), _req(w2)
     T, H, W, Cin = x.shape
     assert x.is_contiguous() and w2.is_contiguous() and w2.shape == (cout, kt * kh * kw * Cin)
+    hp, th = _hist_arg(hist, x, kt)
     To, Ho, Wo = out_shape
     if out is None:
         out = torch.empty(To, Ho, Wo, cout, device=x.device, dtype=torch.bfloat16)
     assert out.is_contiguous() and out.shape[-1] == cout
-    _lib.check(_lib.lib().scail_conv3d_strided_cl(_ptr(x), T, H, W, Cin, _ptr(w2), cout, kt, kh, kw, _ptr(bias), _ptr(out), cout,
-                                                  To, Ho, Wo, sstride, pad_h, pad_w, tstride, toff, _stream()),
-               "scail_conv3d_strided_cl")
+    _lib.check(_lib.lib().scail_conv3d_strided_cl_hist(_ptr(x), T, H, W, Cin, _ptr(w2), cout, kt, kh, kw, _ptr(bias), _ptr(out),
+                                                       cout, To, Ho, Wo, sstride, pad_h, pad_w, tstride, toff, hp, th, _stream()),
+               "scail_conv3d_strided_cl_hist")
     _count()
     return out
 
