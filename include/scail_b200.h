@@ -40,7 +40,8 @@ enum {
 
 /* C[M,N] = epilogue(A[M,K] @ W[N,K]^T); A, W, C bf16 row-major with leading dims lda/ldw/ldc
  * (elements, multiples of 8; ldc % 4 for a float32 C).  bias [N] bf16 or NULL; gate [B, gate_stride] bf16 indexed by
- * row / rows_per_batch; residual [M, ldr] bf16.  c_fp32 != 0 writes float32 C instead.  C, bias, gate and residual must be
+ * row / rows_per_batch; residual [M, ldr] bf16.  c_fp32 != 0 writes float32 C instead (not with the
+ * residual epilogues: -1).  C, bias, gate and residual must be
  * 16-byte aligned (-1 otherwise).
  * Replaces ColumnParallelLinear.forward / RowParallelLinear.forward (sat/mpu/layers.py:230-243,
  * :425-444) and nn.Linear / nn.Conv3d-as-GEMM call sites of the DiT. */

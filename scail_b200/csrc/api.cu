@@ -63,27 +63,30 @@ struct MapKey {
     const void* ptr;
     uint64_t rows, cols, ld;
     uint32_t box_rows, box_cols;
+    bool f32;
     bool operator==(const MapKey& o) const {
         return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows &&
-               box_cols == o.box_cols;
+               box_cols == o.box_cols && f32 == o.f32;
     }
 };
 struct MapKeyHash {
     size_t operator()(const MapKey& k) const {
         size_t h = reinterpret_cast<size_t>(k.ptr);
         auto mix = [&](uint64_t v) { h ^= v + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2); };
-        mix(k.rows); mix(k.cols); mix(k.ld); mix(k.box_rows); mix(k.box_cols);
+        mix(k.rows); mix(k.cols); mix(k.ld); mix(k.box_rows); mix(k.box_cols); mix(k.f32);
         return h;
     }
 };
 std::mutex g_map_mu;
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 
-// 2-D bf16 row-major [rows, cols] with leading dimension ld (elements); box = [box_rows, box_cols],
-// box_cols * 2 bytes == 128 (SWIZZLE_128B).  Out-of-bounds elements are zero-filled.
+// 2-D bf16 (or, with f32, fp32) row-major [rows, cols] with leading dimension ld (elements); box = [box_rows, box_cols],
+// box_cols * element size == 128 bytes (SWIZZLE_128B).  Out-of-bounds elements are zero-filled on loads and not written
+// by stores.
 int make_tmap_2d(const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t box_cols,
-                 CUtensorMap* out) {
-    MapKey key{ptr, rows, cols, ld, box_rows, box_cols};
+                 CUtensorMap* out, bool f32 = false) {
+    MapKey key{ptr, rows, cols, ld, box_rows, box_cols, f32};
+    const uint64_t esize = f32 ? 4 : 2;
     {
         std::lock_guard<std::mutex> lk(g_map_mu);
         auto it = g_maps.find(key);
@@ -94,13 +97,13 @@ int make_tmap_2d(const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uin
     }
     EncodeTiledFn enc = get_encode_fn();
     if (!enc) return fail(-3, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
-    if ((reinterpret_cast<uintptr_t>(ptr) & 15) || ((ld * 2) & 15)) return fail(-1, "TMA operand must be 16-byte aligned (ptr=%p ld=%llu)", ptr, (unsigned long long)ld);
+    if ((reinterpret_cast<uintptr_t>(ptr) & 15) || ((ld * esize) & 15)) return fail(-1, "TMA operand must be 16-byte aligned (ptr=%p ld=%llu)", ptr, (unsigned long long)ld);
     cuuint64_t gdim[2] = {cols, rows};
-    cuuint64_t gstride[1] = {ld * 2};
+    cuuint64_t gstride[1] = {ld * esize};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUtensorMap m;
-    CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+    CUresult r = enc(&m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(-3, "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu ld=%llu box=%ux%u", (int)r,
@@ -215,6 +218,16 @@ static int launch_conv(const CUtensorMap& tx, const CUtensorMap& tw, const CUten
     return 0;
 }
 
+template <int EPI, bool F32>
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const CUtensorMap& tr,
+                       const scail::GemmParams& p, int grid, cudaStream_t st) {
+    using namespace scail;
+    int rc;
+    if ((rc = set_smem(gemm_bf16_kernel<EPI, F32>, GEMM_SMEM_BYTES))) return rc;
+    gemm_bf16_kernel<EPI, F32><<<grid, GEMM_THREADS, GEMM_SMEM_BYTES, st>>>(ta, tw, tc, tr, p);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
 
 template <int LP, int VPL>
 static int launch_rmsnorm_cl(const void* x, const void* gamma, void* out, int64_t npix, int C, int silu, cudaStream_t st) {
@@ -257,30 +270,48 @@ int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, cons
     if (epilogue == EPI_BIAS_GATE_RES) SCAIL_REQUIRE(gate && residual && gate_stride % 8 == 0, "gemm: gate/residual required");
     if (epilogue == EPI_BIAS_RES) SCAIL_REQUIRE(residual, "gemm: residual required");
     if (residual) SCAIL_REQUIRE(ldr % 8 == 0, "gemm: ldr must be a multiple of 8");
-    CUtensorMap ta, tw;
+    const bool res_epi = epilogue == EPI_BIAS_GATE_RES || epilogue == EPI_BIAS_RES;
+    SCAIL_REQUIRE(!(c_fp32 && res_epi), "gemm: the residual epilogues write a bf16 output");
+    CUtensorMap ta, tw, tc, tr;
     int rc;
     GemmParams p;
     p.M = (int)M; p.N = (int)N; p.K = (int)K;
     p.bias = static_cast<const __nv_bfloat16*>(bias);
     p.gate = static_cast<const __nv_bfloat16*>(gate);
-    p.residual = static_cast<const __nv_bfloat16*>(residual);
-    p.C = c_fp32 ? nullptr : static_cast<__nv_bfloat16*>(C);
-    p.C32 = c_fp32 ? static_cast<float*>(C) : nullptr;
-    p.ldc = ldc; p.ldr = ldr; p.gate_stride = gate_stride;
+    p.gate_stride = gate_stride;
     p.rows_per_batch = rows_per_batch > 0 ? (int)rows_per_batch : (int)M;
-    p.epilogue = epilogue;
     static const int gm_env = getenv("SCAIL_GEMM_GROUP_M") ? atoi(getenv("SCAIL_GEMM_GROUP_M")) : 0;
     const int sms = sm_count();
     SCAIL_REQUIRE(sms > 0, "gemm: no CUDA device");
     if ((rc = make_tmap_2d(A, M, K, lda, GEMM_BM, GEMM_BK, &ta))) return rc;
     if ((rc = make_tmap_2d(W, N, K, ldw, GEMM_BN, GEMM_BK, &tw))) return rc;
+    // C (and the residual) in 64-row boxes of 128 bytes: one box per warpgroup and staging column chunk
+    if ((rc = make_tmap_2d(C, M, N, ldc, 64, c_fp32 ? 32 : 64, &tc, c_fp32 != 0))) return rc;
+    if (res_epi) {
+        if ((rc = make_tmap_2d(residual, M, N, ldr, 64, 64, &tr))) return rc;
+    } else {
+        tr = tc;  // unused
+    }
     p.group_m = gm_env > 0 ? gm_env : 16;
-    if ((rc = set_smem(gemm_bf16_kernel, GEMM_SMEM_BYTES))) return rc;
     const int num_tiles = blocks_for(M, GEMM_BM) * blocks_for(N, GEMM_BN);
     const int grid = num_tiles < sms ? num_tiles : sms;
-    gemm_bf16_kernel<<<grid, GEMM_THREADS, GEMM_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(ta, tw, p);
-    SCAIL_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    switch (epilogue) {
+        case EPI_BIAS:
+            return c_fp32 ? launch_gemm<EPI_BIAS, true>(ta, tw, tc, tr, p, grid, st)
+                          : launch_gemm<EPI_BIAS, false>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GELU:
+            return c_fp32 ? launch_gemm<EPI_BIAS_GELU, true>(ta, tw, tc, tr, p, grid, st)
+                          : launch_gemm<EPI_BIAS_GELU, false>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_SILU:
+            return c_fp32 ? launch_gemm<EPI_BIAS_SILU, true>(ta, tw, tc, tr, p, grid, st)
+                          : launch_gemm<EPI_BIAS_SILU, false>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GELU_ERF:
+            return c_fp32 ? launch_gemm<EPI_BIAS_GELU_ERF, true>(ta, tw, tc, tr, p, grid, st)
+                          : launch_gemm<EPI_BIAS_GELU_ERF, false>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GATE_RES: return launch_gemm<EPI_BIAS_GATE_RES, false>(ta, tw, tc, tr, p, grid, st);
+        default: return launch_gemm<EPI_BIAS_RES, false>(ta, tw, tc, tr, p, grid, st);
+    }
 }
 
 int scail_ln_modulate(const void* x, void* out, const void* gamma, const void* beta, const void* shift,

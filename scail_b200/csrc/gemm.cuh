@@ -1,9 +1,14 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = epi(A[M,K] * W[N,K]^T)
-//   * one producer warp streams A/W tiles with TMA (SWIZZLE_128B) into a 4-deep shared-memory ring,
+//   * one producer warp streams A/W tiles with TMA (SWIZZLE_128B) into a 3-deep shared-memory ring,
+//   * a second producer warp loads what the epilogue shares per tile: the tile's 256 bias values and gate rows into
+//     shared memory and, for the residual epilogues, the 128 x 256 residual tile by TMA into the output staging buffer,
+//     while the consumers are still in the main loop,
 //   * two consumer warpgroups each own 64 rows of the 128 x 256 tile: wgmma m64n256k16 with fp32 accumulators in registers,
 //     one wgmma group kept in flight so that a ring stage is released as soon as the MMAs that read it have retired,
-//   * the epilogue (bias / activation / gate / residual, one bf16 rounding) runs on the accumulator registers while the
-//     producer already fills the ring with the next tile's operands.
+//   * the epilogue (chosen at compile time: bias / activation / gate / residual in fp32, one bf16 rounding) writes the
+//     tile into the swizzled staging buffer and one thread per warpgroup stores it with TMA; the store drains while the
+//     next tile's main loop runs.  TMA clips the store to [M, N], so ragged edges and C as a column slab of a wider
+//     buffer never write outside the output.
 // Replaces the reference's F.linear calls (sat/mpu/layers.py:230-243, :425-444) together with
 // the elementwise ops that follow them (bias, GELU-tanh, gate*out + residual).
 #pragma once
@@ -20,29 +25,35 @@ enum GemmEpilogue : int {
     EPI_BIAS_GELU_ERF = 5,  // C = gelu(acc + bias), exact erf form (MLPProj, dit_video_crossattn_sc_xc.py:38)
 };
 
+// C and the residual are addressed through tensor maps; these are the operands the epilogue reads directly.
 struct GemmParams {
     int M, N, K;
-    const __nv_bfloat16* bias;      // [N] or null
-    const __nv_bfloat16* gate;      // [B, gate_stride] (row b = m / rows_per_batch) or null
-    const __nv_bfloat16* residual;  // [M, ldr] or null
-    __nv_bfloat16* C;               // [M, ldc]
-    float* C32;                     // optional fp32 output instead of bf16
-    int64_t ldc, ldr, gate_stride;
+    const __nv_bfloat16* bias;  // [N] or null
+    const __nv_bfloat16* gate;  // [B, gate_stride] (row b = m / rows_per_batch) or null
+    int64_t gate_stride;
     int rows_per_batch;
-    int epilogue;
     int group_m;  // rasterisation: m-blocks per L2 group
 };
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BN = 256;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_STAGES = 4;
+// 3 stages: the 64 KB output staging tile does not fit beside a 4th 48 KB stage in 227 KB.
+constexpr int GEMM_STAGES = 3;
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;  // 16 KB
 constexpr int GEMM_B_BYTES = GEMM_BN * GEMM_BK * 2;  // 32 KB
 constexpr int GEMM_STAGE_BYTES = GEMM_A_BYTES + GEMM_B_BYTES;
-constexpr int GEMM_SMEM_BYTES = GEMM_STAGES * GEMM_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+// Output staging: 4 column chunks of [128 rows][128 B] (64 bf16 or 32 fp32 columns), TMA SWIZZLE_128B layout.
+// Warpgroup w owns rows [64 w, 64 w + 64) of every chunk, so each warpgroup stores 64-row boxes of its own.
+constexpr int GEMM_OUT_CHUNK_BYTES = GEMM_BM * 128;  // 16 KB
+constexpr int GEMM_OUT_OFF = GEMM_STAGES * GEMM_STAGE_BYTES;
+constexpr int GEMM_BIAS_OFF = GEMM_OUT_OFF + 4 * GEMM_OUT_CHUNK_BYTES;  // fp32 [256], zeros without a bias
+constexpr int GEMM_GATE_OFF = GEMM_BIAS_OFF + GEMM_BN * 4;              // bf16 [2][256]: the gate rows of the tile's first two batches
+constexpr int GEMM_BAR_OFF = GEMM_GATE_OFF + 2 * GEMM_BN * 2;
+constexpr int GEMM_SMEM_BYTES = GEMM_BAR_OFF + 128 /*barriers*/ + 1024 /*align*/;
 constexpr int GEMM_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: consumers
 static_assert(GEMM_SMEM_BYTES <= 232448, "gemm: shared memory budget");
+static_assert(GEMM_OUT_OFF % 1024 == 0, "gemm: the staging buffer must be 1024-B aligned for SWIZZLE_128B");
 
 __device__ __forceinline__ void gemm_tile_coords(int tile, int num_m, int num_n, int group_m, int& m_blk, int& n_blk) {
     int per_group = group_m * num_n;
@@ -54,49 +65,37 @@ __device__ __forceinline__ void gemm_tile_coords(int tile, int num_m, int num_n,
     m_blk = first_m + (r - n_blk * gsize);
 }
 
-__device__ __forceinline__ float epi_act(float v, int epilogue) {
-    if (epilogue == EPI_BIAS_GELU) return gelu_tanh(v);
-    if (epilogue == EPI_BIAS_SILU) return v / (1.0f + __expf(-v));
-    if (epilogue == EPI_BIAS_GELU_ERF) return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));
-    return v;
+template <int EPI>
+__device__ __forceinline__ float epi_act(float v) {
+    if constexpr (EPI == EPI_BIAS_GELU) return gelu_tanh(v);
+    else if constexpr (EPI == EPI_BIAS_SILU) return v / (1.0f + __expf(-v));
+    else if constexpr (EPI == EPI_BIAS_GELU_ERF) return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));
+    else return v;
 }
 
-// Epilogue of one column pair (col, col + 1) of one row: bias, activation, gate, residual in fp32, one rounding.
-__device__ __forceinline__ void gemm_epilogue_pair(const GemmParams& p, int row, int col, float f0, float f1) {
-    if (row >= p.M || col >= p.N) return;
-    if (p.bias) {
-        const float2 b2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
-        f0 += b2.x;
-        f1 += b2.y;
-    }
-    if (p.epilogue == EPI_BIAS_GELU || p.epilogue == EPI_BIAS_SILU || p.epilogue == EPI_BIAS_GELU_ERF) {
-        f0 = epi_act(f0, p.epilogue);
-        f1 = epi_act(f1, p.epilogue);
-    }
-    if (p.epilogue == EPI_BIAS_GATE_RES) {
-        const int bidx = row / p.rows_per_batch;
-        const float2 g2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.gate + bidx * p.gate_stride + col));
-        f0 *= g2.x;
-        f1 *= g2.y;
-    }
-    if (p.epilogue == EPI_BIAS_GATE_RES || p.epilogue == EPI_BIAS_RES) {
-        const float2 r2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.residual + static_cast<int64_t>(row) * p.ldr + col));
-        f0 += r2.x;
-        f1 += r2.y;
-    }
-    if (p.C32) *reinterpret_cast<float2*>(p.C32 + static_cast<int64_t>(row) * p.ldc + col) = make_float2(f0, f1);
-    else *reinterpret_cast<uint32_t*>(p.C + static_cast<int64_t>(row) * p.ldc + col) = pack_bf16(f0, f1);
-}
-
+// F32: fp32 output (no residual epilogues).  The fp32 tile is twice the staging buffer, so it is stored in two
+// 128-column passes.
+template <int EPI, bool F32>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+                 const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r,
                  const GemmParams p) {
+    constexpr bool RES = EPI == EPI_BIAS_GATE_RES || EPI == EPI_BIAS_RES;
+    constexpr bool GATE = EPI == EPI_BIAS_GATE_RES;
+    static_assert(!(F32 && RES), "gemm: the residual epilogues write bf16");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = smem_base + GEMM_STAGES * GEMM_STAGE_BYTES;
-    // barrier layout (8 B each): full[S], empty[S]
+    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
+    const uint32_t out_base = smem_base + GEMM_OUT_OFF;
+    const uint32_t bias_base = smem_base + GEMM_BIAS_OFF;
+    const uint32_t bar_base = smem_base + GEMM_BAR_OFF;
+    // barrier layout (8 B each): full[S], empty[S], epi_full, epi_empty, res_full, out_free
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (GEMM_STAGES + s); };
+    const uint32_t epi_full = bar_base + 16u * GEMM_STAGES;  // bias / gate of the tile are in shared memory
+    const uint32_t epi_empty = epi_full + 8;                 // both warpgroups are done reading them
+    const uint32_t res_full = epi_full + 16;                 // the residual tile has landed in the staging buffer
+    const uint32_t out_free = epi_full + 24;                 // both warpgroups' previous stores have read the staging buffer
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -108,10 +107,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_w);
+        tma_prefetch_desc(&tmap_c);
+        if (RES) tma_prefetch_desc(&tmap_r);
         for (int s = 0; s < GEMM_STAGES; ++s) {
             mbar_init(full_bar(s), 1);
             mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
         }
+        mbar_init(epi_full, 32);  // every lane of the epilogue loader warp
+        mbar_init(epi_empty, 2);
+        mbar_init(res_full, 1);
+        mbar_init(out_free, 2);
         fence_barrier_init();
     }
     __syncthreads();
@@ -134,22 +139,85 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                     if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
                 }
             }
+        } else if (warp == 1) {
+            // ---- epilogue loader: per-tile bias and gate rows, and the residual tile ----
+            float* bias_s = reinterpret_cast<float*>(smem + GEMM_BIAS_OFF);
+            __nv_bfloat16* gate_s = reinterpret_cast<__nv_bfloat16*>(smem + GEMM_GATE_OFF);
+            int it = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+                int m_blk, n_blk;
+                gemm_tile_coords(tile, num_m, num_n, p.group_m, m_blk, n_blk);
+                const int m0 = m_blk * GEMM_BM, n0 = n_blk * GEMM_BN;
+                const int c = 8 * lane, col = n0 + c;  // N % 8 == 0: an 8-column group is wholly inside or outside
+                mbar_wait(epi_empty, (it & 1) ^ 1, 4);
+                uint4 braw = make_uint4(0, 0, 0, 0);
+                if (p.bias && col < p.N) braw = *reinterpret_cast<const uint4*>(p.bias + col);
+                const float2 b01 = unpack_bf16(braw.x), b23 = unpack_bf16(braw.y);
+                const float2 b45 = unpack_bf16(braw.z), b67 = unpack_bf16(braw.w);
+                *reinterpret_cast<float4*>(bias_s + c) = make_float4(b01.x, b01.y, b23.x, b23.y);
+                *reinterpret_cast<float4*>(bias_s + c + 4) = make_float4(b45.x, b45.y, b67.x, b67.y);
+                if constexpr (GATE) {
+                    const int b0 = m0 / p.rows_per_batch;
+#pragma unroll
+                    for (int s = 0; s < 2; ++s) {
+                        uint4 g = make_uint4(0, 0, 0, 0);
+                        const int b = b0 + s;
+                        if (col < p.N && static_cast<int64_t>(b) * p.rows_per_batch < p.M)
+                            g = *reinterpret_cast<const uint4*>(p.gate + b * p.gate_stride + col);
+                        *reinterpret_cast<uint4*>(gate_s + s * GEMM_BN + c) = g;
+                    }
+                }
+                mbar_arrive(epi_full);
+                if constexpr (RES) {
+                    if (lane == 0) {
+                        mbar_wait(out_free, it & 1, 5);
+                        uint32_t bytes = 0;
+                        for (int h = 0; h < 2; ++h)
+                            for (int cc = 0; cc < 4; ++cc)
+                                if (m0 + 64 * h < p.M && n0 + 64 * cc < p.N) bytes += GEMM_OUT_CHUNK_BYTES / 2;
+                        mbar_expect_tx(res_full, bytes);
+                        for (int h = 0; h < 2; ++h)
+                            for (int cc = 0; cc < 4; ++cc)
+                                if (m0 + 64 * h < p.M && n0 + 64 * cc < p.N)
+                                    tma_load_2d(out_base + cc * GEMM_OUT_CHUNK_BYTES + h * (GEMM_OUT_CHUNK_BYTES / 2), &tmap_r,
+                                                res_full, n0 + 64 * cc, m0 + 64 * h);
+                    }
+                    __syncwarp();
+                }
+            }
         }
     } else {
         // ===================== consumer warpgroups =====================
         setmaxnreg_inc<232>();
         const int wg = (warp >> 2) - 1;  // 0 or 1: rows [64 wg, 64 wg + 64) of the tile
         const int t = threadIdx.x & 127;
-        const bool releaser = t == 0;
+        const bool leader = t == 0;  // releases ring stages, issues and waits for this warpgroup's stores
+        // accumulator fragment: rows r0 (acc[4j], acc[4j+1]) and r0 + 8 (acc[4j+2], acc[4j+3]), columns 8 j + 2 q (+1)
+        const int r0 = (t >> 5) * 16 + ((t & 31) >> 2);
+        const int q = t & 3;
+        const uint32_t sw = static_cast<uint32_t>(r0 & 7);  // SWIZZLE_128B: 16-B unit u of row r sits at u ^ (r & 7)
+        const uint32_t out_rows = out_base + wg * (GEMM_OUT_CHUNK_BYTES / 2) + r0 * 128;
+        // shared address of columns (8 j + 2 q, +1), row r0 (+ 8 rows = + 1024 B)
+        auto out_addr = [&](int j) -> uint32_t {
+            if constexpr (F32) {
+                const int jp = j & 15;  // column 8 j + 2 q of the 128-column pass
+                return out_rows + (jp >> 2) * GEMM_OUT_CHUNK_BYTES + (((2u * (jp & 3) + (q >> 1)) ^ sw) << 4) + 8 * (q & 1);
+            } else {
+                return out_rows + (j >> 3) * GEMM_OUT_CHUNK_BYTES + (((j & 7) ^ sw) << 4) + 4 * q;
+            }
+        };
         int stage = 0;
         uint32_t phase = 0;
         float acc[GEMM_BN / 2];
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int it = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
             int m_blk, n_blk;
             gemm_tile_coords(tile, num_m, num_n, p.group_m, m_blk, n_blk);
+            const int m0 = m_blk * GEMM_BM, n0 = n_blk * GEMM_BN;
 #pragma unroll
             for (int i = 0; i < GEMM_BN / 2; ++i) acc[i] = 0.f;
             int prev_stage = -1;
+            const int kb_free = num_k > 1 ? 1 : 0;
             for (int kb = 0; kb < num_k; ++kb) {
                 mbar_wait(full_bar(stage), phase, 3);
                 const uint32_t sa = smem_base + stage * GEMM_STAGE_BYTES;
@@ -162,22 +230,110 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                 wgmma_commit();
                 wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
                 fence_regs(acc);
-                if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
+                if (prev_stage >= 0 && leader) mbar_arrive(empty_bar(prev_stage));
                 prev_stage = stage;
                 if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
+                // early in the tile: once the previous tile's store has read the staging buffer, hand it to the
+                // loader (residual) or to this warpgroup's epilogue
+                if (kb == kb_free && leader) {
+                    bulk_wait_read_all();
+                    mbar_arrive(out_free);
+                }
             }
             wgmma_wait<0>();
             fence_regs(acc);
-            if (prev_stage >= 0 && releaser) mbar_arrive(empty_bar(prev_stage));
-            // ---- epilogue straight from the accumulator fragments ----
-            const int row0 = m_blk * GEMM_BM + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
-            const int colb = n_blk * GEMM_BN + 2 * (t & 3);
+            if (prev_stage >= 0 && leader) mbar_arrive(empty_bar(prev_stage));
+
+            // ---- epilogue: fp32 in registers, one rounding, into the staging buffer ----
+            mbar_wait(epi_full, it & 1, 6);
+            if constexpr (RES) mbar_wait(res_full, it & 1, 7);
+            else named_bar_sync(1 + wg, 128);  // the leader has seen the previous store finish reading the buffer
+            const __nv_bfloat16* grow[2];
+            int gmax[2];
+            if constexpr (GATE) {
+                const int b0 = m0 / p.rows_per_batch;
 #pragma unroll
-            for (int j = 0; j < GEMM_BN / 8; ++j) {
-                gemm_epilogue_pair(p, row0, colb + 8 * j, acc[4 * j], acc[4 * j + 1]);
-                gemm_epilogue_pair(p, row0 + 8, colb + 8 * j, acc[4 * j + 2], acc[4 * j + 3]);
+                for (int h = 0; h < 2; ++h) {
+                    const int b = min(m0 + wg * 64 + r0 + 8 * h, p.M - 1) / p.rows_per_batch;
+                    if (b - b0 < 2) {
+                        grow[h] = reinterpret_cast<const __nv_bfloat16*>(smem + GEMM_GATE_OFF) + (b - b0) * GEMM_BN;
+                        gmax[h] = GEMM_BN - 2;
+                    } else {  // rows_per_batch < 128: a tile spanning more than two batches reads the gate in place
+                        grow[h] = p.gate + b * p.gate_stride + n0;
+                        gmax[h] = p.N - 2 - n0;
+                    }
+                }
             }
+            auto issue_store = [&](int pass) {
+                fence_proxy_async_smem();
+                named_bar_sync(1 + wg, 128);
+                if (leader) {
+                    const int rows = m0 + wg * 64;
+                    constexpr int chunk_cols = F32 ? 32 : 64;
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        const int col = n0 + pass * 128 + c * chunk_cols;
+                        if (rows < p.M && col < p.N)
+                            tma_store_2d(&tmap_c, out_base + c * GEMM_OUT_CHUNK_BYTES + wg * (GEMM_OUT_CHUNK_BYTES / 2), col, rows);
+                    }
+                    bulk_commit();
+                }
+            };
+            // G accumulator column groups (8 G columns) at a time: their shared-memory loads are issued together
+            constexpr int G = F32 ? 4 : 8;  // fewer live registers where the fp32 stores need them (no spills)
+#pragma unroll
+            for (int cc = 0; cc < 32 / G; ++cc) {
+                if constexpr (F32) {
+                    if (cc == 16 / G) {  // first 128 columns are staged: store them, wait until they are read
+                        issue_store(0);
+                        if (leader) bulk_wait_read_all();
+                        named_bar_sync(1 + wg, 128);
+                    }
+                }
+                float2 bb[G];
+                uint32_t gg[2 * G], rr[2 * G];
+#pragma unroll
+                for (int jj = 0; jj < G; ++jj) {
+                    const int j = G * cc + jj;
+                    bb[jj] = lds_f2(bias_base + 4 * (8 * j + 2 * q));
+                    if constexpr (GATE) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            gg[2 * jj + h] = *reinterpret_cast<const uint32_t*>(grow[h] + min(8 * j + 2 * q, gmax[h]));
+                    }
+                    if constexpr (RES) {
+                        rr[2 * jj] = lds_u32(out_addr(j));
+                        rr[2 * jj + 1] = lds_u32(out_addr(j) + 1024);
+                    }
+                }
+#pragma unroll
+                for (int jj = 0; jj < G; ++jj) {
+                    const int j = G * cc + jj;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float f0 = __fadd_rn(acc[4 * j + 2 * h], bb[jj].x);
+                        float f1 = __fadd_rn(acc[4 * j + 2 * h + 1], bb[jj].y);
+                        f0 = epi_act<EPI>(f0);
+                        f1 = epi_act<EPI>(f1);
+                        if constexpr (GATE) {
+                            const float2 g2 = unpack_bf16(gg[2 * jj + h]);
+                            f0 = __fmul_rn(f0, g2.x);
+                            f1 = __fmul_rn(f1, g2.y);
+                        }
+                        if constexpr (RES) {
+                            const float2 r2 = unpack_bf16(rr[2 * jj + h]);
+                            f0 = __fadd_rn(f0, r2.x);
+                            f1 = __fadd_rn(f1, r2.y);
+                        }
+                        if constexpr (F32) sts_f2(out_addr(j) + 1024 * h, f0, f1);
+                        else sts_u32(out_addr(j) + 1024 * h, pack_bf16(f0, f1));
+                    }
+                }
+            }
+            issue_store(F32 ? 1 : 0);
+            if (leader) mbar_arrive(epi_empty);  // bias and gate reads are behind the barrier in issue_store
         }
+        if (leader) bulk_wait_all();
     }
 }
 

@@ -15,3 +15,9 @@ timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$O
     > "$OUT/memcheck_chunked_pytest.log" 2>&1
 echo "sanitizer exit code $?" >> "$OUT/memcheck_chunked_pytest.log"
 tail -3 "$OUT/memcheck_chunked_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_chunked.log" | head -5
+# GEMM staged epilogue at small shapes: TMA residual loads and clipped TMA stores at ragged M / N and column slabs
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$OUT/memcheck_gemm_tiles.log" \
+    python -m pytest tests/test_gemm_tiles_gpu.py -q -x --timeout 600 -k "not bench_shapes" \
+    > "$OUT/memcheck_gemm_tiles_pytest.log" 2>&1
+echo "sanitizer exit code $?" >> "$OUT/memcheck_gemm_tiles_pytest.log"
+tail -3 "$OUT/memcheck_gemm_tiles_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_gemm_tiles.log" | head -5
