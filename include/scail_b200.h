@@ -49,6 +49,21 @@ int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, cons
                     int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
                     int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, scail_stream_t stream);
 
+/* FP8 (e4m3) GEMM: C[M,N] = epilogue((A_q[M,K] @ W_q[N,K]^T) * scale_a[m] * scale_w[n]); the scaled fp32 product goes
+ * through the same epilogues, in the same order, as scail_gemm_bf16.  A_q, W_q are e4m3 bytes (torch.float8_e4m3fn) with
+ * leading dims lda/ldw in elements; K, lda, ldw must be multiples of 16.  scale_a [M] and scale_w [N] are float32 (one per
+ * row, see scail_quant_rows_fp8).  C, bias, gate, residual as for scail_gemm_bf16; the output is bf16 only (c_fp32 != 0
+ * is refused with -1). */
+int scail_gemm_fp8(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
+                   int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
+                   int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, const float* scale_a,
+                   const float* scale_w, scail_stream_t stream);
+
+/* Row-wise e4m3 quantisation of a row-strided bf16 x [M, ldx]: scale[m] = amax(|x[m, :K]|) / 448 (IEEE division; 1 for an
+ * all-zero row), q[m, k] = satfinite_rn(x[m, k] / scale[m]) written densely as e4m3 [M, K].  K % 16 == 0, K <= 16384,
+ * ldx % 8 == 0; x and q 16-byte aligned. */
+int scail_quant_rows_fp8(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream);
+
 /* out = modulate(LayerNorm(x)) per row.  gamma/beta (bf16 [D]) and shift/scale (bf16 [B, mod_stride])
  * are optional (NULL).  Reads rows [in_row_offset, in_row_offset+rows_out) of each batch of
  * in_batch_rows rows; writes [B*rows_out, D] densely.  D % 8 == 0, D <= 5120.
@@ -57,6 +72,11 @@ int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, cons
 int scail_ln_modulate(const void* x, void* out, const void* gamma, const void* beta, const void* shift,
                       const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
                       int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream);
+/* The same rows quantised for scail_gemm_fp8: out_q e4m3 [B*rows_out, D] and out_scale float32 [B*rows_out], equal bit for
+ * bit to scail_quant_rows_fp8 of what scail_ln_modulate writes.  D % 16 == 0. */
+int scail_ln_modulate_fp8(const void* x, void* out_q, float* out_scale, const void* gamma, const void* beta, const void* shift,
+                          const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
+                          int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream);
 
 /* In-place RMSNorm over D columns (fp32 math, affine weight) of 1 or 2 column slabs of a
  * [rows, ld] bf16 matrix, optionally followed by interleaved-pair RoPE with per-token fp32

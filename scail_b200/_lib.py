@@ -24,7 +24,11 @@ SIGNATURES = {
     "scail_device_sm_count": [c_int],
     "scail_gemm_bf16": [c_p, c_i64, c_p, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_p, c_i64, c_i64, c_p,
                         c_i64, c_int, c_p],
+    "scail_gemm_fp8": [c_p, c_i64, c_p, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_p, c_i64, c_i64, c_p,
+                       c_i64, c_int, c_p, c_p, c_p],
+    "scail_quant_rows_fp8": [c_p, c_i64, c_p, c_p, c_i64, c_i64, c_p],
     "scail_ln_modulate": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
+    "scail_ln_modulate_fp8": [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
     "scail_rmsnorm_rope": [c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_f, c_p],
     "scail_attention": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                         c_i64, c_i64, c_f, c_int, c_p],

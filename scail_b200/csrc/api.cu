@@ -63,30 +63,31 @@ struct MapKey {
     const void* ptr;
     uint64_t rows, cols, ld;
     uint32_t box_rows, box_cols;
-    bool f32;
+    uint32_t esize;
     bool operator==(const MapKey& o) const {
         return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows &&
-               box_cols == o.box_cols && f32 == o.f32;
+               box_cols == o.box_cols && esize == o.esize;
     }
 };
 struct MapKeyHash {
     size_t operator()(const MapKey& k) const {
         size_t h = reinterpret_cast<size_t>(k.ptr);
         auto mix = [&](uint64_t v) { h ^= v + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2); };
-        mix(k.rows); mix(k.cols); mix(k.ld); mix(k.box_rows); mix(k.box_cols); mix(k.f32);
+        mix(k.rows); mix(k.cols); mix(k.ld); mix(k.box_rows); mix(k.box_cols); mix(k.esize);
         return h;
     }
 };
 std::mutex g_map_mu;
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 
-// 2-D bf16 (or, with f32, fp32) row-major [rows, cols] with leading dimension ld (elements); box = [box_rows, box_cols],
-// box_cols * element size == 128 bytes (SWIZZLE_128B).  Out-of-bounds elements are zero-filled on loads and not written
-// by stores.
+// 2-D row-major [rows, cols] with leading dimension ld (elements) of bf16 (esize 2), fp32 (4) or bytes (1: e4m3);
+// box = [box_rows, box_cols], box_cols * esize == 128 bytes (SWIZZLE_128B).  Out-of-bounds elements are zero-filled on loads
+// and not written by stores.
 int make_tmap_2d(const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t box_cols,
-                 CUtensorMap* out, bool f32 = false) {
-    MapKey key{ptr, rows, cols, ld, box_rows, box_cols, f32};
-    const uint64_t esize = f32 ? 4 : 2;
+                 CUtensorMap* out, uint32_t esize = 2) {
+    MapKey key{ptr, rows, cols, ld, box_rows, box_cols, esize};
+    const CUtensorMapDataType dtype = esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                      : esize == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     {
         std::lock_guard<std::mutex> lk(g_map_mu);
         auto it = g_maps.find(key);
@@ -103,7 +104,7 @@ int make_tmap_2d(const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uin
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUtensorMap m;
-    CUresult r = enc(&m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+    CUresult r = enc(&m, dtype, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(-3, "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu ld=%llu box=%ux%u", (int)r,
@@ -229,6 +230,18 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUten
     return 0;
 }
 
+template <int EPI>
+static int launch_gemm_fp8(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const CUtensorMap& tr,
+                           const scail::GemmParams& p, int grid, cudaStream_t st) {
+    using namespace scail;
+    constexpr int smem = GemmCfg<true>::SMEM_BYTES;
+    int rc;
+    if ((rc = set_smem(gemm_fp8_kernel<EPI>, smem))) return rc;
+    gemm_fp8_kernel<EPI><<<grid, GEMM_THREADS, smem, st>>>(ta, tw, tc, tr, p);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 template <int LP, int VPL>
 static int launch_rmsnorm_cl(const void* x, const void* gamma, void* out, int64_t npix, int C, int silu, cudaStream_t st) {
     const int pix_per_block = 8 * (32 / LP);
@@ -286,7 +299,7 @@ int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, cons
     if ((rc = make_tmap_2d(A, M, K, lda, GEMM_BM, GEMM_BK, &ta))) return rc;
     if ((rc = make_tmap_2d(W, N, K, ldw, GEMM_BN, GEMM_BK, &tw))) return rc;
     // C (and the residual) in 64-row boxes of 128 bytes: one box per warpgroup and staging column chunk
-    if ((rc = make_tmap_2d(C, M, N, ldc, 64, c_fp32 ? 32 : 64, &tc, c_fp32 != 0))) return rc;
+    if ((rc = make_tmap_2d(C, M, N, ldc, 64, c_fp32 ? 32 : 64, &tc, c_fp32 ? 4 : 2))) return rc;
     if (res_epi) {
         if ((rc = make_tmap_2d(residual, M, N, ldr, 64, 64, &tr))) return rc;
     } else {
@@ -314,22 +327,114 @@ int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, cons
     }
 }
 
-int scail_ln_modulate(const void* x, void* out, const void* gamma, const void* beta, const void* shift,
-                      const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
-                      int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream) {
+int scail_gemm_fp8(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
+                   int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
+                   int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, const float* scale_a,
+                   const float* scale_w, scail_stream_t stream) {
     using namespace scail;
-    SCAIL_REQUIRE(x && out, "ln_modulate: null operand");
+    using Cfg = GemmCfg<true>;
+    SCAIL_REQUIRE(A && W && C && scale_a && scale_w, "gemm_fp8: null operand");
+    SCAIL_REQUIRE(!c_fp32, "gemm_fp8: the output is bf16 (c_fp32 must be 0)");
+    SCAIL_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
+    SCAIL_REQUIRE(K % 16 == 0 && lda % 16 == 0 && ldw % 16 == 0,
+                  "gemm_fp8: K, lda and ldw must be multiples of 16 (16-byte e4m3 row pitch)");
+    SCAIL_REQUIRE(N % 8 == 0 && ldc % 8 == 0, "gemm_fp8: N and ldc must be multiples of 8");
+    SCAIL_REQUIRE(aligned16(C) && aligned16(bias) && aligned16(gate) && aligned16(residual),
+                  "gemm_fp8: C, bias, gate and residual must be 16-byte aligned (the epilogue uses 16-byte accesses)");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(scale_a) & 3) == 0 && (reinterpret_cast<uintptr_t>(scale_w) & 3) == 0,
+                  "gemm_fp8: scales must be 4-byte aligned float32");
+    SCAIL_REQUIRE(epilogue >= 0 && epilogue <= 5, "gemm_fp8: unknown epilogue %d", epilogue);
+    if (epilogue == EPI_BIAS_GATE_RES) SCAIL_REQUIRE(gate && residual && gate_stride % 8 == 0, "gemm_fp8: gate/residual required");
+    if (epilogue == EPI_BIAS_RES) SCAIL_REQUIRE(residual, "gemm_fp8: residual required");
+    if (residual) SCAIL_REQUIRE(ldr % 8 == 0, "gemm_fp8: ldr must be a multiple of 8");
+    const bool res_epi = epilogue == EPI_BIAS_GATE_RES || epilogue == EPI_BIAS_RES;
+    CUtensorMap ta, tw, tc, tr;
+    int rc;
+    GemmParams p;
+    p.M = (int)M; p.N = (int)N; p.K = (int)K;
+    p.bias = static_cast<const __nv_bfloat16*>(bias);
+    p.gate = static_cast<const __nv_bfloat16*>(gate);
+    p.gate_stride = gate_stride;
+    p.rows_per_batch = rows_per_batch > 0 ? (int)rows_per_batch : (int)M;
+    p.group_m = 16;
+    p.scale_a = scale_a;
+    p.scale_w = scale_w;
+    const int sms = sm_count();
+    SCAIL_REQUIRE(sms > 0, "gemm_fp8: no CUDA device");
+    if ((rc = make_tmap_2d(A, M, K, lda, Cfg::BM, Cfg::BK, &ta, 1))) return rc;
+    if ((rc = make_tmap_2d(W, N, K, ldw, Cfg::BN, Cfg::BK, &tw, 1))) return rc;
+    if ((rc = make_tmap_2d(C, M, N, ldc, 64, 64, &tc))) return rc;
+    if (res_epi) {
+        if ((rc = make_tmap_2d(residual, M, N, ldr, 64, 64, &tr))) return rc;
+    } else {
+        tr = tc;  // unused
+    }
+    const int num_tiles = blocks_for(M, Cfg::BM) * blocks_for(N, Cfg::BN);
+    const int grid = num_tiles < sms ? num_tiles : sms;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    switch (epilogue) {
+        case EPI_BIAS: return launch_gemm_fp8<EPI_BIAS>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GELU: return launch_gemm_fp8<EPI_BIAS_GELU>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_SILU: return launch_gemm_fp8<EPI_BIAS_SILU>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GELU_ERF: return launch_gemm_fp8<EPI_BIAS_GELU_ERF>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GATE_RES: return launch_gemm_fp8<EPI_BIAS_GATE_RES>(ta, tw, tc, tr, p, grid, st);
+        default: return launch_gemm_fp8<EPI_BIAS_RES>(ta, tw, tc, tr, p, grid, st);
+    }
+}
+
+int scail_quant_rows_fp8(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(x && q && scale, "quant_rows_fp8: null operand");
+    SCAIL_REQUIRE(M > 0 && K > 0 && K % 16 == 0 && ldx % 8 == 0 && aligned16(x) && aligned16(q),
+                  "quant_rows_fp8: K must be a multiple of 16, ldx of 8, x and q 16-byte aligned");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(scale) & 3) == 0, "quant_rows_fp8: scale must be 4-byte aligned float32");
+    auto xp = static_cast<const __nv_bfloat16*>(x);
+    auto qp = static_cast<uint8_t*>(q);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int vpt = blocks_for(K / 8, ROW_THREADS);  // 16-byte vectors per thread
+    if (vpt <= 4) quant_rows_fp8_kernel<4><<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
+    else if (vpt <= 8) quant_rows_fp8_kernel<8><<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
+    else if (vpt <= 16) quant_rows_fp8_kernel<16><<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
+    else return fail(-1, "quant_rows_fp8: K=%lld exceeds %d", (long long)K, 16 * ROW_THREADS * 8);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+static int ln_modulate_impl(const void* x, void* out, void* out_q, float* out_scale, const void* gamma, const void* beta,
+                            const void* shift, const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out,
+                            int64_t in_batch_rows, int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream) {
+    using namespace scail;
     SCAIL_REQUIRE(D % 8 == 0 && D <= ROW_MAXV * ROW_THREADS * 8, "ln_modulate: D=%lld must be a multiple of 8 and <= %d", (long long)D, ROW_MAXV * ROW_THREADS * 8);
     SCAIL_REQUIRE((gamma == nullptr) == (beta == nullptr) && (shift == nullptr) == (scale == nullptr), "ln_modulate: gamma/beta and shift/scale come in pairs");
     LnModParams p;
     p.x = static_cast<const __nv_bfloat16*>(x); p.out = static_cast<__nv_bfloat16*>(out);
+    p.out_q = static_cast<uint8_t*>(out_q); p.out_scale = out_scale;
     p.gamma = static_cast<const __nv_bfloat16*>(gamma); p.beta = static_cast<const __nv_bfloat16*>(beta);
     p.shift = static_cast<const __nv_bfloat16*>(shift); p.scale = static_cast<const __nv_bfloat16*>(scale);
     p.mod_stride = mod_stride; p.D = (int)D; p.rows_out = (int)rows_out; p.in_batch_rows = (int)in_batch_rows;
     p.in_row_offset = (int)in_row_offset; p.total_rows = (int)(B * rows_out); p.eps = eps;
-    ln_modulate_kernel<<<p.total_rows, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    if (out_q) ln_modulate_kernel<true><<<p.total_rows, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    else ln_modulate_kernel<false><<<p.total_rows, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int scail_ln_modulate(const void* x, void* out, const void* gamma, const void* beta, const void* shift,
+                      const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
+                      int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && out, "ln_modulate: null operand");
+    return ln_modulate_impl(x, out, nullptr, nullptr, gamma, beta, shift, scale, mod_stride, B, rows_out, in_batch_rows,
+                            in_row_offset, D, eps, stream);
+}
+
+int scail_ln_modulate_fp8(const void* x, void* out_q, float* out_scale, const void* gamma, const void* beta, const void* shift,
+                          const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
+                          int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && out_q && out_scale, "ln_modulate_fp8: null operand");
+    SCAIL_REQUIRE(D % 16 == 0 && aligned16(out_q) && (reinterpret_cast<uintptr_t>(out_scale) & 3) == 0,
+                  "ln_modulate_fp8: D must be a multiple of 16, out_q 16-byte aligned, out_scale 4-byte aligned");
+    return ln_modulate_impl(x, nullptr, out_q, out_scale, gamma, beta, shift, scale, mod_stride, B, rows_out, in_batch_rows,
+                            in_row_offset, D, eps, stream);
 }
 
 int scail_rmsnorm_rope(void* buf, int64_t ld, int64_t rows, int64_t rows_per_batch, int64_t D, int nslabs,

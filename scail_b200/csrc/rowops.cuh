@@ -1,6 +1,8 @@
 // HBM-bound row / elementwise kernels of the SCAIL DiT step (everything that is not a GEMM or attention).
 // One warp per row, 16-byte vectorised loads, fp32 statistics, bf16 in/out.
 #pragma once
+#include <cuda_fp8.h>
+
 #include "sm90.cuh"
 
 namespace scail {
@@ -28,9 +30,72 @@ __device__ __forceinline__ float row_block_sum(float v, float* red) {
     return t;
 }
 
+// max over the 128-thread block; same contract as row_block_sum
+__device__ __forceinline__ float row_block_max(float v, float* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    const float t = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
+    __syncthreads();
+    return t;
+}
+
+// ---- e4m3 row quantisation, the one format of the fp8 GEMMs: s = amax(|row|) / 448 (IEEE division), q = satfinite_rn(x / s);
+// an all-zero row gets s = 1 and q = 0.  torch: (x.float() / s[:, None]).clamp(-448, 448).to(torch.float8_e4m3fn)
+constexpr float FP8_E4M3_MAX = 448.0f;
+
+__device__ __forceinline__ float absmax_bf16x2(float m, uint32_t w) {
+    const float2 f = unpack_bf16(w);
+    return fmaxf(m, fmaxf(fabsf(f.x), fabsf(f.y)));
+}
+__device__ __forceinline__ float fp8_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, FP8_E4M3_MAX) : 1.0f; }
+// 8 bf16 -> 8 e4m3 bytes
+__device__ __forceinline__ uint2 quant_bf16x8(const uint4 v, float s) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint32_t h[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float2 f = unpack_bf16(w[k]);
+        h[k] = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(f.x, s), __fdiv_rn(f.y, s)), __NV_SATFINITE, __NV_E4M3);
+    }
+    return make_uint2(h[0] | (h[1] << 16), h[2] | (h[3] << 16));
+}
+
+// One 128-thread block per row of a row-strided bf16 [M, K] (K % 16 == 0, K <= 8 * ROW_THREADS * V): the row stays in registers
+// between the amax reduction and the quantisation, so it is read once.
+template <int V>
+__global__ void __launch_bounds__(ROW_THREADS) quant_rows_fp8_kernel(const __nv_bfloat16* x, int64_t ldx, uint8_t* q,
+                                                                      float* scale, int K) {
+    __shared__ float red[4];
+    const int64_t row = blockIdx.x;
+    const uint4* xin = reinterpret_cast<const uint4*>(x + row * ldx);
+    const int nvec = K >> 3;
+    uint4 v[V];
+    float amax = 0.f;
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+        const int i = j * ROW_THREADS + threadIdx.x;
+        if (i < nvec) {
+            v[j] = xin[i];
+            amax = absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(amax, v[j].x), v[j].y), v[j].z), v[j].w);
+        }
+    }
+    const float s = fp8_row_scale(row_block_max(amax, red));
+    if (threadIdx.x == 0) scale[row] = s;
+    uint2* o = reinterpret_cast<uint2*>(q + row * K);
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+        const int i = j * ROW_THREADS + threadIdx.x;
+        if (i < nvec) o[i] = quant_bf16x8(v[j], s);
+    }
+}
+
 struct LnModParams {
     const __nv_bfloat16* x;      // input rows
-    __nv_bfloat16* out;          // output rows [B*rows_out, D]
+    __nv_bfloat16* out;          // output rows [B*rows_out, D] (bf16 form)
+    uint8_t* out_q;              // fp8 form: e4m3 rows [B*rows_out, D] and their fp32 scales [B*rows_out]
+    float* out_scale;
     const __nv_bfloat16* gamma;  // optional affine
     const __nv_bfloat16* beta;
     const __nv_bfloat16* shift;  // optional modulation [B, mod_stride]
@@ -68,6 +133,9 @@ __device__ __forceinline__ float hsum_f32x2(uint64_t v) {
 // LayerNorm (+optional affine) (+optional AdaLN modulate x*(1+scale)+shift).
 // Restates F.layer_norm + modulate (dit_video_crossattn_sc_xc.py:760-761, :1031-1032, :1045-1046, :825).
 // The row is unpacked to fp32 pairs once and stays in registers (4 x ROW_MAXV packed f32x2 per thread) for all three passes.
+// FP8: the bf16 row the bf16 form would write is quantised to e4m3 in registers (one more block reduction for its amax),
+// so the result equals quant_rows_fp8 of the bf16 form bit for bit.
+template <bool FP8>
 __global__ void __launch_bounds__(ROW_THREADS) ln_modulate_kernel(const LnModParams p) {
     __shared__ float red[4];
     const int row = blockIdx.x;
@@ -107,6 +175,8 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_modulate_kernel(const LnModPar
     const float rstd = rsqrtf(row_block_sum(hsum_f32x2(acc), red) / p.D + p.eps);
     const uint64_t rstd2 = pack_f32x2(rstd, rstd), one2 = pack_f32x2(1.0f, 1.0f);
     uint4* o = reinterpret_cast<uint4*>(p.out + static_cast<int64_t>(row) * p.D);
+    [[maybe_unused]] uint4 ob[ROW_MAXV];  // fp8: the bf16 row, kept for the quantisation
+    [[maybe_unused]] float amax = 0.f;
 #pragma unroll
     for (int j = 0; j < ROW_MAXV; ++j) {
         const int i = j * ROW_THREADS + threadIdx.x;
@@ -135,7 +205,22 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_modulate_kernel(const LnModPar
             ov.y = f32x2_to_bf16x2(y[1]);
             ov.z = f32x2_to_bf16x2(y[2]);
             ov.w = f32x2_to_bf16x2(y[3]);
-            o[i] = ov;
+            if constexpr (FP8) {
+                ob[j] = ov;
+                amax = absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(amax, ov.x), ov.y), ov.z), ov.w);
+            } else {
+                o[i] = ov;
+            }
+        }
+    }
+    if constexpr (FP8) {
+        const float s = fp8_row_scale(row_block_max(amax, red));
+        if (threadIdx.x == 0) p.out_scale[row] = s;
+        uint2* oq = reinterpret_cast<uint2*>(p.out_q + static_cast<int64_t>(row) * p.D);
+#pragma unroll
+        for (int j = 0; j < ROW_MAXV; ++j) {
+            const int i = j * ROW_THREADS + threadIdx.x;
+            if (i < nvec) oq[i] = quant_bf16x8(ob[j], s);
         }
     }
 }

@@ -18,6 +18,7 @@ sequences launches.  There is no CPU path: calling forward without CUDA raises.
 """
 import argparse
 import math
+import weakref
 from functools import reduce
 from operator import mul
 
@@ -64,6 +65,11 @@ class _Linear(nn.Module):
         super().__init__()
         self.weight = nn.Parameter(torch.randn(out_features, in_features) * std)
         self.bias = nn.Parameter(torch.zeros(out_features)) if bias else None
+
+    def __getstate__(self):  # the e4m3 copy (AdaLNMixin.fp8_weight) is derived data holding a weakref: not pickled
+        state = self.__dict__.copy()
+        state.pop("_fp8_cache", None)
+        return state
 
 
 class _Norm(nn.Module):
@@ -290,7 +296,7 @@ class AdaLNMixin(BaseMixin):
 
     def __init__(self, hidden_size, num_layers, time_embed_dim, compressed_num_frames, transformer_args, qk_ln=True,
                  qk_ln_affine=None, hidden_size_head=None, params_dtype=torch.float, device=torch.device("cpu"),
-                 elementwise_affine=True, share_adaln=False, use_i2v_clip=False):
+                 elementwise_affine=True, share_adaln=False, use_i2v_clip=False, fp8_linear=False):
         super().__init__()
         if not (qk_ln and share_adaln and use_i2v_clip) or hidden_size_head != hidden_size:
             raise NotImplementedError("scail_b200 implements qk_ln=True over the full hidden width, share_adaln=True, use_i2v_clip=True")
@@ -316,6 +322,65 @@ class AdaLNMixin(BaseMixin):
         # an explicit handle — nothing is keyed on tensor addresses) and every step reuses them: numerically identical.
         # bench.py keeps it OFF so that the timed step does the reference's full work.
         self.cache_cross_kv = False
+        # Opt-in: the six per-block linears over all tokens (QKV, self-attention out, cross q, cross-attention out, fc1, fc2) run
+        # as e4m3 GEMMs with one scale per token and per output channel (scail_gemm_fp8); everything else stays bf16.  The
+        # e4m3 weights are derived on the GPU on first use and are not part of the state_dict.  A plain attribute: it can be
+        # toggled between forwards.
+        self.fp8_linear = fp8_linear
+
+    # -- fp8 linears ---------------------------------------------------------------------------
+    FP8_LINEARS = ("attention.query_key_value", "attention.dense", "cross_attention.query", "cross_attention.dense",
+                   "mlp.dense_h_to_4h", "mlp.dense_4h_to_h")
+
+    def fp8_weight(self, lin, streams=()):
+        """(q e4m3 [out, in], scale fp32 [out]) of `lin.weight`, quantised on the current stream on first use and again
+        whenever the parameter object, its storage or its version has changed (a checkpoint loaded after construction, an
+        in-place edit), so a stale copy is never used.  The copy lives on `lin` (not in the state_dict) with only a weak
+        reference to the weight: a replaced parameter is neither kept alive nor served.  A changed weight of the same shape
+        is re-derived into the same buffers, so the pointers a CUDA graph captured stay valid.  Newly allocated buffers are
+        recorded on `streams`, the other streams that will read them."""
+        w = lin.weight
+        tag = (w.data_ptr(), w._version)
+        c = getattr(lin, "_fp8_cache", None)
+        if c is not None and c[0]() is w and c[1] == tag:
+            return c[2], c[3]
+        if c is not None and c[2].shape == w.shape and c[2].device == w.device:
+            q, sc = ops.quant_rows_fp8(w.detach(), c[2], c[3])
+        else:
+            lin._fp8_cache = None  # free the old copy before allocating the new one
+            q, sc = ops.quant_rows_fp8(w.detach())
+            for st in streams:
+                q.record_stream(st)
+                sc.record_stream(st)
+        lin._fp8_cache = (weakref.ref(w), tag, q, sc)
+        return q, sc
+
+    def prepare_fp8_weights(self, num_layers=None, streams=()):
+        """Bring the e4m3 copies of the first `num_layers` blocks' six linears up to date on the current stream.  Work that
+        reads them on other streams must be ordered after this (DiffusionTransformer.forward does it before the context-parallel
+        branch streams fork).  Returns the copies."""
+        out = []
+        for layer in list(self.transformer.layers)[:num_layers]:
+            for name in self.FP8_LINEARS:
+                out.extend(self.fp8_weight(layer.get_submodule(name), streams))
+        return out
+
+    def _fp8_act(self, x2, name):
+        """x2 bf16 [M, K] -> its e4m3 rows and scales, in the per-stream workspace `name`."""
+        M, K = x2.shape
+        q = _WS.get(name, (M, K), x2.device, ops.FP8)
+        sc = _WS.get(name + "_scale", (M,), x2.device, torch.float32)
+        return ops.quant_rows_fp8(x2, q, sc)
+
+    def _linear(self, x2, lin, x_scale=None, out=None, name="act8", **kw):
+        """epilogue(x2 @ lin.weight^T + lin.bias) into `out`.  bf16 GEMM unless fp8_linear; then the e4m3 GEMM, on x2 itself when
+        it is already e4m3 (with its row scales x_scale), else on x2 quantised into workspace `name`."""
+        if not self.fp8_linear:
+            return ops.gemm(x2, lin.weight, lin.bias, out=out, **kw)
+        if x2.dtype != ops.FP8:
+            x2, x_scale = self._fp8_act(x2, name)
+        wq, ws = self.fp8_weight(lin)
+        return ops.gemm_fp8(x2, x_scale, wq, ws, lin.bias, out=out, **kw)
 
     # -- hooks ---------------------------------------------------------------------------------
     def layer_forward(self, hidden_states, mask, *args, **kwargs):
@@ -336,39 +401,51 @@ class AdaLNMixin(BaseMixin):
         eps = self.layernorm_epsilon
         x2 = x.view(B * N, d)
         mod = ops.adaln_modulation(kwargs["emb"], self.adaLN_modulations[l].view(-1)).view(B, 6, d)  # :1025-1028
-        lnb = _WS.get("ln", (B, N, d), dev)
+        fp8 = self.fp8_linear
+        if fp8:
+            ln8 = (_WS.get("ln8", (B * N, d), dev, ops.FP8), _WS.get("ln8_scale", (B * N,), dev, torch.float32))
+        else:
+            lnb = _WS.get("ln", (B, N, d), dev)
+
+        def ln(**kw):
+            """The block's LNs feed linears only: with fp8_linear they write e4m3 rows + scales.  -> (rows [B, N, d], scales)"""
+            if fp8:
+                ops.ln_modulate(x, eps=eps, out_fp8=ln8, **kw)
+                return ln8[0].view(B, N, d), ln8[1]
+            return ops.ln_modulate(x, out=lnb, eps=eps, **kw), None
 
         # ---- self attention (:1031-1036) ----
-        ops.ln_modulate(x, out=lnb, shift=mod[:, 0], scale=mod[:, 1], eps=eps)
+        h, hs = ln(shift=mod[:, 0], scale=mod[:, 1])
         ctx = _WS.get("ctx", (B * N, d), dev)
-        self.attention_forward(lnb, mask, _ctx_out=ctx, **kwargs)  # leaves merged-head context in ctx
+        self.attention_forward(h, mask, _ctx_out=ctx, _fp8_scale=hs, **kwargs)  # leaves merged-head context in ctx
         a = layer.attention
-        ops.gemm(ctx, a.dense.weight, a.dense.bias, out=x2, epilogue=ops.EPI_BIAS_GATE_RES, gate=mod[:, 2],
-                 residual=x2, rows_per_batch=N)
+        self._linear(ctx, a.dense, out=x2, name="ctx8", epilogue=ops.EPI_BIAS_GATE_RES, gate=mod[:, 2], residual=x2,
+                     rows_per_batch=N)
 
         # ---- cross attention (:1039-1042) ----
         pl = layer.post_cross_attention_layernorm
-        ops.ln_modulate(x, out=lnb, gamma=pl.weight, beta=pl.bias, eps=eps)
+        h, hs = ln(gamma=pl.weight, beta=pl.bias)
         xkv_all = kwargs.get("_xkv_layers")
-        self.cross_attention_forward(lnb, kwargs.get("cross_attention_mask"), kwargs["encoder_outputs"], _ctx_out=ctx,
-                                     _xkv=xkv_all[l] if xkv_all is not None else None,
+        self.cross_attention_forward(h, kwargs.get("cross_attention_mask"), kwargs["encoder_outputs"], _ctx_out=ctx,
+                                     _xkv=xkv_all[l] if xkv_all is not None else None, _fp8_scale=hs,
                                      **{k: v for k, v in kwargs.items() if k not in ("cross_attention_mask", "encoder_outputs")})
         c = layer.cross_attention
-        ops.gemm(ctx, c.dense.weight, c.dense.bias, out=x2, epilogue=ops.EPI_BIAS_RES, residual=x2)
+        self._linear(ctx, c.dense, out=x2, name="ctx8", epilogue=ops.EPI_BIAS_RES, residual=x2)
 
         # ---- MLP (:1045-1050) ----
-        ops.ln_modulate(x, out=lnb, shift=mod[:, 3], scale=mod[:, 4], eps=eps)
+        h, hs = ln(shift=mod[:, 3], scale=mod[:, 4])
         m = layer.mlp
         inner = m.dense_h_to_4h.weight.shape[0]
         h1 = _WS.get("mlp", (B * N, inner), dev)
-        ops.gemm(lnb.view(B * N, d), m.dense_h_to_4h.weight, m.dense_h_to_4h.bias, out=h1, epilogue=ops.EPI_BIAS_GELU)
-        ops.gemm(h1, m.dense_4h_to_h.weight, m.dense_4h_to_h.bias, out=x2, epilogue=ops.EPI_BIAS_GATE_RES,
-                 gate=mod[:, 5], residual=x2, rows_per_batch=N)
+        self._linear(h.view(B * N, d), m.dense_h_to_4h, hs, out=h1, epilogue=ops.EPI_BIAS_GELU)
+        self._linear(h1, m.dense_4h_to_h, out=x2, name="mlp8", epilogue=ops.EPI_BIAS_GATE_RES, gate=mod[:, 5], residual=x2,
+                     rows_per_batch=N)
         return x
 
-    def attention_forward(self, hidden_states, mask, _ctx_out=None, **kw_args):
+    def attention_forward(self, hidden_states, mask, _ctx_out=None, _fp8_scale=None, **kw_args):
         """:1058-1105.  Returns the out-projected attention output unless `_ctx_out` is given (then the
-        merged-head context is left there for the fused out-proj epilogue of layer_forward)."""
+        merged-head context is left there for the fused out-proj epilogue of layer_forward).  hidden_states may be e4m3 rows
+        with their scales in `_fp8_scale` (fp8_linear)."""
         l = int(kw_args["layer_id"])
         a = self.transformer.layers[l].attention
         B, N, d = hidden_states.shape
@@ -376,24 +453,28 @@ class AdaLNMixin(BaseMixin):
         H = self.num_attention_heads
         cos, sin = self._rope_tables(dev, **kw_args)
         h2 = hidden_states.view(B * N, d)
+        if self.fp8_linear and h2.dtype != ops.FP8:
+            h2, _fp8_scale = self._fp8_act(h2, "ln8")
         ctx = _ctx_out if _ctx_out is not None else torch.empty(B * N, d, device=dev, dtype=torch.bfloat16)
         wq, wk = self.query_layernorm_list[l].weight, self.key_layernorm_list[l].weight
         if self.cp is None or self.cp.size == 1:
             qkv = _WS.get("qkv", (B * N, 3 * d), dev)
-            ops.gemm(h2, a.query_key_value.weight, a.query_key_value.bias, out=qkv)
+            self._linear(h2, a.query_key_value, _fp8_scale, out=qkv)
             ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon)
             ops.attention(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, N)
         else:
             # engine-style sequence parallelism (diffusion_video.py:495-552): the latents arrive pre-chunked on H or W, so the
             # RoPE tables built from rope_H/W_shift are already this rank's; otherwise tokens were sharded by shard_tokens()
             self.cp.self_attention(self, a, h2, B, N, d, H, wq, wk, cos, sin, ctx,
-                                   tables_local=kw_args.get("chunk_dim") is not None)
+                                   tables_local=kw_args.get("chunk_dim") is not None, h_scale=_fp8_scale)
         if _ctx_out is not None:
             return None
-        return ops.gemm(ctx, a.dense.weight, a.dense.bias).view(B, N, d)
+        return self._linear(ctx, a.dense, name="ctx8").view(B, N, d)
 
-    def cross_attention_forward(self, hidden_states, cross_attention_mask, encoder_outputs, _ctx_out=None, **kw_args):
-        """:1107-1203: text K/V and CLIP K/V are two separate softmaxes whose outputs are summed (F4)."""
+    def cross_attention_forward(self, hidden_states, cross_attention_mask, encoder_outputs, _ctx_out=None, _fp8_scale=None,
+                                **kw_args):
+        """:1107-1203: text K/V and CLIP K/V are two separate softmaxes whose outputs are summed (F4).  hidden_states may be
+        e4m3 rows with their scales in `_fp8_scale` (fp8_linear)."""
         l = int(kw_args["layer_id"])
         c = self.transformer.layers[l].cross_attention
         B, N, d = hidden_states.shape
@@ -405,7 +486,7 @@ class AdaLNMixin(BaseMixin):
         clip = kw_args["image_clip_features"].to(bf).contiguous()
         Lt, Lc = text.shape[1], clip.shape[1]
         xq = _WS.get("xq", (B * N, d), dev)
-        ops.gemm(hidden_states.view(B * N, d), c.query.weight, c.query.bias, out=xq)
+        self._linear(hidden_states.view(B * N, d), c.query, _fp8_scale, out=xq, name="ln8")
         ops.rmsnorm_rope(xq, N, d, [(0, self.cross_query_layernorm_list[l].weight)], eps=eps)
         pre = kw_args.get("_xkv")  # (tkv, ckv) of this layer from a Conditioning handle (rows of this call's batch elements)
         if pre is not None:
@@ -417,7 +498,7 @@ class AdaLNMixin(BaseMixin):
         ops.attention(xq, ckv[:, :d], ckv[:, d:], ctx, B, H, N, Lc, accumulate=True)
         if _ctx_out is not None:
             return None
-        return ops.gemm(ctx, c.dense.weight, c.dense.bias).view(B, N, d)
+        return self._linear(ctx, c.dense, name="ctx8").view(B, N, d)
 
     def cross_kv(self, l, text, clip, keep=False):
         """Text and CLIP K,V of layer l (:1117-1130): K/V projection + K RMSNorm.  keep=True allocates fresh buffers (for a
@@ -463,7 +544,7 @@ class DiffusionTransformer(nn.Module):
                  latent_height=300, patch_size=(1, 2, 2), in_channels=20, out_channels=16, hidden_size=5120,
                  text_dim=4096, num_layers=40, num_attention_heads=40, elementwise_affine=False, time_freq_dim=256,
                  time_embed_dim=None, modules=None, share_adaln=True, use_SwiGLU=False, use_RMSNorm=False,
-                 layernorm_epsilon=1e-6, inner_hidden_size=None, use_i2v_clip=True, dtype="bf16", **kwargs):
+                 layernorm_epsilon=1e-6, inner_hidden_size=None, use_i2v_clip=True, dtype="bf16", fp8_linear=False, **kwargs):
         super().__init__()
         if use_SwiGLU or use_RMSNorm:
             raise NotImplementedError("SCAIL-14B uses the non-gated GELU-tanh MLP and LayerNorm (yaml:42-43)")
@@ -498,7 +579,7 @@ class DiffusionTransformer(nn.Module):
         self.add_mixin("patch_embed", ImagePatchEmbeddingMixin(in_channels, d, self.patch_size))
         self.add_mixin("adaln_layer", AdaLNMixin(d, num_layers, self.time_embed_dim, frames, targs, qk_ln=True,
                                                  qk_ln_affine=True, hidden_size_head=d, elementwise_affine=elementwise_affine,
-                                                 share_adaln=True, use_i2v_clip=True))
+                                                 share_adaln=True, use_i2v_clip=True, fp8_linear=fp8_linear))
         self.add_mixin("final_layer", FinalLayerMixin(d, self.time_embed_dim, self.patch_size, out_channels,
                                                       elementwise_affine, layernorm_epsilon, True))
         object.__setattr__(self.mixins["adaln_layer"], "_pos_embed", self.mixins["pos_embed"])
@@ -619,6 +700,8 @@ class DiffusionTransformer(nn.Module):
         local = hidden if chunk_dim is not None else cp.shard_tokens(hidden)
         main = torch.cuda.current_stream()
         streams = cp.branch_streams(b, x.device)
+        if ad.fp8_linear:  # every branch reads the same e4m3 weights: derive them here, before the branch streams wait on main
+            ad.prepare_fp8_weights(n_layers, streams)
         per = []
         for i in range(b):
             kwi = dict(kw, emb=adaln[i:i + 1], encoder_outputs=text[i:i + 1], image_clip_features=clip[i:i + 1])

@@ -51,17 +51,73 @@ def gemm(a, w, bias=None, out=None, epilogue=EPI_BIAS, gate=None, residual=None,
     return out
 
 
-def ln_modulate(x, out=None, gamma=None, beta=None, shift=None, scale=None, eps=1e-6, rows_out=None, row_offset=0):
-    """x [B, Nin, D] -> out [B, rows_out, D] = modulate(LN(x[:, row_offset:row_offset+rows_out]))."""
+FP8 = torch.float8_e4m3fn
+
+
+def gemm_fp8(a, a_scale, w, w_scale, bias=None, out=None, epilogue=EPI_BIAS, gate=None, residual=None, rows_per_batch=0):
+    """out[M,N] (bf16) = epilogue((a[M,K] @ w[N,K]^T) * a_scale[m] * w_scale[n]); a, w e4m3 with fp32 per-row scales (as
+    quant_rows_fp8 makes them).  a/out may be row-strided 2-D views (stride(1)==1), K % 16 == 0."""
+    _req(a, FP8), _req(w, FP8), _req(a_scale, torch.float32), _req(w_scale, torch.float32)
+    M, K = a.shape
+    N = w.shape[0]
+    assert w.shape[1] == K and a.stride(1) == 1 and w.stride(1) == 1
+    assert a_scale.shape == (M,) and w_scale.shape == (N,) and a_scale.stride(0) == 1 and w_scale.stride(0) == 1
+    if out is None:
+        out = torch.empty(M, N, device=a.device, dtype=torch.bfloat16)
+    _req(out)
+    assert out.shape == (M, N) and out.stride(1) == 1
+    gs = gate.stride(0) if gate is not None else 0
+    _lib.check(_lib.lib().scail_gemm_fp8(
+        _ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(bias), _ptr(out), out.stride(0), M, N, K, epilogue,
+        _ptr(gate), gs, rows_per_batch, _ptr(residual), residual.stride(0) if residual is not None else 0, 0,
+        _ptr(a_scale), _ptr(w_scale), _stream()), "scail_gemm_fp8")
+    _count()
+    return out
+
+
+def quant_rows_fp8(x, q=None, scale=None):
+    """Row-wise e4m3: x bf16 [M, K] (row-strided 2-D view) -> (q e4m3 [M, K], scale fp32 [M]) with scale = amax(|row|) / 448
+    (1 for an all-zero row) and q = satfinite_rn(x / scale)."""
+    _req(x)
+    assert x.dim() == 2 and x.stride(1) == 1
+    M, K = x.shape
+    if q is None:
+        q = torch.empty(M, K, device=x.device, dtype=FP8)
+    if scale is None:
+        scale = torch.empty(M, device=x.device, dtype=torch.float32)
+    _req(q, FP8), _req(scale, torch.float32)
+    assert q.shape == (M, K) and q.is_contiguous() and scale.shape == (M,) and scale.is_contiguous()
+    _lib.check(_lib.lib().scail_quant_rows_fp8(_ptr(x), x.stride(0), _ptr(q), _ptr(scale), M, K, _stream()),
+               "scail_quant_rows_fp8")
+    _count()
+    return q, scale
+
+
+def ln_modulate(x, out=None, gamma=None, beta=None, shift=None, scale=None, eps=1e-6, rows_out=None, row_offset=0,
+                out_fp8=None):
+    """x [B, Nin, D] -> out [B, rows_out, D] = modulate(LN(x[:, row_offset:row_offset+rows_out])).
+    out_fp8=(q, s): write that result quantised instead, q e4m3 [B*rows_out, D] and s fp32 [B*rows_out] (bit for bit
+    quant_rows_fp8 of the bf16 result), and return (q, s)."""
     _req(x)
     B, n_in, D = x.shape
     rows_out = n_in if rows_out is None else rows_out
-    if out is None:
-        out = torch.empty(B, rows_out, D, device=x.device, dtype=torch.bfloat16)
-    assert x.is_contiguous() and out.is_contiguous()
+    assert x.is_contiguous()
     ms = shift.stride(0) if shift is not None else 0
     if shift is not None:
         assert shift.stride(-1) == 1 and scale.stride(-1) == 1 and scale.stride(0) == ms
+    if out_fp8 is not None:
+        assert out is None
+        q, s = out_fp8
+        _req(q, FP8), _req(s, torch.float32)
+        assert q.is_contiguous() and q.numel() == B * rows_out * D and s.is_contiguous() and s.numel() == B * rows_out
+        _lib.check(_lib.lib().scail_ln_modulate_fp8(_ptr(x), _ptr(q), _ptr(s), _ptr(gamma), _ptr(beta), _ptr(shift),
+                                                    _ptr(scale), ms, B, rows_out, n_in, row_offset, D, eps, _stream()),
+                   "scail_ln_modulate_fp8")
+        _count()
+        return out_fp8
+    if out is None:
+        out = torch.empty(B, rows_out, D, device=x.device, dtype=torch.bfloat16)
+    assert out.is_contiguous()
     _lib.check(_lib.lib().scail_ln_modulate(_ptr(x), _ptr(out), _ptr(gamma), _ptr(beta), _ptr(shift), _ptr(scale), ms,
                                             B, rows_out, n_in, row_offset, D, eps, _stream()), "scail_ln_modulate")
     _count()

@@ -123,10 +123,11 @@ class ContextParallel:
         return works
 
     # ---- the block's self-attention under CP (kernels) ----
-    def self_attention(self, mixin, attn, h2, B, n_local, d, H, wq, wk, cos, sin, ctx, tables_local=False):
+    def self_attention(self, mixin, attn, h2, B, n_local, d, H, wq, wk, cos, sin, ctx, tables_local=False, h_scale=None):
         """tables_local: cos/sin already describe this rank's tokens (engine-style pre-chunked latents whose RoPE offsets
         come from rope_H/W_shift); otherwise they cover the full sequence and this rank's contiguous slice is taken.
-        Keys/values are gathered in rank order either way (softmax is order-free)."""
+        Keys/values are gathered in rank order either way (softmax is order-free).  h2 e4m3 with row scales h_scale
+        (mixin.fp8_linear): the K, V and Q projections are fp8 GEMMs on row slices of the e4m3 QKV weight."""
         dev = h2.device
         P = self.size
         eps = mixin.layernorm_epsilon
@@ -140,23 +141,30 @@ class ContextParallel:
                                  "tokens must be sharded with shard_tokens() (or pass chunk_dim for pre-chunked latents)")
             cos_l, sin_l = self.rope_slice(cos, sin, n_local)
         w, bias = attn.query_key_value.weight, attn.query_key_value.bias
+        if h2.dtype == ops.FP8:
+            w8, ws8 = mixin.fp8_weight(attn.query_key_value)
+
+        def proj(rows, cols, out):  # out = h2[rows] @ w[cols]^T + bias[cols]; per-row scales slice with the rows
+            if h2.dtype == ops.FP8:
+                return ops.gemm_fp8(h2[rows], h_scale[rows], w8[cols], ws8[cols], bias[cols], out=out)
+            return ops.gemm(h2[rows], w[cols], bias[cols], out=out)
         # K and V travel separately so that the K gather is already in flight during the V (and Q) projection and the V gather
         # during the Q projection: with one CFG branch per rank (HybridParallel) there is no second stream to hide it behind
         kbuf = self.kv_buffer(B, n_local, d, dev, width=d, tag="k")
         vbuf = self.kv_buffer(B, n_local, d, dev, width=d, tag="v")
         for b in range(B):  # K projection + RMSNorm/RoPE straight into this rank's slot of the gather buffer
             slot = kbuf[b, self.rank]
-            ops.gemm(h2[b * n_local:(b + 1) * n_local], w[d:2 * d], bias[d:2 * d], out=slot)
+            proj(slice(b * n_local, (b + 1) * n_local), slice(d, 2 * d), slot)
             ops.rmsnorm_rope(slot, n_local, d, [(0, wk)], cos_l, sin_l, eps=eps)
         works = self.gather_kv(kbuf, async_op=True)
         for b in range(B):
-            ops.gemm(h2[b * n_local:(b + 1) * n_local], w[2 * d:], bias[2 * d:], out=vbuf[b, self.rank])
+            proj(slice(b * n_local, (b + 1) * n_local), slice(2 * d, 3 * d), vbuf[b, self.rank])
         works += self.gather_kv(vbuf, async_op=True)
         qkey = (B * n_local, d, str(dev), torch.cuda.current_stream(dev).cuda_stream)
         if qkey not in self._q:
             self._q[qkey] = torch.empty(B * n_local, d, device=dev, dtype=torch.bfloat16)
         q = self._q[qkey]
-        ops.gemm(h2, w[:d], bias[:d], out=q)  # overlaps the all-gathers
+        proj(slice(None), slice(0, d), q)  # overlaps the all-gathers
         ops.rmsnorm_rope(q, n_local, d, [(0, wq)], cos_l, sin_l, eps=eps)
         k2, v2 = kbuf.view(B * P * n_local, d), vbuf.view(B * P * n_local, d)
         if not self.local_first:

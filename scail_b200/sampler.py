@@ -139,7 +139,9 @@ class GraphedStep:
     captured ONCE in a CUDA graph and replayed per step: 3 host launches per step (timestep fill, graph replay, CFG+Euler)
     instead of ~780, and none of the reference's per-layer host syncs (sat/transformer_defaults.py:56-57) by construction.
     The latent `x`, the timestep vector and the conditioning tensors are static buffers owned by this object; results are
-    bit-identical to `sampler_step` (same kernels, same order).  Single-GPU path (NCCL collectives are not captured)."""
+    bit-identical to `sampler_step` (same kernels, same order).  Single-GPU path (NCCL collectives are not captured).
+    The graph runs in the `fp8_linear` mode of construction time.  With fp8 it reads the e4m3 weight copies in place: every
+    call first re-derives, into the same buffers, the copies of weights that changed since (e.g. after load_state_dict)."""
 
     def __init__(self, model, x, cond, uc, scale=4.0):
         if getattr(model.mixins["adaln_layer"], "cp", None) is not None:
@@ -152,6 +154,10 @@ class GraphedStep:
         self.kw = dict(y=None, ref_concat=cond["ref_concat"], concat_smpl_render=cond["concat_smpl_render"],
                        image_clip_features=cond["image_clip_features"], concat_images=cond.get("concat_images"))
         assert ops.ATTN_EVENTS is None, "event timing of individual launches cannot be captured"
+        self.adaln = model.mixins["adaln_layer"]
+        self.fp8 = getattr(self.adaln, "fp8_linear", False)
+        # the e4m3 weights are derived on this stream and held here: the graph replays against these very buffers
+        self._fp8_weights = self.adaln.prepare_fp8_weights() if self.fp8 else []
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():  # warm-up on the capture stream: workspaces and TMA descriptors exist
@@ -168,6 +174,8 @@ class GraphedStep:
         return self.model(torch.cat([self.x, self.x], 0), timesteps=self.ts, context=self.ctx, **self.kw).contiguous()
 
     def __call__(self, sigma, next_sigma):
+        if self.fp8:
+            self.adaln.prepare_fp8_weights()
         self.ts.fill_(float(sigma) * 1000.0)
         self.graph.replay()
         return ops.cfg_euler_(self.x, self.v, self.scale, float(next_sigma) - float(sigma))

@@ -21,3 +21,9 @@ timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$O
     > "$OUT/memcheck_gemm_tiles_pytest.log" 2>&1
 echo "sanitizer exit code $?" >> "$OUT/memcheck_gemm_tiles_pytest.log"
 tail -3 "$OUT/memcheck_gemm_tiles_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_gemm_tiles.log" | head -5
+# fp8 linears at small shapes: row quantiser, fp8 LayerNorm, fp8 GEMM (ragged tiles, gate rows, column slabs)
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$OUT/memcheck_fp8.log" \
+    python -m pytest tests/test_fp8_gpu.py -q -x --timeout 600 -k "ragged or gate_rows or column_slabs or refuses or small_model" \
+    > "$OUT/memcheck_fp8_pytest.log" 2>&1
+echo "sanitizer exit code $?" >> "$OUT/memcheck_fp8_pytest.log"
+tail -3 "$OUT/memcheck_fp8_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_fp8.log" | head -5
