@@ -85,6 +85,30 @@ int scail_ln_modulate_fp8(const void* x, void* out_q, float* out_scale, const vo
 int scail_rmsnorm_rope(void* buf, int64_t ld, int64_t rows, int64_t rows_per_batch, int64_t D, int nslabs,
                        int64_t col_offset0, const void* weight0, int64_t col_offset1, const void* weight1,
                        const float* cos, const float* sin, float eps, scail_stream_t stream);
+/* The same rows quantised for scail_attention_fp8 instead of written back: slab s goes to e4m3 rows q8_s [rows, ld8] with
+ * one float32 scale per (token, head) in s8_s, head-major [B, D/128, L_pad] where B = rows / rows_per_batch and the
+ * tokens [rows_per_batch, L_pad) are written as zeros.  Each 128-wide head of a token is one row of the e4m3 row format
+ * (scail_quant_rows_fp8), equal bit for bit to quantising what scail_rmsnorm_rope writes.  buf is read only.
+ * D % 128 == 0, ld8 % 16 == 0, rows_per_batch <= L_pad, L_pad % 128 == 0. */
+int scail_rmsnorm_rope_fp8(const void* buf, int64_t ld, int64_t rows, int64_t rows_per_batch, int64_t D, int nslabs,
+                           int64_t col_offset0, const void* weight0, int64_t col_offset1, const void* weight1,
+                           const float* cos, const float* sin, float eps, void* q8_0, float* s8_0, void* q8_1, float* s8_1,
+                           int64_t ld8, int64_t L_pad, scail_stream_t stream);
+
+/* V operand of scail_attention_fp8: V bf16 [B*L, H*head_dim] (column slab, leading dim ldv) -> vt e4m3 [B, H, 128, L_pad]
+ * (keys contiguous; inside every 16-key group logical column k holds key 2*((k%16)/4) + (k%2) + 8*((k%4)/2); zeros past L)
+ * and v_scale float32 [B, H, 128]: one e4m3 row-format scale per channel over the L keys.  amax_work: [B, H*128] 32-bit
+ * workspace, zeroed and used by this call.  head_dim must be 128, L <= L_pad, L_pad % 128 == 0. */
+int scail_quant_vt_fp8(const void* v, int64_t ldv, void* vt, float* v_scale, void* amax_work, int64_t B, int64_t H,
+                       int64_t head_dim, int64_t L, int64_t L_pad, scail_stream_t stream);
+
+/* FP8 (e4m3) self-attention, non-causal, softmax scale = scale, q_len == kv_len == L: Q, K e4m3 [B*L, H*128] with
+ * leading dims ldq/ldk and scales q_scale/k_scale [B, H, L_pad] (scail_rmsnorm_rope_fp8); vt/v_scale from
+ * scail_quant_vt_fp8.  out bf16 [B*L, ldo] (merged heads).  P = softmax numerator is quantised with the fixed scale 2^-8;
+ * Hopper fp8 MMAs are accumulated per 128-key tile and summed in fp32.  head_dim must be 128. */
+int scail_attention_fp8(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                        const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H, int64_t head_dim,
+                        int64_t L, int64_t L_pad, float scale, scail_stream_t stream);
 
 /* Flash attention, head_dim 128, bf16, non-causal, softmax scale = scale.  Q/K/V are column slabs
  * (head h at columns [h*128, h*128+128)) of row-major matrices with leading dims ldq/ldk/ldv; batch b

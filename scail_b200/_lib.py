@@ -30,6 +30,11 @@ SIGNATURES = {
     "scail_ln_modulate": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
     "scail_ln_modulate_fp8": [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
     "scail_rmsnorm_rope": [c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_f, c_p],
+    "scail_rmsnorm_rope_fp8": [c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_f, c_p, c_p, c_p,
+                               c_p, c_i64, c_i64, c_p],
+    "scail_quant_vt_fp8": [c_p, c_i64, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
+    "scail_attention_fp8": [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f,
+                            c_p],
     "scail_attention": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                         c_i64, c_i64, c_f, c_int, c_p],
     "scail_attention_partial": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,

@@ -453,7 +453,95 @@ int scail_rmsnorm_rope(void* buf, int64_t ld, int64_t rows, int64_t rows_per_bat
     p.nslabs = nslabs; p.D = (int)D; p.rows = (int)rows; p.rows_per_batch = (int)rows_per_batch;
     p.cos = cos; p.sin = sin; p.eps = eps;
     dim3 grid((unsigned)rows, nslabs);
-    rmsnorm_rope_kernel<<<grid, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    rmsnorm_rope_kernel<false><<<grid, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+int scail_rmsnorm_rope_fp8(const void* buf, int64_t ld, int64_t rows, int64_t rows_per_batch, int64_t D, int nslabs,
+                           int64_t col_offset0, const void* weight0, int64_t col_offset1, const void* weight1,
+                           const float* cos, const float* sin, float eps, void* q8_0, float* s8_0, void* q8_1, float* s8_1,
+                           int64_t ld8, int64_t L_pad, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(buf && weight0 && q8_0 && s8_0 && (nslabs == 1 || (nslabs == 2 && weight1 && q8_1 && s8_1)),
+                  "rmsnorm_rope_fp8: null operand");
+    SCAIL_REQUIRE(D % 128 == 0 && D <= ROW_MAXV * ROW_THREADS * 8, "rmsnorm_rope_fp8: D=%lld must be a multiple of the 128-wide head and <= %d",
+                  (long long)D, ROW_MAXV * ROW_THREADS * 8);
+    SCAIL_REQUIRE(ld % 8 == 0 && col_offset0 % 8 == 0 && col_offset1 % 8 == 0 && aligned16(buf), "rmsnorm_rope_fp8: bad ld/offset");
+    SCAIL_REQUIRE(ld8 % 16 == 0 && ld8 >= D && aligned16(q8_0) && aligned16(q8_1) && aligned4(s8_0) && aligned4(s8_1),
+                  "rmsnorm_rope_fp8: ld8 must be a multiple of 16 and >= D, q8 16-byte and s8 4-byte aligned");
+    SCAIL_REQUIRE(rows > 0 && rows_per_batch > 0 && rows % rows_per_batch == 0, "rmsnorm_rope_fp8: bad row counts");
+    SCAIL_REQUIRE(L_pad % 128 == 0 && rows_per_batch <= L_pad, "rmsnorm_rope_fp8: L_pad=%lld must be a multiple of 128 and >= L=%lld",
+                  (long long)L_pad, (long long)rows_per_batch);
+    SCAIL_REQUIRE((cos == nullptr) == (sin == nullptr), "rmsnorm_rope_fp8: cos/sin come in pairs");
+    RmsRopeParams p;
+    p.buf = const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(buf)); p.ld = ld;
+    p.col_offset[0] = (int)col_offset0; p.col_offset[1] = (int)col_offset1;
+    p.weight[0] = static_cast<const __nv_bfloat16*>(weight0); p.weight[1] = static_cast<const __nv_bfloat16*>(weight1);
+    p.nslabs = nslabs; p.D = (int)D; p.rows = (int)rows; p.rows_per_batch = (int)rows_per_batch;
+    p.cos = cos; p.sin = sin; p.eps = eps;
+    p.q8[0] = static_cast<uint8_t*>(q8_0); p.q8[1] = static_cast<uint8_t*>(q8_1);
+    p.s8[0] = s8_0; p.s8[1] = s8_1; p.ld8 = ld8; p.L_pad = (int)L_pad;
+    dim3 grid((unsigned)rows, nslabs);
+    rmsnorm_rope_kernel<true><<<grid, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_quant_vt_fp8(const void* v, int64_t ldv, void* vt, float* v_scale, void* amax_work, int64_t B, int64_t H,
+                       int64_t head_dim, int64_t L, int64_t L_pad, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(v && vt && v_scale && amax_work, "quant_vt_fp8: null operand");
+    SCAIL_REQUIRE(head_dim == ATT_D, "quant_vt_fp8: head_dim=%lld, only 128 is supported", (long long)head_dim);
+    SCAIL_REQUIRE(B > 0 && H > 0 && L > 0 && L_pad % 128 == 0 && L <= L_pad,
+                  "quant_vt_fp8: bad shape B=%lld H=%lld L=%lld L_pad=%lld (L <= L_pad, L_pad %% 128 == 0)", (long long)B,
+                  (long long)H, (long long)L, (long long)L_pad);
+    SCAIL_REQUIRE(ldv % 8 == 0 && ldv >= H * ATT_D && aligned16(v) && aligned16(vt) && aligned4(v_scale) && aligned4(amax_work),
+                  "quant_vt_fp8: ldv must be a multiple of 8 and >= H*128, v and vt 16-byte aligned, v_scale and amax_work 4-byte aligned");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int D = (int)(H * ATT_D);
+    SCAIL_CHECK_CUDA(cudaMemsetAsync(amax_work, 0, sizeof(unsigned) * B * D, st));
+    dim3 ga(blocks_for(L, VT_AMAX_ROWS), (unsigned)B, blocks_for(D, 128 * 8));
+    quant_vt_amax_kernel<<<ga, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(v), ldv, static_cast<unsigned*>(amax_work),
+                                             (int)L, D);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    dim3 gt((unsigned)(L_pad / VT_KEYS), (unsigned)H, (unsigned)B);
+    quant_vt_fp8_kernel<<<gt, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(v), ldv, static_cast<const unsigned*>(amax_work),
+                                            static_cast<uint8_t*>(vt), v_scale, (int)L, (int)L_pad, (int)H);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_attention_fp8(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                        const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H, int64_t head_dim,
+                        int64_t L, int64_t L_pad, float scale, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(Q && q_scale && K && k_scale && vt && v_scale && out, "attention_fp8: null operand");
+    SCAIL_REQUIRE(head_dim == ATT_D, "attention_fp8: head_dim=%lld, only 128 is supported", (long long)head_dim);
+    SCAIL_REQUIRE(B > 0 && H > 0 && L > 0 && L_pad % 128 == 0 && L <= L_pad,
+                  "attention_fp8: bad shape B=%lld H=%lld L=%lld L_pad=%lld (L <= L_pad, L_pad %% 128 == 0)", (long long)B,
+                  (long long)H, (long long)L, (long long)L_pad);
+    SCAIL_REQUIRE(ldq % 16 == 0 && ldk % 16 == 0 && ldq >= H * ATT_D && ldk >= H * ATT_D && ldo % 8 == 0 && ldo >= H * ATT_D,
+                  "attention_fp8: ldq and ldk must be multiples of 16, ldo of 8, all >= H*128");
+    SCAIL_REQUIRE(aligned16(Q) && aligned16(K) && aligned16(vt) && aligned16(out) && aligned16(k_scale) && aligned4(q_scale) &&
+                      (reinterpret_cast<uintptr_t>(v_scale) & 7) == 0,
+                  "attention_fp8: Q, K, vt, out and k_scale must be 16-byte aligned, v_scale 8-byte, q_scale 4-byte");
+    CUtensorMap tq, tk, tv;
+    int rc;
+    const uint64_t cols = (uint64_t)H * ATT_D;
+    if ((rc = make_tmap_2d(Q, B * L, cols, ldq, ATT_BQ, 128, &tq, 1))) return rc;
+    if ((rc = make_tmap_2d(K, B * L, cols, ldk, ATT_BKV, 128, &tk, 1))) return rc;
+    if ((rc = make_tmap_2d(vt, B * H * ATT_D, L_pad, L_pad, ATT_D, 128, &tv, 1))) return rc;
+    Attn8Params p;
+    p.out = static_cast<__nv_bfloat16*>(out); p.ldo = ldo;
+    p.q_scale = q_scale; p.k_scale = k_scale; p.v_scale = v_scale;
+    p.L = (int)L; p.L_pad = (int)L_pad; p.heads = (int)H;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    if ((rc = set_smem(attention_fp8_kernel, ATT8_SMEM_BYTES))) return rc;
+    dim3 grid((unsigned)(L_pad / ATT_BQ), (unsigned)H, (unsigned)B);
+    attention_fp8_kernel<<<grid, ATT_THREADS, ATT8_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(tq, tk, tv, p);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -234,6 +234,234 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     }
 }
 
+// ================================================================================================================
+// FP8 (e4m3) self-attention (q_len == kv_len == L), opt-in.  Operands, as rmsnorm_rope_kernel<true> and quant_vt_fp8_kernel
+// write them (the e4m3 row format of rowops.cuh: s = amax / 448, q = satfinite_rn(x / s), s = 1 for a zero row):
+//   Q, K : e4m3 [B*L, ld] (head h = columns h*128..), one fp32 scale per (token, head): head-major [B, H, L_pad]
+//   V^T  : e4m3 [B, H, 128, L_pad] (keys contiguous, permuted inside every 16-key group by fp8_vt_key, zero past L),
+//          one fp32 scale per (batch, head, channel) over all L keys: [B, H, 128]
+//   P    : fixed scale, P^ = e4m3(2^8 * exp2(s - m_running)); the 2^8 is the +8 in the exp2 argument.  l sums the fp32 values.
+// Same roles as attention_fwd_kernel: a TMA producer warp and two consumer warpgroups of 64 query rows; one CTA per 128
+// query rows of one (batch, head).  Every Q / K / V^T tile is one 128 x 128-byte SWIZZLE_128B box (16 KB).
+//   S = Q K^T : wgmma m64n128k32 e4m3 x 4 (descriptor +2 per k32 step); S *= K scale per column, then the bf16 kernel's
+//               online softmax with the row's Q scale folded into scale_log2.
+//   O_t = P^ V^ : wgmma m64n128k32 x 4 with A = P^ from registers into a fresh accumulator (Hopper's fp8 wgmma keeps ~14
+//               accumulator bits), then O = O * alpha + O_t in fp32.
+// P^ as the A operand without shuffles: a thread holds S columns {2q, 2q+1, 8+2q, 9+2q, ...} of each 32-key group but the
+// A fragment wants k = 4q..4q+3 (wgmma_rs_e4m3).  So the reduction is reindexed instead of the data: register a[0] of key
+// group g packs S columns 32g + {2q, 2q+1, 8+2q, 9+2q}, and V^T column k holds key fp8_vt_key(k), the inverse relabelling.
+constexpr int ATT8_STAGES = 4;
+constexpr int ATT8_TILE_BYTES = 128 * 128;  // 16 KB: one e4m3 tile
+constexpr int ATT8_KS_BYTES = ATT_BKV * 4;  // the K tile's 128 fp32 scales
+constexpr int ATT8_SMEM_BYTES = (1 + 2 * ATT8_STAGES) * ATT8_TILE_BYTES + ATT8_STAGES * ATT8_KS_BYTES + 1024 + 256;
+static_assert(ATT8_SMEM_BYTES <= 232448, "attention_fp8: shared memory budget");
+
+// the key stored at logical column k of V^T (a permutation inside every 16-key group)
+__host__ __device__ __forceinline__ int fp8_vt_key(int k) {
+    return 16 * (k / 16) + 2 * ((k % 16) / 4) + (k % 2) + 8 * ((k % 4) / 2);
+}
+
+struct Attn8Params {
+    __nv_bfloat16* out;  // [B*L, ldo] bf16, head h at columns [h*128, h*128+128)
+    int64_t ldo;
+    const float* q_scale;   // [B, H, L_pad]
+    const float* k_scale;   // [B, H, L_pad]
+    const float* v_scale;   // [B, H, 128]
+    int L, L_pad, heads;
+    float scale_log2;       // softmax scale * log2(e)
+};
+
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                     const __grid_constant__ CUtensorMap tmap_vt, const Attn8Params p) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    const uint32_t q_smem = smem_base;
+    const uint32_t k_smem = q_smem + ATT8_TILE_BYTES;
+    const uint32_t v_smem = k_smem + ATT8_STAGES * ATT8_TILE_BYTES;
+    const uint32_t ks_smem = v_smem + ATT8_STAGES * ATT8_TILE_BYTES;
+    const uint32_t bar_base = ks_smem + ATT8_STAGES * ATT8_KS_BYTES;
+    enum {
+        B_QFULL = 0,
+        B_KFULL = 1,
+        B_KEMPTY = B_KFULL + ATT8_STAGES,
+        B_VFULL = B_KEMPTY + ATT8_STAGES,
+        B_VEMPTY = B_VFULL + ATT8_STAGES,
+        B_COUNT = B_VEMPTY + ATT8_STAGES
+    };
+    static_assert(8 * B_COUNT <= 256, "attention_fp8: barrier area");
+    auto bar = [&](int i) { return bar_base + 8u * i; };
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int head = blockIdx.y;
+    const int batch = blockIdx.z;
+    const int q0 = blockIdx.x * ATT_BQ;
+    const int n_kv = (p.L + ATT_BKV - 1) / ATT_BKV;
+    const int64_t bh = static_cast<int64_t>(batch) * p.heads + head;
+
+    if (warp == 0 && lane == 0) {
+        tma_prefetch_desc(&tmap_q);
+        tma_prefetch_desc(&tmap_k);
+        tma_prefetch_desc(&tmap_vt);
+        mbar_init(bar(B_QFULL), 1);
+        for (int s = 0; s < ATT8_STAGES; ++s) {
+            mbar_init(bar(B_KFULL + s), 1);
+            mbar_init(bar(B_KEMPTY + s), 2);  // one arrive per consumer warpgroup
+            mbar_init(bar(B_VFULL + s), 1);
+            mbar_init(bar(B_VEMPTY + s), 2);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        // ===================== TMA producer =====================
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
+            const int col = head * ATT_D;
+            const int row0 = batch * p.L;
+            mbar_expect_tx(bar(B_QFULL), ATT8_TILE_BYTES);
+            tma_load_2d(q_smem, &tmap_q, bar(B_QFULL), col, row0 + q0);
+            const float* ks = p.k_scale + bh * p.L_pad;
+            for (int j = 0; j < n_kv; ++j) {
+                const int s = j % ATT8_STAGES;
+                const uint32_t par = ((j / ATT8_STAGES) & 1) ^ 1;
+                mbar_wait(bar(B_KEMPTY + s), par, 10);
+                mbar_expect_tx(bar(B_KFULL + s), ATT8_TILE_BYTES + ATT8_KS_BYTES);
+                tma_load_2d(k_smem + s * ATT8_TILE_BYTES, &tmap_k, bar(B_KFULL + s), col, row0 + j * ATT_BKV);
+                bulk_load_1d(ks_smem + s * ATT8_KS_BYTES, ks + j * ATT_BKV, ATT8_KS_BYTES, bar(B_KFULL + s));
+                mbar_wait(bar(B_VEMPTY + s), par, 11);
+                mbar_expect_tx(bar(B_VFULL + s), ATT8_TILE_BYTES);
+                tma_load_2d(v_smem + s * ATT8_TILE_BYTES, &tmap_vt, bar(B_VFULL + s), j * ATT_BKV, static_cast<int>(bh * ATT_D));
+            }
+        }
+    } else {
+        // ===================== consumer warpgroups =====================
+        setmaxnreg_inc<232>();
+        const int wg = (warp >> 2) - 1;
+        const int t = threadIdx.x & 127;
+        const bool releaser = t == 0;
+        const int quad = t & 3;
+        const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);  // rows r0, r0 + 8 of the CTA's 128
+        float sl2[2];  // scale_log2 * Q scale of the two rows (rows past L read the zero-filled padding: masked at the end)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) sl2[h] = p.scale_log2 * p.q_scale[bh * p.L_pad + q0 + r0 + 8 * h];
+        float m_run[2] = {-INFINITY, -INFINITY};
+        float l_run[2] = {0.f, 0.f};
+        float o[ATT_D / 2];
+#pragma unroll
+        for (int i = 0; i < ATT_D / 2; ++i) o[i] = 0.f;
+        const uint64_t q_desc = wgmma_desc_kmajor_sw128(q_smem + wg * (64 * 128));
+        mbar_wait(bar(B_QFULL), 0, 20);
+#pragma unroll 1
+        for (int j = 0; j < n_kv; ++j) {
+            const int s = j % ATT8_STAGES;
+            const uint32_t par = (j / ATT8_STAGES) & 1;
+            const int valid = min(ATT_BKV, p.L - j * ATT_BKV);
+            // ---- S = Q K^T ----
+            float sc[ATT_BKV / 2];
+            mbar_wait(bar(B_KFULL + s), par, 21);
+            const uint64_t k_desc = wgmma_desc_kmajor_sw128(k_smem + s * ATT8_TILE_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_ss_e4m3<ATT_BKV>(sc, q_desc + 2 * k, k_desc + 2 * k, k != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(sc);
+            // K scales of this thread's columns 8c + 2 quad + {0, 1}
+            const uint32_t ksa = ks_smem + s * ATT8_KS_BYTES + 8 * quad;
+#pragma unroll
+            for (int c = 0; c < ATT_BKV / 8; ++c) {
+                const float2 ksc = lds_f2(ksa + 32 * c);
+                sc[4 * c] *= ksc.x;
+                sc[4 * c + 1] *= ksc.y;
+                sc[4 * c + 2] *= ksc.x;
+                sc[4 * c + 3] *= ksc.y;
+            }
+            if (releaser) mbar_arrive(bar(B_KEMPTY + s));
+            if (valid < ATT_BKV) {
+#pragma unroll
+                for (int c = 0; c < ATT_BKV / 8; ++c) {
+                    const int col = 8 * c + 2 * quad;
+                    if (col >= valid) { sc[4 * c] = -INFINITY; sc[4 * c + 2] = -INFINITY; }
+                    if (col + 1 >= valid) { sc[4 * c + 1] = -INFINITY; sc[4 * c + 3] = -INFINITY; }
+                }
+            }
+            float alpha[2], neg_m[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int c = 0; c < ATT_BKV / 8; ++c) mx = fmaxf(mx, fmaxf(sc[4 * c + 2 * h], sc[4 * c + 2 * h + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                const float m_new = fmaxf(m_run[h], mx * sl2[h]);  // sl2 > 0: the max commutes with the scaling
+                alpha[h] = fast_exp2(m_run[h] - m_new);
+                m_run[h] = m_new;
+                l_run[h] *= alpha[h];
+                neg_m[h] = 8.0f - m_new;  // P^ = 2^8 exp2(s - m)
+            }
+            // P^ as e4m3 A fragments, one set of 4 registers per 32-key group g: a[0] = row r0, S columns 32g + {2q, 2q+1,
+            // 8+2q, 9+2q} = sc[16g + {0, 1, 4, 5}]; a[1] = row r0 + 8 (sc[16g + {2, 3, 6, 7}]); a[2], a[3]: the same + 8 sc
+            uint32_t pa[ATT_BKV / 32][4];
+#pragma unroll
+            for (int g = 0; g < ATT_BKV / 32; ++g) {
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    const int b0 = 16 * g + 8 * (r >> 1) + 2 * (r & 1);  // sc index of the first of the four values
+                    const int h = r & 1;
+                    float e[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        e[i] = fast_exp2(fmaf(sc[b0 + (i & 1) + 4 * (i >> 1)], sl2[h], neg_m[h]));
+                        l_run[h] += e[i];
+                    }
+                    pa[g][r] = pack_e4m3x4(e[0], e[1], e[2], e[3]);
+                }
+            }
+            // ---- O_t = P^ V^ (fresh accumulator), O = O * alpha + O_t ----
+            float ot[ATT_D / 2];
+            mbar_wait(bar(B_VFULL + s), par, 22);
+            const uint64_t v_desc = wgmma_desc_kmajor_sw128(v_smem + s * ATT8_TILE_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int g = 0; g < ATT_BKV / 32; ++g) wgmma_rs_e4m3<ATT_D>(ot, pa[g], v_desc + 2 * g, g != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(ot);
+            if (releaser) mbar_arrive(bar(B_VEMPTY + s));
+#pragma unroll
+            for (int c = 0; c < ATT_D / 8; ++c) {
+                o[4 * c] = fmaf(o[4 * c], alpha[0], ot[4 * c]);
+                o[4 * c + 1] = fmaf(o[4 * c + 1], alpha[0], ot[4 * c + 1]);
+                o[4 * c + 2] = fmaf(o[4 * c + 2], alpha[1], ot[4 * c + 2]);
+                o[4 * c + 3] = fmaf(o[4 * c + 3], alpha[1], ot[4 * c + 3]);
+            }
+        }
+        // ---- epilogue: O * s_v[channel] / l -> bf16 ----
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+            l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+        }
+        const float* vs = p.v_scale + bh * ATT_D + 2 * quad;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int qi = q0 + r0 + 8 * h;
+            if (qi >= p.L) continue;
+            const float inv_l = 1.0f / l_run[h];
+            __nv_bfloat16* dst = p.out + (static_cast<int64_t>(batch) * p.L + qi) * p.ldo + head * ATT_D + 2 * quad;
+#pragma unroll
+            for (int c = 0; c < ATT_D / 8; ++c) {
+                const float2 sv = *reinterpret_cast<const float2*>(vs + 8 * c);
+                *reinterpret_cast<uint32_t*>(dst + 8 * c) =
+                    pack_bf16(o[4 * c + 2 * h] * sv.x * inv_l, o[4 * c + 2 * h + 1] * sv.y * inv_l);
+            }
+        }
+    }
+}
+
 // Combine two partial attention results over disjoint key sets (context parallelism: local shard first, remote shards once
 // the all-gather has landed).  Each partial is normalised by its own row sum l and carries (m, l) with m in log2 units:
 //   out = (w_a O_a + w_b O_b) / (w_a + w_b),  w_x = l_x 2^(m_x - max(m_a, m_b)).   One warp per (row, head).

@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_fp8.h>
 
+#include "attention.cuh"  // ATT_D and fp8_vt_key (the V^T pre-pass)
 #include "sm90.cuh"
 
 namespace scail {
@@ -237,10 +238,20 @@ struct RmsRopeParams {
     const float* cos;     // optional [rows_per_batch, 128] fp32 tables (token = row % rows_per_batch)
     const float* sin;
     float eps;
+    // fp8 form (rmsnorm_rope_kernel<true>): slab s goes to e4m3 rows q8[s] [rows, ld8] (buf is not written) with one fp32
+    // scale per (token, head) in s8[s], head-major [B, H, L_pad] (rows_per_batch = L tokens; [L, L_pad) written as zeros)
+    uint8_t* q8[2];
+    float* s8[2];
+    int64_t ld8;
+    int L_pad;
 };
 
 // RMSNorm over the full hidden width (dit_video_crossattn_sc_xc.py:61-68, F5) fused with the
 // interleaved-pair 3-D RoPE (:336-340, :525-645).  grid.y selects the slab (q / k).
+// FP8: the bf16 row the bf16 form would write is quantised per 128-wide head (the e4m3 row format above, one row = one head of
+// one token), so the result equals quant_rows_fp8 of the bf16 form's heads bit for bit.  A head's 16 vectors are held by 16
+// consecutive lanes (D % 128 == 0), so its amax is four shuffles.
+template <bool FP8>
 __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_rope_kernel(const RmsRopeParams p) {
     __shared__ float red[4];
     const int row = blockIdx.x;
@@ -279,6 +290,7 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_rope_kernel(const RmsRope
     const float rstd = rsqrtf(row_block_sum(hsum_f32x2(acc), red) / p.D + p.eps);
     const uint64_t rstd2 = pack_f32x2(rstd, rstd);
     const __nv_bfloat16* wgt = slab ? p.weight[1] : p.weight[0];  // (a dynamic index would spill the param arrays to local memory)
+    [[maybe_unused]] uint4 ob[ROW_MAXV];  // fp8: the bf16 row, kept for the quantisation
 #pragma unroll
     for (int j = 0; j < ROW_MAXV; ++j) {
         const int i = j * ROW_THREADS + threadIdx.x;
@@ -296,9 +308,110 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_rope_kernel(const RmsRope
                 }
                 ow[k] = f32x2_to_bf16x2(y);
             }
-            xin[i] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+            if constexpr (FP8) ob[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+            else xin[i] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
         }
     }
+    if constexpr (FP8) {
+        uint8_t* q8 = (slab ? p.q8[1] : p.q8[0]) + static_cast<int64_t>(row) * p.ld8;
+        float* s8 = slab ? p.s8[1] : p.s8[0];
+        const int b = row / p.rows_per_batch, tok = row - b * p.rows_per_batch;
+        const int heads = p.D >> 7;
+#pragma unroll
+        for (int j = 0; j < ROW_MAXV; ++j) {
+            const int i = j * ROW_THREADS + threadIdx.x;
+            // all lanes shuffle (a lane past the row contributes 0); the 16 lanes of a head are all in or all out
+            float amax = 0.f;
+            if (i < nvec) amax = absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(0.f, ob[j].x), ob[j].y), ob[j].z), ob[j].w);
+#pragma unroll
+            for (int o = 1; o < 16; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+            if (i < nvec) {
+                const float s = fp8_row_scale(amax);
+                reinterpret_cast<uint2*>(q8)[i] = quant_bf16x8(ob[j], s);
+                if ((i & 15) == 0) {
+                    float* sh = s8 + (static_cast<int64_t>(b) * heads + (i >> 4)) * p.L_pad;
+                    sh[tok] = s;
+                    for (int pad = p.rows_per_batch + tok; pad < p.L_pad; pad += p.rows_per_batch) sh[pad] = 0.f;
+                }
+            }
+        }
+    }
+}
+
+// ---- V^T pre-pass of the fp8 self-attention (attention_fp8_kernel): V [B*L, H*128] bf16 (a column slab, row pitch ldv) ->
+// V^T e4m3 [B, H, 128, L_pad] with one scale per (batch, channel) over the L keys, keys permuted by fp8_vt_key inside every
+// 16-key group, zeros at keys >= L.  Two launches after a memset of `amax` ([B, H*128] fp32 bits):
+//   quant_vt_amax_kernel : per-channel amax by atomicMax on the bits of non-negative floats (order-independent: deterministic);
+//   quant_vt_fp8_kernel  : scale = amax / 448 (1 for an all-zero channel), tiled transpose + quantisation.
+constexpr int VT_AMAX_ROWS = 256;  // tokens per block of the amax pass
+
+__global__ void __launch_bounds__(128) quant_vt_amax_kernel(const __nv_bfloat16* v, int64_t ldv, unsigned* amax, int L, int D) {
+    const int b = blockIdx.y;
+    const int col = (blockIdx.z * 128 + threadIdx.x) * 8;
+    if (col >= D) return;
+    const int r0 = blockIdx.x * VT_AMAX_ROWS, r1 = min(L, r0 + VT_AMAX_ROWS);
+    float m[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const __nv_bfloat16* src = v + (static_cast<int64_t>(b) * L) * ldv + col;
+    for (int r = r0; r < r1; ++r) {
+        const uint4 x = *reinterpret_cast<const uint4*>(src + static_cast<int64_t>(r) * ldv);
+        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float2 f = unpack_bf16(w[k]);
+            m[2 * k] = fmaxf(m[2 * k], fabsf(f.x));
+            m[2 * k + 1] = fmaxf(m[2 * k + 1], fabsf(f.y));
+        }
+    }
+    unsigned* dst = amax + static_cast<int64_t>(b) * D + col;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) atomicMax(dst + k, __float_as_uint(m[k]));
+}
+
+constexpr int VT_KEYS = 64;  // keys per block of the transpose pass
+
+// grid (L_pad / 64, H, B), 256 threads: 64 keys x 128 channels of one head through shared memory
+__global__ void __launch_bounds__(256) quant_vt_fp8_kernel(const __nv_bfloat16* v, int64_t ldv, const unsigned* amax,
+                                                            uint8_t* vt, float* v_scale, int L, int L_pad, int H) {
+    __shared__ __nv_bfloat16 tile[VT_KEYS][ATT_D + 8];
+    __shared__ float sc[ATT_D];
+    const int h = blockIdx.y, b = blockIdx.z;
+    const int k0 = blockIdx.x * VT_KEYS;
+    const int64_t bh = static_cast<int64_t>(b) * H + h;
+    if (threadIdx.x < ATT_D) {
+        const float s = fp8_row_scale(__uint_as_float(amax[static_cast<int64_t>(b) * H * ATT_D + h * ATT_D + threadIdx.x]));
+        sc[threadIdx.x] = s;
+        if (blockIdx.x == 0) v_scale[bh * ATT_D + threadIdx.x] = s;
+    }
+    // load: 64 keys x 16 vectors of 8 channels, 4 per thread
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+        const int idx = it * 256 + threadIdx.x;
+        const int key = idx >> 4, vec = idx & 15;
+        uint4 x = make_uint4(0u, 0u, 0u, 0u);
+        if (k0 + key < L) x = *reinterpret_cast<const uint4*>(v + (static_cast<int64_t>(b) * L + k0 + key) * ldv + h * ATT_D + vec * 8);
+        *reinterpret_cast<uint4*>(&tile[key][vec * 8]) = x;
+    }
+    __syncthreads();
+    // store: channel c = thread / 2, logical keys [32 (thread % 2), +32) of the tile as two 16-byte vectors
+    const int c = threadIdx.x >> 1, half = threadIdx.x & 1;
+    const float s = sc[c];
+    uint4 out[2];
+    uint32_t* ow = reinterpret_cast<uint32_t*>(out);
+#pragma unroll
+    for (int w = 0; w < 8; ++w) {
+        float f[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int k = 32 * half + 4 * w + i;
+            f[i] = __fdiv_rn(__bfloat162float(tile[fp8_vt_key(k)][c]), s);
+        }
+        const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(f[0], f[1]), __NV_SATFINITE, __NV_E4M3);
+        const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(f[2], f[3]), __NV_SATFINITE, __NV_E4M3);
+        ow[w] = lo | (hi << 16);
+    }
+    uint4* dst = reinterpret_cast<uint4*>(vt + (bh * ATT_D + c) * L_pad + k0 + 32 * half);
+    dst[0] = out[0];
+    dst[1] = out[1];
 }
 
 // mod[b, i] = emb[b, i] + param[i]   (dit_video_crossattn_sc_xc.py:1025-1028, :823) fp32 add, one bf16 rounding

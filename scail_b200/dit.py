@@ -296,7 +296,7 @@ class AdaLNMixin(BaseMixin):
 
     def __init__(self, hidden_size, num_layers, time_embed_dim, compressed_num_frames, transformer_args, qk_ln=True,
                  qk_ln_affine=None, hidden_size_head=None, params_dtype=torch.float, device=torch.device("cpu"),
-                 elementwise_affine=True, share_adaln=False, use_i2v_clip=False, fp8_linear=False):
+                 elementwise_affine=True, share_adaln=False, use_i2v_clip=False, fp8_linear=False, fp8_attention=False):
         super().__init__()
         if not (qk_ln and share_adaln and use_i2v_clip) or hidden_size_head != hidden_size:
             raise NotImplementedError("scail_b200 implements qk_ln=True over the full hidden width, share_adaln=True, use_i2v_clip=True")
@@ -327,6 +327,9 @@ class AdaLNMixin(BaseMixin):
         # e4m3 weights are derived on the GPU on first use and are not part of the state_dict.  A plain attribute: it can be
         # toggled between forwards.
         self.fp8_linear = fp8_linear
+        # Opt-in, independent of fp8_linear: the self-attention runs on e4m3 Q, K (one scale per token and head) and V (one
+        # scale per channel) through attention_fp8_kernel; cross-attention stays bf16.  A plain attribute, like fp8_linear.
+        self.fp8_attention = fp8_attention
 
     # -- fp8 linears ---------------------------------------------------------------------------
     FP8_LINEARS = ("attention.query_key_value", "attention.dense", "cross_attention.query", "cross_attention.dense",
@@ -460,9 +463,13 @@ class AdaLNMixin(BaseMixin):
         if self.cp is None or self.cp.size == 1:
             qkv = _WS.get("qkv", (B * N, 3 * d), dev)
             self._linear(h2, a.query_key_value, _fp8_scale, out=qkv)
-            ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon)
-            ops.attention(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, N)
+            if self.fp8_attention:
+                self._self_attention_fp8(qkv, B, N, d, H, wq, wk, cos, sin, ctx)
+            else:
+                ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon)
+                ops.attention(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, N)
         else:
+            self._refuse_fp8_attention_cp()
             # engine-style sequence parallelism (diffusion_video.py:495-552): the latents arrive pre-chunked on H or W, so the
             # RoPE tables built from rope_H/W_shift are already this rank's; otherwise tokens were sharded by shard_tokens()
             self.cp.self_attention(self, a, h2, B, N, d, H, wq, wk, cos, sin, ctx,
@@ -470,6 +477,23 @@ class AdaLNMixin(BaseMixin):
         if _ctx_out is not None:
             return None
         return self._linear(ctx, a.dense, name="ctx8").view(B, N, d)
+
+    def _self_attention_fp8(self, qkv, B, N, d, H, wq, wk, cos, sin, ctx):
+        """Self-attention of the fused QKV buffer in e4m3: RMSNorm+RoPE writes quantised Q and K, the V slab is transposed and
+        quantised per channel, then attention_fp8 writes the merged-head context into ctx.  Buffers: per-stream workspace."""
+        dev, f32 = qkv.device, torch.float32
+        Lp = ops.fp8_pad(N)
+        q8 = (_WS.get("q8", (B * N, d), dev, ops.FP8), _WS.get("q8_scale", (B, H, Lp), dev, f32))
+        k8 = (_WS.get("k8", (B * N, d), dev, ops.FP8), _WS.get("k8_scale", (B, H, Lp), dev, f32))
+        ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon, out_fp8=[q8, k8])
+        vt, vs = ops.quant_vt_fp8(qkv[:, 2 * d:], B, H, N, _WS.get("vt8", (B, H, 128, Lp), dev, ops.FP8),
+                                  _WS.get("vt8_scale", (B, H, 128), dev, f32), _WS.get("vt8_amax", (B, d), dev, torch.int32))
+        ops.attention_fp8(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N)
+
+    def _refuse_fp8_attention_cp(self):
+        if self.fp8_attention and self.cp is not None and self.cp.size > 1:
+            raise NotImplementedError("fp8_attention is not implemented under context parallelism (a ContextParallel of size "
+                                      f"{self.cp.size}); turn fp8_attention off or run without context parallelism")
 
     def cross_attention_forward(self, hidden_states, cross_attention_mask, encoder_outputs, _ctx_out=None, _fp8_scale=None,
                                 **kw_args):
@@ -544,7 +568,8 @@ class DiffusionTransformer(nn.Module):
                  latent_height=300, patch_size=(1, 2, 2), in_channels=20, out_channels=16, hidden_size=5120,
                  text_dim=4096, num_layers=40, num_attention_heads=40, elementwise_affine=False, time_freq_dim=256,
                  time_embed_dim=None, modules=None, share_adaln=True, use_SwiGLU=False, use_RMSNorm=False,
-                 layernorm_epsilon=1e-6, inner_hidden_size=None, use_i2v_clip=True, dtype="bf16", fp8_linear=False, **kwargs):
+                 layernorm_epsilon=1e-6, inner_hidden_size=None, use_i2v_clip=True, dtype="bf16", fp8_linear=False,
+                 fp8_attention=False, **kwargs):
         super().__init__()
         if use_SwiGLU or use_RMSNorm:
             raise NotImplementedError("SCAIL-14B uses the non-gated GELU-tanh MLP and LayerNorm (yaml:42-43)")
@@ -579,7 +604,8 @@ class DiffusionTransformer(nn.Module):
         self.add_mixin("patch_embed", ImagePatchEmbeddingMixin(in_channels, d, self.patch_size))
         self.add_mixin("adaln_layer", AdaLNMixin(d, num_layers, self.time_embed_dim, frames, targs, qk_ln=True,
                                                  qk_ln_affine=True, hidden_size_head=d, elementwise_affine=elementwise_affine,
-                                                 share_adaln=True, use_i2v_clip=True, fp8_linear=fp8_linear))
+                                                 share_adaln=True, use_i2v_clip=True, fp8_linear=fp8_linear,
+                                                 fp8_attention=fp8_attention))
         self.add_mixin("final_layer", FinalLayerMixin(d, self.time_embed_dim, self.patch_size, out_channels,
                                                       elementwise_affine, layernorm_epsilon, True))
         object.__setattr__(self.mixins["adaln_layer"], "_pos_embed", self.mixins["pos_embed"])
@@ -673,6 +699,7 @@ class DiffusionTransformer(nn.Module):
                   _xkv_layers=cond.xkv if cond is not None else None)
         ad = self.mixins["adaln_layer"]
         cp = ad.cp
+        ad._refuse_fp8_attention_cp()
         chunk_dim = kwargs.get("chunk_dim")
         if chunk_dim is not None:  # :1578-1585
             if cp is None or cp.size == 1:

@@ -124,12 +124,35 @@ def ln_modulate(x, out=None, gamma=None, beta=None, shift=None, scale=None, eps=
     return out
 
 
-def rmsnorm_rope(buf, rows_per_batch, D, slabs, cos=None, sin=None, eps=1e-6):
-    """In-place RMSNorm(+RoPE) on column slabs [(col_offset, weight), ...] of the 2-D bf16 matrix buf."""
+def fp8_pad(L):
+    """L_pad of the fp8 self-attention operands: L rounded up to the 128-key tile."""
+    return (L + 127) // 128 * 128
+
+
+def rmsnorm_rope(buf, rows_per_batch, D, slabs, cos=None, sin=None, eps=1e-6, out_fp8=None):
+    """In-place RMSNorm(+RoPE) on column slabs [(col_offset, weight), ...] of the 2-D bf16 matrix buf.
+    out_fp8=[(q8, s8) per slab]: write the result quantised instead (buf is left as it is) for attention_fp8: q8 e4m3
+    [rows, D] (2-D, stride(1)==1) and s8 fp32 [B, D/128, L_pad] (one scale per token and 128-wide head, zeros past
+    rows_per_batch); bit for bit quant_rows_fp8 of the bf16 result viewed as [rows * D/128, 128].  Returns out_fp8."""
     _req(buf)
     assert buf.dim() == 2 and buf.stride(1) == 1 and 1 <= len(slabs) <= 2
     (o0, w0) = slabs[0]
     (o1, w1) = slabs[1] if len(slabs) == 2 else (0, None)
+    if out_fp8 is not None:
+        assert len(out_fp8) == len(slabs)
+        rows = buf.shape[0]
+        q8s = [q for q, _ in out_fp8]
+        for q, s in out_fp8:
+            _req(q, FP8), _req(s, torch.float32)
+            assert q.dim() == 2 and q.shape == (rows, D) and q.stride(1) == 1 and q.stride(0) == q8s[0].stride(0)
+            assert s.is_contiguous() and s.shape == (rows // rows_per_batch, D // 128, s.shape[-1])
+        (qa, sa) = out_fp8[0]
+        (qb, sb) = out_fp8[1] if len(out_fp8) == 2 else (None, None)
+        _lib.check(_lib.lib().scail_rmsnorm_rope_fp8(
+            _ptr(buf), buf.stride(0), rows, rows_per_batch, D, len(slabs), o0, _ptr(w0), o1, _ptr(w1), _ptr(cos), _ptr(sin), eps,
+            _ptr(qa), _ptr(sa), _ptr(qb), _ptr(sb), qa.stride(0), sa.shape[-1], _stream()), "scail_rmsnorm_rope_fp8")
+        _count()
+        return out_fp8
     _lib.check(_lib.lib().scail_rmsnorm_rope(_ptr(buf), buf.stride(0), buf.shape[0], rows_per_batch, D, len(slabs),
                                              o0, _ptr(w0), o1, _ptr(w1), _ptr(cos), _ptr(sin), eps, _stream()),
                "scail_rmsnorm_rope")
@@ -152,6 +175,56 @@ def attention(q, k, v, out, B, H, q_len, kv_len, q_batch_rows=None, kv_batch_row
     _lib.check(_lib.lib().scail_attention(_ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
                                           out.stride(0), B, H, q_len, kv_len, q_batch_rows, kv_batch_rows, q.shape[0],
                                           k.shape[0], scale, 1 if accumulate else 0, _stream()), "scail_attention")
+    if ev is not None:
+        ev[1].record()
+        ATTN_EVENTS.append(ev)
+    _count()
+    return out
+
+
+def quant_vt_fp8(v, B, H, L, vt=None, scale=None, work=None):
+    """V operand of attention_fp8: v bf16 [B*L, H*128] (2-D row-strided view) -> (vt e4m3 [B, H, 128, L_pad], scale fp32
+    [B, H, 128]): Vt's rows are the channels over the keys in the e4m3 row format, zero past L, and inside every 16-key group
+    logical column k holds key 2*((k%16)//4) + k%2 + 8*((k%4)//2) (attention_fp8's P fragment order).  work: int32 [B, H*128] workspace (allocated when None)."""
+    _req(v)
+    assert v.dim() == 2 and v.stride(1) == 1 and v.shape == (B * L, H * 128)
+    Lp = fp8_pad(L)
+    if vt is None:
+        vt = torch.empty(B, H, 128, Lp, device=v.device, dtype=FP8)
+    if scale is None:
+        scale = torch.empty(B, H, 128, device=v.device, dtype=torch.float32)
+    if work is None:
+        work = torch.empty(B, H * 128, device=v.device, dtype=torch.int32)
+    _req(vt, FP8), _req(scale, torch.float32), _req(work, torch.int32)
+    assert vt.is_contiguous() and vt.shape == (B, H, 128, Lp) and scale.is_contiguous() and scale.shape == (B, H, 128)
+    assert work.is_contiguous() and work.numel() >= B * H * 128
+    _lib.check(_lib.lib().scail_quant_vt_fp8(_ptr(v), v.stride(0), _ptr(vt), _ptr(scale), _ptr(work), B, H, 128, L, Lp,
+                                             _stream()), "scail_quant_vt_fp8")
+    _count(2)
+    return vt, scale
+
+
+def attention_fp8(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, scale=None):
+    """FP8 self-attention (q_len == kv_len == L): q8/k8 e4m3 [B*L, H*128] (2-D row-strided) with scales [B, H, L_pad] as
+    rmsnorm_rope(out_fp8=...) writes them, (vt, v_scale) from quant_vt_fp8; out bf16 [B*L, H*128] merged heads."""
+    for t in (q8, k8):
+        _req(t, FP8)
+        assert t.dim() == 2 and t.stride(1) == 1 and t.shape == (B * L, H * 128)
+    Lp = fp8_pad(L)
+    for s in (q_scale, k_scale):
+        _req(s, torch.float32)
+        assert s.is_contiguous() and s.shape == (B, H, Lp)
+    _req(vt, FP8), _req(v_scale, torch.float32), _req(out)
+    assert vt.is_contiguous() and vt.shape == (B, H, 128, Lp) and v_scale.is_contiguous() and v_scale.shape == (B, H, 128)
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape == (B * L, H * 128)
+    scale = 1.0 / math.sqrt(128) if scale is None else scale
+    ev = None
+    if ATTN_EVENTS is not None and L > 1024:
+        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+        ev[0].record()
+    _lib.check(_lib.lib().scail_attention_fp8(_ptr(q8), q8.stride(0), _ptr(q_scale), _ptr(k8), k8.stride(0), _ptr(k_scale),
+                                              _ptr(vt), _ptr(v_scale), _ptr(out), out.stride(0), B, H, 128, L, Lp, scale,
+                                              _stream()), "scail_attention_fp8")
     if ev is not None:
         ev[1].record()
         ATTN_EVENTS.append(ev)

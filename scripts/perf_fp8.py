@@ -4,8 +4,8 @@ power limit.
   1. The six per-block GEMMs at b = 2, N = 27 904 (M = 55 808): our bf16 GEMM; our fp8 GEMM alone and together with the
      quantisation of its activation (quant_rows_fp8 for the out-projections and fc2, the fp8 LayerNorm for QKV, cross q
      and fc1, timed against the bf16 LayerNorm it replaces); torch._scaled_mm with row-wise scales on the same operands.
-  2. Sampler steps/s of the 40-block 14B model (bench.py's model and inputs) with fp8_linear on and off on the same
-     instance, and the rel-L2 of the fp8 CFG velocity against the bf16 one.
+  2. Sampler steps/s of the 40-block 14B model (bench.py's model and inputs) in four modes on the same instance (bf16,
+     fp8 linears, fp8 attention, both), and the rel-L2 of each mode's CFG velocity against the bf16 one.
 ITERS (default 20) launches per GEMM timing, REPS (default 2) alternating rounds, STEPS (default 2) timed sampler steps."""
 import json
 import os
@@ -114,11 +114,12 @@ def steps():
     uc = dict(crossattn=dv["context_uncond"])
     sig = sampler.make_flow_timesteps(50, 5.0)
     ad = m.mixins["adaln_layer"]
-    res, vel = {"bf16": [], "fp8": []}, {}
+    modes = {"bf16": (False, False), "fp8_linear": (True, False), "fp8_attention": (False, True), "fp8_both": (True, True)}
+    res, vel = {k: [] for k in modes}, {}
     with torch.no_grad():
         for rep in range(REPS):
-            for mode in ("bf16", "fp8"):
-                ad.fp8_linear = mode == "fp8"
+            for mode, (lin, att) in modes.items():
+                ad.fp8_linear, ad.fp8_attention = lin, att
                 vel[mode] = sampler.guided_velocity(m, dv["x"], float(sig[10]), cond, uc, 4.0)  # warm-up (fp8: quantises weights)
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
@@ -126,10 +127,10 @@ def steps():
                     sampler.sampler_step(m, dv["x"].clone(), sig[10 + i], sig[11 + i], cond, uc, 4.0)
                 torch.cuda.synchronize()
                 res[mode].append(round(STEPS / (time.perf_counter() - t0), 4))
-    v16, v8 = vel["bf16"].float(), vel["fp8"].float()
-    rel = float((v8 - v16).norm() / v16.norm())
+    v16 = vel["bf16"].float()
+    rel = {k: float((v.float() - v16).norm() / v16.norm()) for k, v in vel.items() if k != "bf16"}
     print(json.dumps({"sampler_steps_per_s": res, "steps_per_rep": STEPS,
-                      "velocity_rel_l2_fp8_vs_bf16": rel, "workload": "SCAIL-14B, 40 blocks, latent 21x64x64, CFG batch 2",
+                      "velocity_rel_l2_vs_bf16": rel, "workload": "SCAIL-14B, 40 blocks, latent 21x64x64, CFG batch 2",
                       **card()}), flush=True)
 
 

@@ -27,3 +27,10 @@ timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$O
     > "$OUT/memcheck_fp8_pytest.log" 2>&1
 echo "sanitizer exit code $?" >> "$OUT/memcheck_fp8_pytest.log"
 tail -3 "$OUT/memcheck_fp8_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_fp8.log" | head -5
+# fp8 self-attention at small shapes: RMSNorm+RoPE fp8 form, V^T pre-pass (padding keys), attention_fp8 (partial last tile)
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$OUT/memcheck_fp8_attention.log" \
+    python -m pytest tests/test_fp8_attention_gpu.py -q -x --timeout 600 \
+    -k "rmsnorm_rope_fp8 and 1000 or rmsnorm_rope_fp8 and 130 or quant_vt and not 48832 or against_fp32_and_chain and not 27904 or small_model or refuses" \
+    > "$OUT/memcheck_fp8_attention_pytest.log" 2>&1
+echo "sanitizer exit code $?" >> "$OUT/memcheck_fp8_attention_pytest.log"
+tail -3 "$OUT/memcheck_fp8_attention_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_fp8_attention.log" | head -5
