@@ -116,7 +116,7 @@ def lib():
     h.scail_last_error.argtypes = []
     for name, args in SIGNATURES.items():
         if _VARIANT and not hasattr(h, name):
-            continue  # experiment builds (scripts/build_variants.sh) may predate an entry point
+            continue  # experiment builds (scripts/ab_attention.sh) may predate an entry point
         fn = getattr(h, name)
         fn.argtypes = args
         fn.restype = c_int

@@ -10,7 +10,8 @@
 //   online softmax on the S fragments (a row lives in the 4 lanes of a quad), P rounded to bf16 in registers,
 //   O += P V  : wgmma m64n128k16 x 8 with A = P straight from registers (the S accumulator fragment IS the A-operand
 //               fragment of the next MMA) and B = the V tile read MN-major from its [kv, d] layout.
-// The two warpgroups run independently, so one's softmax overlaps the other's tensor-core work.
+// The two warpgroups take strict turns at the tensor cores (named barriers 1 and 2): a turn issues PV of the previous tile
+// and QK^T of the next, so one warpgroup's softmax always runs under the other's MMAs.
 #pragma once
 #include "sm90.cuh"
 
@@ -23,6 +24,7 @@ constexpr int ATT_STAGES = 2;
 constexpr int ATT_TILE_BYTES = 128 * 128 * 2;  // 32 KB: one 128x128 bf16 tile (two 64-column halves)
 constexpr int ATT_HALF_BYTES = ATT_TILE_BYTES / 2;
 constexpr int ATT_THREADS = 384;
+constexpr int ATT_TURN_BAR = 1;  // named barriers 1 and 2: the consumer warpgroups' MMA turns (attention_fwd_kernel)
 constexpr int ATT_SMEM_BYTES = (1 + 2 * ATT_STAGES) * ATT_TILE_BYTES + 1024 + 256;
 static_assert(ATT_SMEM_BYTES <= 232448, "attention: shared memory budget");
 
@@ -123,17 +125,12 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         float o[ATT_D / 2];
 #pragma unroll
         for (int i = 0; i < ATT_D / 2; ++i) o[i] = 0.f;
+        uint32_t pa[ATT_BKV / 16][4];  // P of the last softmaxed tile as bf16 A fragments, one set per 16-key MMA step
         const uint64_t q_desc = wgmma_desc_kmajor_sw128(q_smem + wg * (64 * 128));
         mbar_wait(bar(B_QFULL), 0, 20);
-#pragma unroll 1
-        for (int j = 0; j < n_kv; ++j) {
-            const int s = j % ATT_STAGES;
-            const uint32_t par = (j / ATT_STAGES) & 1;
-            const int valid = j < n_kv0 ? min(ATT_BKV, p.kv_len - j * ATT_BKV) : min(ATT_BKV, p.kv_len1 - (j - n_kv0) * ATT_BKV);
-            // ---- S = Q K^T ----
-            float sc[ATT_BKV / 2];
-            mbar_wait(bar(B_KFULL + s), par, 21);
-            const uint64_t k_desc = wgmma_desc_kmajor_sw128(k_smem + s * ATT_TILE_BYTES);
+        // S = Q K^T of tile j into sc (issued and committed, not waited for)
+        auto issue_qk = [&](int j, float(&sc)[ATT_BKV / 2]) {
+            const uint64_t k_desc = wgmma_desc_kmajor_sw128(k_smem + (j % ATT_STAGES) * ATT_TILE_BYTES);
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
@@ -141,10 +138,27 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
                 wgmma_ss<ATT_BKV>(sc, q_desc + off, k_desc + off, k != 0);
             }
             wgmma_commit();
+        };
+        // O += P V of tile j, waited for; the V stage is released
+        auto pv = [&](int j) {
+            const int s = j % ATT_STAGES;
+            const uint64_t v_desc = wgmma_desc_mnmajor_sw128(v_smem + s * ATT_TILE_BYTES, ATT_HALF_BYTES);
+            fence_regs(o);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < ATT_BKV / 16; ++k) wgmma_rs_tb<ATT_D>(o, pa[k], v_desc + k * (2048 >> 4));  // 16 kv rows = 2048 B
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(o);
+            if (releaser) mbar_arrive(bar(B_VEMPTY + s));
+        };
+        // waits for S of tile j, releases the K stage, then the online softmax: O *= alpha, P -> pa
+        // (thread: rows r = sc[4c + 0/1], r + 8 = sc[4c + 2/3], columns 8c + 2 quad + 0/1)
+        auto softmax = [&](int j, float(&sc)[ATT_BKV / 2]) {
+            const int valid = j < n_kv0 ? min(ATT_BKV, p.kv_len - j * ATT_BKV) : min(ATT_BKV, p.kv_len1 - (j - n_kv0) * ATT_BKV);
             wgmma_wait<0>();
             fence_regs(sc);
-            if (releaser) mbar_arrive(bar(B_KEMPTY + s));
-            // ---- online softmax (thread: rows r = sc[4c + 0/1], r + 8 = sc[4c + 2/3], columns 8c + 2 quad + 0/1) ----
+            if (releaser) mbar_arrive(bar(B_KEMPTY + j % ATT_STAGES));
             if (valid < ATT_BKV) {
 #pragma unroll
                 for (int c = 0; c < ATT_BKV / 8; ++c) {
@@ -174,7 +188,6 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
                 o[4 * c + 2] *= alpha[1];
                 o[4 * c + 3] *= alpha[1];
             }
-            uint32_t pa[ATT_BKV / 16][4];  // P as bf16 A fragments, one set of 4 registers per 16-key MMA step
 #pragma unroll
             for (int c = 0; c < ATT_BKV / 8; ++c) {
                 float e[4];
@@ -186,18 +199,40 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
                 pa[c >> 1][(c & 1) * 2] = pack_bf16(e[0], e[1]);
                 pa[c >> 1][(c & 1) * 2 + 1] = pack_bf16(e[2], e[3]);
             }
-            // ---- O += P V ----
-            mbar_wait(bar(B_VFULL + s), par, 22);
-            const uint64_t v_desc = wgmma_desc_mnmajor_sw128(v_smem + s * ATT_TILE_BYTES, ATT_HALF_BYTES);
-            fence_regs(o);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < ATT_BKV / 16; ++k) wgmma_rs_tb<ATT_D>(o, pa[k], v_desc + k * (2048 >> 4));  // 16 kv rows = 2048 B
-            wgmma_commit();
-            wgmma_wait<0>();
-            fence_regs(o);
-            if (releaser) mbar_arrive(bar(B_VEMPTY + s));
+        };
+        // Ping-pong: the two warpgroups take turns at the tensor cores.  Turn j of a warpgroup issues O += P V of tile j - 1,
+        // waits for it, issues S = Q K^T of tile j and passes the turn on; the softmax of tile j then runs while the other
+        // warpgroup's turn keeps the tensor cores busy.  Named barrier ATT_TURN_BAR + w is warpgroup w's turn: w waits on it
+        // (bar.sync) and the other warpgroup arrives on it (bar.arrive) when its own turn ends.  Warpgroup 0 takes turn 0
+        // without waiting and warpgroup 1's last turn passes nothing on, so both take n_kv + 1 turns (whether or not their
+        // rows are valid), every barrier phase sees exactly 256 threads and none is left pending at exit.  The host requires
+        // kv_len > 0, so n_kv >= 1.  The first and last turns are peeled rather than guarded inside one loop: a wgmma under
+        // a branch makes ptxas serialise all of them (C7518).  PV is waited for before QK^T is issued, so P (32 registers)
+        // and S (64) are never live together beside O (64): the schedule fits the 168 registers of the 384-thread bound.
+        const int turn_bar = ATT_TURN_BAR + wg, next_bar = ATT_TURN_BAR + (wg ^ 1);
+        {
+            float sc[ATT_BKV / 2];
+            mbar_wait(bar(B_KFULL), 0, 21);
+            if (wg == 1) named_bar_sync(turn_bar, 256);
+            issue_qk(0, sc);
+            named_bar_arrive(next_bar, 256);
+            softmax(0, sc);
         }
+#pragma unroll 1
+        for (int j = 1; j < n_kv; ++j) {
+            float sc[ATT_BKV / 2];
+            mbar_wait(bar(B_KFULL + j % ATT_STAGES), (j / ATT_STAGES) & 1, 21);
+            mbar_wait(bar(B_VFULL + (j - 1) % ATT_STAGES), ((j - 1) / ATT_STAGES) & 1, 22);
+            named_bar_sync(turn_bar, 256);
+            pv(j - 1);
+            issue_qk(j, sc);
+            named_bar_arrive(next_bar, 256);
+            softmax(j, sc);
+        }
+        mbar_wait(bar(B_VFULL + (n_kv - 1) % ATT_STAGES), ((n_kv - 1) / ATT_STAGES) & 1, 22);
+        named_bar_sync(turn_bar, 256);
+        pv(n_kv - 1);
+        if (wg == 0) named_bar_arrive(next_bar, 256);
         // ---- epilogue: O / l -> bf16 (or normalised fp32 partial + (m, l)) -> global ----
 #pragma unroll
         for (int h = 0; h < 2; ++h) {

@@ -300,5 +300,9 @@ __device__ __forceinline__ float gelu_tanh(float x) {
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// counts this warp's threads towards named barrier `id` without waiting for it (the waiting side calls named_bar_sync)
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 }  // namespace scail
