@@ -109,6 +109,12 @@ int scail_quant_vt_fp8(const void* v, int64_t ldv, void* vt, float* v_scale, voi
 int scail_attention_fp8(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
                         const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H, int64_t head_dim,
                         int64_t L, int64_t L_pad, float scale, scail_stream_t stream);
+/* Block-sparse form of scail_attention_fp8 (see scail_attention_sparse for the map).  Extra checks: kv_tile_ptr and
+ * kv_tile_idx non-NULL and 4-byte aligned, ceil(L/128) <= nnz <= ceil(L/128)^2. */
+int scail_attention_fp8_sparse(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                               const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H,
+                               int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
+                               const int32_t* kv_tile_idx, int64_t nnz, scail_stream_t stream);
 
 /* Flash attention, head_dim 128, bf16, non-causal, softmax scale = scale.  Q/K/V are column slabs
  * (head h at columns [h*128, h*128+128)) of row-major matrices with leading dims ldq/ldk/ldv; batch b
@@ -119,6 +125,16 @@ int scail_attention(const void* Q, int64_t ldq, const void* K, int64_t ldk, cons
                     int64_t ldo, int64_t B, int64_t H, int64_t q_len, int64_t kv_len, int64_t q_batch_rows,
                     int64_t kv_batch_rows, int64_t q_rows_total, int64_t kv_rows_total, float scale, int accumulate,
                     scail_stream_t stream);
+/* Block-sparse self-attention (q_len == kv_len), same arguments and kernel as scail_attention plus a CSR map of 128 x 128
+ * tiles shared by every (batch, head): query tile t (rows [128t, 128t + 128)) attends to exactly the keys of the key tiles
+ * kv_tile_idx[kv_tile_ptr[t] .. kv_tile_ptr[t + 1]) (keys [128k, 128k + 128) clipped to kv_len); kv_tile_ptr int32
+ * [ceil(q_len/128) + 1] from 0 to nnz, kv_tile_idx int32 [nnz].  Every row must be non-empty and strictly ascending with
+ * indices < ceil(kv_len/128): the host checks only the pointers, their alignment and ceil(q_len/128) <= nnz <=
+ * ceil(q_len/128) * ceil(kv_len/128); the contents are the caller's (scail_b200.ops.TileMap validates them). */
+int scail_attention_sparse(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, void* out,
+                           int64_t ldo, int64_t B, int64_t H, int64_t q_len, int64_t kv_len, int64_t q_batch_rows,
+                           int64_t kv_batch_rows, int64_t q_rows_total, int64_t kv_rows_total, float scale, int accumulate,
+                           const int32_t* kv_tile_ptr, const int32_t* kv_tile_idx, int64_t nnz, scail_stream_t stream);
 
 /* Context parallelism: attention over a SUBSET of the keys, to be merged later.  Keys are the rows
  * [kv_off0, kv_off0 + kv_len0) and (optionally, kv_len1 > 0) [kv_off1, kv_off1 + kv_len1) of every batch of kv_batch_rows rows

@@ -35,8 +35,12 @@ SIGNATURES = {
     "scail_quant_vt_fp8": [c_p, c_i64, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_attention_fp8": [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f,
                             c_p],
+    "scail_attention_fp8_sparse": [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                   c_f, c_p, c_p, c_i64, c_p],
     "scail_attention": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                         c_i64, c_i64, c_f, c_int, c_p],
+    "scail_attention_sparse": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
+                               c_i64, c_i64, c_f, c_int, c_p, c_p, c_i64, c_p],
     "scail_attention_partial": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                                 c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
     "scail_attention_merge": [c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_p],

@@ -514,9 +514,23 @@ int scail_quant_vt_fp8(const void* v, int64_t ldv, void* vt, float* v_scale, voi
     return 0;
 }
 
-int scail_attention_fp8(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
-                        const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H, int64_t head_dim,
-                        int64_t L, int64_t L_pad, float scale, scail_stream_t stream) {
+// Host checks of a block-sparse map (the contents live on the device: the Python wrapper validates them when it builds
+// the map).  `what` names the entry point in the message.
+static int check_tile_map(const char* what, const int32_t* kv_tile_ptr, const int32_t* kv_tile_idx, int64_t nnz, int64_t q_len,
+                          int64_t kv_len) {
+    SCAIL_REQUIRE(kv_tile_ptr && kv_tile_idx, "%s: null tile map", what);
+    SCAIL_REQUIRE(aligned4(kv_tile_ptr) && aligned4(kv_tile_idx), "%s: kv_tile_ptr and kv_tile_idx must be 4-byte aligned int32", what);
+    const int64_t n_q_tiles = (q_len + scail::ATT_BQ - 1) / scail::ATT_BQ, n_kv_tiles = (kv_len + scail::ATT_BKV - 1) / scail::ATT_BKV;
+    SCAIL_REQUIRE(nnz >= n_q_tiles && nnz <= n_q_tiles * n_kv_tiles,
+                  "%s: nnz=%lld must lie in [n_q_tiles, n_q_tiles * n_kv_tiles] = [%lld, %lld] (every row non-empty, no repeats)",
+                  what, (long long)nnz, (long long)n_q_tiles, (long long)(n_q_tiles * n_kv_tiles));
+    return 0;
+}
+
+static int attention_fp8_impl(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                              const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H,
+                              int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
+                              const int32_t* kv_tile_idx, scail_stream_t stream) {
     using namespace scail;
     SCAIL_REQUIRE(Q && q_scale && K && k_scale && vt && v_scale && out, "attention_fp8: null operand");
     SCAIL_REQUIRE(head_dim == ATT_D, "attention_fp8: head_dim=%lld, only 128 is supported", (long long)head_dim);
@@ -539,18 +553,42 @@ int scail_attention_fp8(const void* Q, int64_t ldq, const float* q_scale, const 
     p.q_scale = q_scale; p.k_scale = k_scale; p.v_scale = v_scale;
     p.L = (int)L; p.L_pad = (int)L_pad; p.heads = (int)H;
     p.scale_log2 = scale * 1.4426950408889634f;
-    if ((rc = set_smem(attention_fp8_kernel, ATT8_SMEM_BYTES))) return rc;
+    p.kv_tile_ptr = kv_tile_ptr; p.kv_tile_idx = kv_tile_idx;
     dim3 grid((unsigned)(L_pad / ATT_BQ), (unsigned)H, (unsigned)B);
-    attention_fp8_kernel<<<grid, ATT_THREADS, ATT8_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(tq, tk, tv, p);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (kv_tile_ptr) {
+        if ((rc = set_smem(attention_fp8_kernel<true>, ATT8_SMEM_BYTES))) return rc;
+        attention_fp8_kernel<true><<<grid, ATT_THREADS, ATT8_SMEM_BYTES, st>>>(tq, tk, tv, p);
+    } else {
+        if ((rc = set_smem(attention_fp8_kernel<false>, ATT8_SMEM_BYTES))) return rc;
+        attention_fp8_kernel<false><<<grid, ATT_THREADS, ATT8_SMEM_BYTES, st>>>(tq, tk, tv, p);
+    }
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int scail_attention_fp8(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                        const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H, int64_t head_dim,
+                        int64_t L, int64_t L_pad, float scale, scail_stream_t stream) {
+    return attention_fp8_impl(Q, ldq, q_scale, K, ldk, k_scale, vt, v_scale, out, ldo, B, H, head_dim, L, L_pad, scale, nullptr,
+                              nullptr, stream);
+}
+
+int scail_attention_fp8_sparse(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                               const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H,
+                               int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
+                               const int32_t* kv_tile_idx, int64_t nnz, scail_stream_t stream) {
+    int rc;
+    if ((rc = check_tile_map("attention_fp8_sparse", kv_tile_ptr, kv_tile_idx, nnz, L, L))) return rc;
+    return attention_fp8_impl(Q, ldq, q_scale, K, ldk, k_scale, vt, v_scale, out, ldo, B, H, head_dim, L, L_pad, scale,
+                              kv_tile_ptr, kv_tile_idx, stream);
 }
 
 static int attention_impl(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, void* out,
                           int64_t ldo, int64_t B, int64_t H, int64_t q_len, int64_t kv_off0, int64_t kv_len0, int64_t kv_off1,
                           int64_t kv_len1, int64_t q_batch_rows, int64_t kv_batch_rows, int64_t q_rows_total,
                           int64_t kv_rows_total, float scale, int accumulate, float* o32, int64_t ldo32, void* state,
-                          scail_stream_t stream) {
+                          const int32_t* kv_tile_ptr, const int32_t* kv_tile_idx, scail_stream_t stream) {
     using namespace scail;
     SCAIL_REQUIRE(Q && K && V && (out || o32), "attention: null operand");
     SCAIL_REQUIRE(B > 0 && H > 0 && q_len > 0 && kv_len0 > 0 && kv_len1 >= 0 && kv_off0 >= 0 && kv_off1 >= 0, "attention: bad shape");
@@ -574,9 +612,16 @@ static int attention_impl(const void* Q, int64_t ldq, const void* K, int64_t ldk
     p.o32 = o32; p.ldo32 = ldo32; p.state = static_cast<float2*>(state); p.heads = (int)H;
     p.scale_log2 = scale * 1.4426950408889634f;
     p.accumulate = accumulate;
-    if ((rc = set_smem(attention_fwd_kernel, ATT_SMEM_BYTES))) return rc;
+    p.kv_tile_ptr = kv_tile_ptr; p.kv_tile_idx = kv_tile_idx;
     dim3 grid(blocks_for(q_len, ATT_BQ), (unsigned)H, (unsigned)B);
-    attention_fwd_kernel<<<grid, ATT_THREADS, ATT_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(tq, tk, tv, p);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (kv_tile_ptr) {
+        if ((rc = set_smem(attention_fwd_kernel<true>, ATT_SMEM_BYTES))) return rc;
+        attention_fwd_kernel<true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, st>>>(tq, tk, tv, p);
+    } else {
+        if ((rc = set_smem(attention_fwd_kernel<false>, ATT_SMEM_BYTES))) return rc;
+        attention_fwd_kernel<false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, st>>>(tq, tk, tv, p);
+    }
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -586,7 +631,19 @@ int scail_attention(const void* Q, int64_t ldq, const void* K, int64_t ldk, cons
                     int64_t kv_batch_rows, int64_t q_rows_total, int64_t kv_rows_total, float scale, int accumulate,
                     scail_stream_t stream) {
     return attention_impl(Q, ldq, K, ldk, V, ldv, out, ldo, B, H, q_len, 0, kv_len, 0, 0, q_batch_rows, kv_batch_rows, q_rows_total,
-                          kv_rows_total, scale, accumulate, nullptr, 0, nullptr, stream);
+                          kv_rows_total, scale, accumulate, nullptr, 0, nullptr, nullptr, nullptr, stream);
+}
+
+int scail_attention_sparse(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, void* out,
+                           int64_t ldo, int64_t B, int64_t H, int64_t q_len, int64_t kv_len, int64_t q_batch_rows,
+                           int64_t kv_batch_rows, int64_t q_rows_total, int64_t kv_rows_total, float scale, int accumulate,
+                           const int32_t* kv_tile_ptr, const int32_t* kv_tile_idx, int64_t nnz, scail_stream_t stream) {
+    SCAIL_REQUIRE(q_len == kv_len, "attention_sparse: self-attention only (q_len=%lld != kv_len=%lld)", (long long)q_len,
+                  (long long)kv_len);
+    int rc;
+    if ((rc = check_tile_map("attention_sparse", kv_tile_ptr, kv_tile_idx, nnz, q_len, kv_len))) return rc;
+    return attention_impl(Q, ldq, K, ldk, V, ldv, out, ldo, B, H, q_len, 0, kv_len, 0, 0, q_batch_rows, kv_batch_rows, q_rows_total,
+                          kv_rows_total, scale, accumulate, nullptr, 0, nullptr, kv_tile_ptr, kv_tile_idx, stream);
 }
 
 int scail_attention_partial(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, float* o32,
@@ -595,7 +652,7 @@ int scail_attention_partial(const void* Q, int64_t ldq, const void* K, int64_t l
                             int64_t kv_rows_total, float scale, scail_stream_t stream) {
     SCAIL_REQUIRE(o32 && state, "attention_partial: null operand");
     return attention_impl(Q, ldq, K, ldk, V, ldv, nullptr, 8, B, H, q_len, kv_off0, kv_len0, kv_off1, kv_len1, q_batch_rows,
-                          kv_batch_rows, q_rows_total, kv_rows_total, scale, 0, o32, ldo32, state, stream);
+                          kv_batch_rows, q_rows_total, kv_rows_total, scale, 0, o32, ldo32, state, nullptr, nullptr, stream);
 }
 
 int scail_attention_merge(const float* o32_a, const void* state_a, const float* o32_b, const void* state_b, void* out,

@@ -43,9 +43,15 @@ struct AttnParams {
     int kv_batch_rows;   // row stride between batches in the K/V matrices
     float scale_log2;    // softmax scale * log2(e)
     int accumulate;      // out += result (second cross-attention pass, dit_video_crossattn_sc_xc.py:1197)
+    const int* kv_tile_ptr;  // block-sparse map (attention_fwd_kernel<true> only, one range, kv_off = 0): query tile t attends
+    const int* kv_tile_idx;  // the key tiles kv_tile_idx[kv_tile_ptr[t] .. kv_tile_ptr[t + 1]), strictly ascending
 };
 
 
+// kSparse: the CTA's key tiles are the row blockIdx.x of the block-sparse map (AttnParams::kv_tile_ptr / kv_tile_idx) instead
+// of every tile of the key ranges.  Only the tile list changes: tile j of the row is loaded from key row 128 kv_tile_idx[j],
+// its valid-key mask is taken from that global start, and the turns run over the row's n_kv tiles exactly as below.
+template <bool kSparse>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                      const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
@@ -71,8 +77,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     const int head = blockIdx.y;
     const int batch = blockIdx.z;
     const int q0 = blockIdx.x * ATT_BQ;
-    const int n_kv0 = (p.kv_len + ATT_BKV - 1) / ATT_BKV;
-    const int n_kv = n_kv0 + (p.kv_len1 + ATT_BKV - 1) / ATT_BKV;
+    const int* kv_tiles = kSparse ? p.kv_tile_idx + p.kv_tile_ptr[blockIdx.x] : nullptr;
+    const int n_kv0 = kSparse ? p.kv_tile_ptr[blockIdx.x + 1] - p.kv_tile_ptr[blockIdx.x] : (p.kv_len + ATT_BKV - 1) / ATT_BKV;
+    const int n_kv = kSparse ? n_kv0 : n_kv0 + (p.kv_len1 + ATT_BKV - 1) / ATT_BKV;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_q);
@@ -99,7 +106,10 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
                 tma_load_2d(q_smem + h * ATT_HALF_BYTES, &tmap_q, bar(B_QFULL), col + h * 64, batch * p.q_batch_rows + q0);
             const int kvbase = batch * p.kv_batch_rows;
             // tile j of the concatenated key ranges starts at this row (a range's last tile may run past its end: masked)
-            auto kv_row = [&](int j) { return kvbase + (j < n_kv0 ? p.kv_off + j * ATT_BKV : p.kv_off1 + (j - n_kv0) * ATT_BKV); };
+            auto kv_row = [&](int j) {
+                if (kSparse) return kvbase + p.kv_off + kv_tiles[j] * ATT_BKV;
+                return kvbase + (j < n_kv0 ? p.kv_off + j * ATT_BKV : p.kv_off1 + (j - n_kv0) * ATT_BKV);
+            };
             for (int j = 0; j < n_kv; ++j) {
                 const int s = j % ATT_STAGES;
                 const uint32_t par = ((j / ATT_STAGES) & 1) ^ 1;
@@ -155,7 +165,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         // waits for S of tile j, releases the K stage, then the online softmax: O *= alpha, P -> pa
         // (thread: rows r = sc[4c + 0/1], r + 8 = sc[4c + 2/3], columns 8c + 2 quad + 0/1)
         auto softmax = [&](int j, float(&sc)[ATT_BKV / 2]) {
-            const int valid = j < n_kv0 ? min(ATT_BKV, p.kv_len - j * ATT_BKV) : min(ATT_BKV, p.kv_len1 - (j - n_kv0) * ATT_BKV);
+            const int valid = kSparse    ? min(ATT_BKV, p.kv_len - kv_tiles[j] * ATT_BKV)
+                              : j < n_kv0 ? min(ATT_BKV, p.kv_len - j * ATT_BKV)
+                                          : min(ATT_BKV, p.kv_len1 - (j - n_kv0) * ATT_BKV);
             wgmma_wait<0>();
             fence_regs(sc);
             if (releaser) mbar_arrive(bar(B_KEMPTY + j % ATT_STAGES));
@@ -304,8 +316,13 @@ struct Attn8Params {
     const float* v_scale;   // [B, H, 128]
     int L, L_pad, heads;
     float scale_log2;       // softmax scale * log2(e)
+    const int* kv_tile_ptr;  // block-sparse map (attention_fp8_kernel<true> only), as AttnParams
+    const int* kv_tile_idx;
 };
 
+// kSparse: the block-sparse map selects the CTA's key tiles, as in attention_fwd_kernel<true>; tile j's K rows, K scales
+// and V^T columns start at key 128 kv_tile_idx[j].
+template <bool kSparse>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                      const __grid_constant__ CUtensorMap tmap_vt, const Attn8Params p) {
@@ -332,7 +349,9 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     const int head = blockIdx.y;
     const int batch = blockIdx.z;
     const int q0 = blockIdx.x * ATT_BQ;
-    const int n_kv = (p.L + ATT_BKV - 1) / ATT_BKV;
+    const int* kv_tiles = kSparse ? p.kv_tile_idx + p.kv_tile_ptr[blockIdx.x] : nullptr;
+    const int n_kv = kSparse ? p.kv_tile_ptr[blockIdx.x + 1] - p.kv_tile_ptr[blockIdx.x] : (p.L + ATT_BKV - 1) / ATT_BKV;
+    auto kv_start = [&](int j) { return (kSparse ? kv_tiles[j] : j) * ATT_BKV; };  // first key of the CTA's tile j
     const int64_t bh = static_cast<int64_t>(batch) * p.heads + head;
 
     if (warp == 0 && lane == 0) {
@@ -364,11 +383,12 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
                 const uint32_t par = ((j / ATT8_STAGES) & 1) ^ 1;
                 mbar_wait(bar(B_KEMPTY + s), par, 10);
                 mbar_expect_tx(bar(B_KFULL + s), ATT8_TILE_BYTES + ATT8_KS_BYTES);
-                tma_load_2d(k_smem + s * ATT8_TILE_BYTES, &tmap_k, bar(B_KFULL + s), col, row0 + j * ATT_BKV);
-                bulk_load_1d(ks_smem + s * ATT8_KS_BYTES, ks + j * ATT_BKV, ATT8_KS_BYTES, bar(B_KFULL + s));
+                const int k0 = kv_start(j);
+                tma_load_2d(k_smem + s * ATT8_TILE_BYTES, &tmap_k, bar(B_KFULL + s), col, row0 + k0);
+                bulk_load_1d(ks_smem + s * ATT8_KS_BYTES, ks + k0, ATT8_KS_BYTES, bar(B_KFULL + s));
                 mbar_wait(bar(B_VEMPTY + s), par, 11);
                 mbar_expect_tx(bar(B_VFULL + s), ATT8_TILE_BYTES);
-                tma_load_2d(v_smem + s * ATT8_TILE_BYTES, &tmap_vt, bar(B_VFULL + s), j * ATT_BKV, static_cast<int>(bh * ATT_D));
+                tma_load_2d(v_smem + s * ATT8_TILE_BYTES, &tmap_vt, bar(B_VFULL + s), k0, static_cast<int>(bh * ATT_D));
             }
         }
     } else {
@@ -393,7 +413,7 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         for (int j = 0; j < n_kv; ++j) {
             const int s = j % ATT8_STAGES;
             const uint32_t par = (j / ATT8_STAGES) & 1;
-            const int valid = min(ATT_BKV, p.L - j * ATT_BKV);
+            const int valid = min(ATT_BKV, p.L - kv_start(j));
             // ---- S = Q K^T ----
             float sc[ATT_BKV / 2];
             mbar_wait(bar(B_KFULL + s), par, 21);

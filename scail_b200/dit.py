@@ -25,7 +25,7 @@ from operator import mul
 import torch
 from torch import nn
 
-from . import ops, rope
+from . import ops, rope, sparse
 
 try:  # when SAT is importable (reference present) be a real BaseMixin so add_mixin / collect_hooks_ accept us
     from sat.model.mixins import BaseMixin as _SatBaseMixin  # type: ignore
@@ -296,7 +296,8 @@ class AdaLNMixin(BaseMixin):
 
     def __init__(self, hidden_size, num_layers, time_embed_dim, compressed_num_frames, transformer_args, qk_ln=True,
                  qk_ln_affine=None, hidden_size_head=None, params_dtype=torch.float, device=torch.device("cpu"),
-                 elementwise_affine=True, share_adaln=False, use_i2v_clip=False, fp8_linear=False, fp8_attention=False):
+                 elementwise_affine=True, share_adaln=False, use_i2v_clip=False, fp8_linear=False, fp8_attention=False,
+                 attention_window=None):
         super().__init__()
         if not (qk_ln and share_adaln and use_i2v_clip) or hidden_size_head != hidden_size:
             raise NotImplementedError("scail_b200 implements qk_ln=True over the full hidden width, share_adaln=True, use_i2v_clip=True")
@@ -330,6 +331,10 @@ class AdaLNMixin(BaseMixin):
         # Opt-in, independent of fp8_linear: the self-attention runs on e4m3 Q, K (one scale per token and head) and V (one
         # scale per channel) through attention_fp8_kernel; cross-attention stays bf16.  A plain attribute, like fp8_linear.
         self.fp8_attention = fp8_attention
+        # Opt-in block-sparse self-attention (scail_b200.sparse): None is dense; an int w >= 0 restricts every query to the
+        # keys within w frames of its own (the ref rows and the ref keys stay dense), through the sparse forms of whichever
+        # self-attention kernel runs (bf16 or fp8_attention).  A plain attribute, toggled between forwards like fp8_attention.
+        self.attention_window = None if attention_window is None else sparse.check_window(attention_window)
 
     # -- fp8 linears ---------------------------------------------------------------------------
     FP8_LINEARS = ("attention.query_key_value", "attention.dense", "cross_attention.query", "cross_attention.dense",
@@ -463,11 +468,15 @@ class AdaLNMixin(BaseMixin):
         if self.cp is None or self.cp.size == 1:
             qkv = _WS.get("qkv", (B * N, 3 * d), dev)
             self._linear(h2, a.query_key_value, _fp8_scale, out=qkv)
+            tiles = self._attention_tiles(dev, N, kw_args)
             if self.fp8_attention:
-                self._self_attention_fp8(qkv, B, N, d, H, wq, wk, cos, sin, ctx)
+                self._self_attention_fp8(qkv, B, N, d, H, wq, wk, cos, sin, ctx, tiles)
             else:
                 ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon)
-                ops.attention(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, N)
+                if tiles is None:
+                    ops.attention(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, N)
+                else:
+                    ops.attention_sparse(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, tiles)
         else:
             self._refuse_fp8_attention_cp()
             # engine-style sequence parallelism (diffusion_video.py:495-552): the latents arrive pre-chunked on H or W, so the
@@ -478,7 +487,17 @@ class AdaLNMixin(BaseMixin):
             return None
         return self._linear(ctx, a.dense, name="ctx8").view(B, N, d)
 
-    def _self_attention_fp8(self, qkv, B, N, d, H, wq, wk, cos, sin, ctx):
+    def _attention_tiles(self, dev, N, kw):
+        """The frame-window tile map of this forward's token layout (built once per geometry, window and device), or None
+        when attention_window is None."""
+        if self.attention_window is None:
+            return None
+        g = sparse.geometry(**kw)
+        if g.ref_length + g.seq_length + g.pose_length != N:
+            raise ValueError(f"attention_window: the token layout {g} does not add up to the sequence length {N}")
+        return sparse.tile_map(g, self.attention_window, dev)
+
+    def _self_attention_fp8(self, qkv, B, N, d, H, wq, wk, cos, sin, ctx, tiles=None):
         """Self-attention of the fused QKV buffer in e4m3: RMSNorm+RoPE writes quantised Q and K, the V slab is transposed and
         quantised per channel, then attention_fp8 writes the merged-head context into ctx.  Buffers: per-stream workspace."""
         dev, f32 = qkv.device, torch.float32
@@ -488,12 +507,15 @@ class AdaLNMixin(BaseMixin):
         ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon, out_fp8=[q8, k8])
         vt, vs = ops.quant_vt_fp8(qkv[:, 2 * d:], B, H, N, _WS.get("vt8", (B, H, 128, Lp), dev, ops.FP8),
                                   _WS.get("vt8_scale", (B, H, 128), dev, f32), _WS.get("vt8_amax", (B, d), dev, torch.int32))
-        ops.attention_fp8(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N)
+        ops.attention_fp8(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, tiles=tiles)
 
     def _refuse_fp8_attention_cp(self):
         if self.fp8_attention and self.cp is not None and self.cp.size > 1:
             raise NotImplementedError("fp8_attention is not implemented under context parallelism (a ContextParallel of size "
                                       f"{self.cp.size}); turn fp8_attention off or run without context parallelism")
+        if self.attention_window is not None and self.cp is not None and self.cp.size > 1:
+            raise NotImplementedError("attention_window is not implemented under context parallelism (a ContextParallel of "
+                                      f"size {self.cp.size}); set attention_window to None or run without context parallelism")
 
     def cross_attention_forward(self, hidden_states, cross_attention_mask, encoder_outputs, _ctx_out=None, _fp8_scale=None,
                                 **kw_args):
@@ -569,7 +591,7 @@ class DiffusionTransformer(nn.Module):
                  text_dim=4096, num_layers=40, num_attention_heads=40, elementwise_affine=False, time_freq_dim=256,
                  time_embed_dim=None, modules=None, share_adaln=True, use_SwiGLU=False, use_RMSNorm=False,
                  layernorm_epsilon=1e-6, inner_hidden_size=None, use_i2v_clip=True, dtype="bf16", fp8_linear=False,
-                 fp8_attention=False, **kwargs):
+                 fp8_attention=False, attention_window=None, **kwargs):
         super().__init__()
         if use_SwiGLU or use_RMSNorm:
             raise NotImplementedError("SCAIL-14B uses the non-gated GELU-tanh MLP and LayerNorm (yaml:42-43)")
@@ -605,7 +627,7 @@ class DiffusionTransformer(nn.Module):
         self.add_mixin("adaln_layer", AdaLNMixin(d, num_layers, self.time_embed_dim, frames, targs, qk_ln=True,
                                                  qk_ln_affine=True, hidden_size_head=d, elementwise_affine=elementwise_affine,
                                                  share_adaln=True, use_i2v_clip=True, fp8_linear=fp8_linear,
-                                                 fp8_attention=fp8_attention))
+                                                 fp8_attention=fp8_attention, attention_window=attention_window))
         self.add_mixin("final_layer", FinalLayerMixin(d, self.time_embed_dim, self.patch_size, out_channels,
                                                       elementwise_affine, layernorm_epsilon, True))
         object.__setattr__(self.mixins["adaln_layer"], "_pos_embed", self.mixins["pos_embed"])

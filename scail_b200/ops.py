@@ -182,6 +182,100 @@ def attention(q, k, v, out, B, H, q_len, kv_len, q_batch_rows=None, kv_batch_row
     return out
 
 
+ATT_TILE = 128  # query rows and keys per attention tile
+
+
+def check_tile_map(kv_tile_ptr, kv_tile_idx, q_len, kv_len):
+    """Validate a block-sparse attention map on the host (array-likes of ints): kv_tile_ptr [ceil(q_len/128) + 1] with
+    ptr[0] == 0 and ptr[-1] == len(kv_tile_idx); every row ptr[q]..ptr[q+1] non-empty, strictly ascending, each index in
+    [0, ceil(kv_len/128)).  Raises ValueError naming the first violation."""
+    import numpy as np
+    ptr = np.asarray(kv_tile_ptr)
+    idx = np.asarray(kv_tile_idx)
+    n_q, n_kv = -(-int(q_len) // ATT_TILE), -(-int(kv_len) // ATT_TILE)
+    if q_len <= 0 or kv_len <= 0:
+        raise ValueError(f"tile map: q_len={q_len} and kv_len={kv_len} must be positive")
+    if ptr.ndim != 1 or idx.ndim != 1 or not np.issubdtype(ptr.dtype, np.integer) or not np.issubdtype(idx.dtype, np.integer):
+        raise ValueError("tile map: kv_tile_ptr and kv_tile_idx must be 1-D integer arrays")
+    if ptr.size != n_q + 1:
+        raise ValueError(f"tile map: kv_tile_ptr has {ptr.size} entries, want n_q_tiles + 1 = {n_q + 1}")
+    if ptr[0] != 0 or ptr[-1] != idx.size:
+        raise ValueError(f"tile map: kv_tile_ptr must run from 0 to nnz = {idx.size} (got {ptr[0]} .. {ptr[-1]})")
+    counts = np.diff(ptr.astype(np.int64))
+    if (counts <= 0).any():
+        raise ValueError(f"tile map: query tile {int(np.argmax(counts <= 0))} has no key tiles (rows must be non-empty)")
+    if idx.size and (idx.min() < 0 or idx.max() >= n_kv):
+        raise ValueError(f"tile map: key tile indices must lie in [0, {n_kv})")
+    step = np.diff(idx.astype(np.int64))
+    row_start = np.zeros(idx.size, dtype=bool)
+    row_start[ptr[:-1]] = True
+    if (step <= 0)[~row_start[1:]].any():
+        raise ValueError("tile map: every row's key tiles must be strictly ascending")
+
+
+class TileMap:
+    """A validated block-sparse self-attention map on one device: for query tile q (rows [128 q, 128 q + 128)) the key tiles
+    kv_tile_idx[kv_tile_ptr[q] : kv_tile_ptr[q + 1]] (keys [128 k, 128 k + 128)), int32.  One map serves every (batch,
+    head).  device=None keeps the validated host arrays only."""
+
+    def __init__(self, kv_tile_ptr, kv_tile_idx, q_len, kv_len, device=None, checked=False):
+        import numpy as np
+        ptr = np.asarray(kv_tile_ptr.cpu() if isinstance(kv_tile_ptr, torch.Tensor) else kv_tile_ptr)
+        idx = np.asarray(kv_tile_idx.cpu() if isinstance(kv_tile_idx, torch.Tensor) else kv_tile_idx)
+        if not checked:
+            check_tile_map(ptr, idx, q_len, kv_len)
+        self.q_len, self.kv_len = int(q_len), int(kv_len)
+        self.n_q_tiles, self.n_kv_tiles, self.nnz = ptr.size - 1, -(-self.kv_len // ATT_TILE), int(idx.size)
+        self.density = self.nnz / float(self.n_q_tiles * self.n_kv_tiles)
+        self.ptr = self.idx = None
+        if device is not None:
+            self.ptr = torch.from_numpy(ptr.astype(np.int32)).to(device)
+            self.idx = torch.from_numpy(idx.astype(np.int32)).to(device)
+
+    def _check_for(self, L, device):
+        if self.q_len != L or self.kv_len != L:
+            raise ValueError(f"tile map built for q_len={self.q_len}, kv_len={self.kv_len}; this launch has L={L}")
+        if self.ptr is None or self.ptr.device != device:
+            raise ValueError(f"tile map lives on {None if self.ptr is None else self.ptr.device}, the operands on {device}")
+
+
+def _tile_map(tiles, L):
+    """A TileMap, or a (kv_tile_ptr, kv_tile_idx) pair validated and uploaded here (once per call)."""
+    if isinstance(tiles, TileMap):
+        return tiles
+    ptr, idx = tiles
+    host = [t.cpu() if isinstance(t, torch.Tensor) else t for t in (ptr, idx)]
+    check_tile_map(*host, L, L)  # before anything touches a device
+    dev = ptr.device if isinstance(ptr, torch.Tensor) and ptr.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    return TileMap(*host, L, L, device=dev, checked=True)
+
+
+def attention_sparse(q, k, v, out, B, H, L, tiles, q_batch_rows=None, kv_batch_rows=None, scale=None, accumulate=False):
+    """Block-sparse bf16 self-attention (q_len == kv_len == L): as attention(), but query tile t attends only to the keys of
+    the key tiles `tiles` lists for it (a TileMap, or a (kv_tile_ptr, kv_tile_idx) pair: see check_tile_map)."""
+    m = _tile_map(tiles, L)
+    for t in (q, k, v, out):
+        _req(t)
+        assert t.dim() == 2 and t.stride(1) == 1
+    m._check_for(L, q.device)
+    q_batch_rows = L if q_batch_rows is None else q_batch_rows
+    kv_batch_rows = L if kv_batch_rows is None else kv_batch_rows
+    scale = 1.0 / math.sqrt(128) if scale is None else scale
+    ev = None
+    if ATTN_EVENTS is not None and L > 1024:
+        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+        ev[0].record()
+    _lib.check(_lib.lib().scail_attention_sparse(_ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
+                                                 out.stride(0), B, H, L, L, q_batch_rows, kv_batch_rows, q.shape[0],
+                                                 k.shape[0], scale, 1 if accumulate else 0, _ptr(m.ptr), _ptr(m.idx), m.nnz,
+                                                 _stream()), "scail_attention_sparse")
+    if ev is not None:
+        ev[1].record()
+        ATTN_EVENTS.append(ev)
+    _count()
+    return out
+
+
 def quant_vt_fp8(v, B, H, L, vt=None, scale=None, work=None):
     """V operand of attention_fp8: v bf16 [B*L, H*128] (2-D row-strided view) -> (vt e4m3 [B, H, 128, L_pad], scale fp32
     [B, H, 128]): Vt's rows are the channels over the keys in the e4m3 row format, zero past L, and inside every 16-key group
@@ -204,9 +298,11 @@ def quant_vt_fp8(v, B, H, L, vt=None, scale=None, work=None):
     return vt, scale
 
 
-def attention_fp8(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, scale=None):
+def attention_fp8(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, scale=None, tiles=None):
     """FP8 self-attention (q_len == kv_len == L): q8/k8 e4m3 [B*L, H*128] (2-D row-strided) with scales [B, H, L_pad] as
-    rmsnorm_rope(out_fp8=...) writes them, (vt, v_scale) from quant_vt_fp8; out bf16 [B*L, H*128] merged heads."""
+    rmsnorm_rope(out_fp8=...) writes them, (vt, v_scale) from quant_vt_fp8; out bf16 [B*L, H*128] merged heads.
+    tiles (attention_fp8_sparse): a block-sparse map as for attention_sparse."""
+    m = _tile_map(tiles, L) if tiles is not None else None
     for t in (q8, k8):
         _req(t, FP8)
         assert t.dim() == 2 and t.stride(1) == 1 and t.shape == (B * L, H * 128)
@@ -222,14 +318,27 @@ def attention_fp8(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, scale=Non
     if ATTN_EVENTS is not None and L > 1024:
         ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
         ev[0].record()
-    _lib.check(_lib.lib().scail_attention_fp8(_ptr(q8), q8.stride(0), _ptr(q_scale), _ptr(k8), k8.stride(0), _ptr(k_scale),
-                                              _ptr(vt), _ptr(v_scale), _ptr(out), out.stride(0), B, H, 128, L, Lp, scale,
-                                              _stream()), "scail_attention_fp8")
+    if m is None:
+        _lib.check(_lib.lib().scail_attention_fp8(_ptr(q8), q8.stride(0), _ptr(q_scale), _ptr(k8), k8.stride(0),
+                                                  _ptr(k_scale), _ptr(vt), _ptr(v_scale), _ptr(out), out.stride(0), B, H, 128, L,
+                                                  Lp, scale, _stream()), "scail_attention_fp8")
+    else:
+        m._check_for(L, q8.device)
+        _lib.check(_lib.lib().scail_attention_fp8_sparse(_ptr(q8), q8.stride(0), _ptr(q_scale), _ptr(k8), k8.stride(0),
+                                                         _ptr(k_scale), _ptr(vt), _ptr(v_scale), _ptr(out), out.stride(0), B, H,
+                                                         128, L, Lp, scale, _ptr(m.ptr), _ptr(m.idx), m.nnz, _stream()),
+                   "scail_attention_fp8_sparse")
     if ev is not None:
         ev[1].record()
         ATTN_EVENTS.append(ev)
     _count()
     return out
+
+
+def attention_fp8_sparse(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, tiles, scale=None):
+    """Block-sparse FP8 self-attention: attention_fp8 over the key tiles `tiles` lists for each query tile (see
+    attention_sparse)."""
+    return attention_fp8(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, scale=scale, tiles=tiles)
 
 
 def attention_partial(q, k, v, o32, state, B, H, q_len, ranges, q_batch_rows=None, kv_batch_rows=None, scale=None):

@@ -140,7 +140,8 @@ class GraphedStep:
     instead of ~780, and none of the reference's per-layer host syncs (sat/transformer_defaults.py:56-57) by construction.
     The latent `x`, the timestep vector and the conditioning tensors are static buffers owned by this object; results are
     bit-identical to `sampler_step` (same kernels, same order).  Single-GPU path (NCCL collectives are not captured).
-    The graph runs in the `fp8_linear` mode of construction time.  With fp8 it reads the e4m3 weight copies in place: every
+    The graph runs in the `fp8_linear`, `fp8_attention` and `attention_window` modes of construction time; a window's tile map
+    is held by scail_b200.sparse for the life of the process, so the graph reads it at a fixed address.  With fp8 it reads the e4m3 weight copies in place: every
     call first re-derives, into the same buffers, the copies of weights that changed since (e.g. after load_state_dict)."""
 
     def __init__(self, model, x, cond, uc, scale=4.0):
