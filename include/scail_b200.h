@@ -184,6 +184,23 @@ int scail_unpatchify(const void* lin, void* out, int64_t B, int64_t T, int64_t H
 int scail_cfg_euler(float* x, const void* v, int64_t n, float scale, float dsigma, scail_stream_t stream);
 int scail_cast_f32_bf16(const float* x, void* out, int64_t n, scail_stream_t stream);
 
+/* First-block residual cache (scail_b200/step_cache.py).  Token tensors are bf16 [B, N, d] (ref || noise || pose rows of
+ * each batch element); the noise rows are rows [n_ref, n_ref + n_seq) of each element.  d % 8 == 0, B*N*d/8 < 2^31, and
+ * every bf16/fp32 tensor is contiguous and 16-byte aligned.
+ * scail_step_cache_indicator: r = bf16_rn(f32(h1) - f32(h0)) -> r_new, the noise rows of h1 -> h1c [B, n_seq, d], and
+ * out = {sum |r - r_ref|, sum |r_ref|, ratio, 0} (fp64; ratio = +inf when the denominator is 0).  fp32 partial sums per CTA
+ * over a fixed partition of the elements (partials: at least 2 * 1024 floats), then one CTA adds them in fp64 in a fixed
+ * order: bit-reproducible, no floating-point atomics.  Two launches.
+ * scail_step_cache_update: R [B, n_seq, d] fp32 = f32(h[noise rows]) - f32(h1c).
+ * scail_step_cache_apply: in place on the noise rows of h, h = bf16_rn(f32(h) + R). */
+int scail_step_cache_indicator(const void* h0, const void* h1, const void* r_ref, void* r_new, void* h1c, float* partials,
+                               int64_t partials_len, double* out, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq,
+                               scail_stream_t stream);
+int scail_step_cache_update(const void* h, const void* h1c, float* R, int64_t B, int64_t N, int64_t d, int64_t n_ref,
+                            int64_t n_seq, scail_stream_t stream);
+int scail_step_cache_apply(void* h, const float* R, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq,
+                           scail_stream_t stream);
+
 /* ---- Wan2.1 VAE decode (sgm/models/wan_vae.py); activations channels-last bf16 [T, H, W, C] ---- */
 enum { SCAIL_CONV_EPI_BIAS = 0, SCAIL_CONV_EPI_BIAS_RES = 1, SCAIL_CONV_EPI_HEAD_CLAMP = 2 };
 

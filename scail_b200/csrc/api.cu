@@ -18,6 +18,7 @@
 #include "conv.cuh"
 #include "gemm.cuh"
 #include "rowops.cuh"
+#include "step_cache.cuh"
 
 namespace {
 
@@ -729,6 +730,65 @@ int scail_cast_f32_bf16(const float* x, void* out, int64_t n, scail_stream_t str
     SCAIL_REQUIRE(x && out, "cast: null operand");
     scail::cast_f32_to_bf16_kernel<<<blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         x, static_cast<__nv_bfloat16*>(out), n);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// Shape checks shared by the three step-cache entry points; returns 0 or the fail() code.
+static int step_cache_shape(const char* what, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq) {
+    SCAIL_REQUIRE(B >= 1 && N >= 1 && d >= 8 && d % 8 == 0, "%s: need B >= 1, N >= 1 and d a positive multiple of 8 (got B=%lld, "
+                  "N=%lld, d=%lld)", what, (long long)B, (long long)N, (long long)d);
+    SCAIL_REQUIRE(n_ref >= 0 && n_seq >= 1 && n_ref + n_seq <= N, "%s: noise rows [n_ref, n_ref + n_seq) = [%lld, %lld) must lie "
+                  "inside the N = %lld rows of a batch element", what, (long long)n_ref, (long long)(n_ref + n_seq), (long long)N);
+    SCAIL_REQUIRE(B * N * (d / 8) < (int64_t(1) << 31), "%s: B * N * d / 8 must be < 2^31 (got %lld)", what,
+                  (long long)(B * N * (d / 8)));
+    return 0;
+}
+
+int scail_step_cache_indicator(const void* h0, const void* h1, const void* r_ref, void* r_new, void* h1c, float* partials,
+                               int64_t partials_len, double* out, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq,
+                               scail_stream_t stream) {
+    SCAIL_REQUIRE(h0 && h1 && r_ref && r_new && h1c && partials && out, "step_cache_indicator: null operand");
+    SCAIL_REQUIRE(aligned16(h0) && aligned16(h1) && aligned16(r_ref) && aligned16(r_new) && aligned16(h1c),
+                  "step_cache_indicator: h0, h1, r_ref, r_new and h1c must be 16-byte aligned");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0,
+                  "step_cache_indicator: partials must be 4-byte and out 8-byte aligned");
+    if (int rc = step_cache_shape("step_cache_indicator", B, N, d, n_ref, n_seq)) return rc;
+    const int64_t nvec = B * N * (d / 8);
+    const int ctas = static_cast<int>(std::min<int64_t>(scail::SC_MAX_CTAS, (nvec + scail::SC_THREADS - 1) / scail::SC_THREADS));
+    SCAIL_REQUIRE(partials_len >= 2 * ctas, "step_cache_indicator: partials holds %lld floats, this shape needs %d",
+                  (long long)partials_len, 2 * ctas);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    scail::step_cache_indicator_kernel<<<ctas, scail::SC_THREADS, 0, st>>>(
+        static_cast<const uint4*>(h0), static_cast<const uint4*>(h1), static_cast<const uint4*>(r_ref), static_cast<uint4*>(r_new),
+        static_cast<uint4*>(h1c), partials, nvec, static_cast<unsigned>(d / 8), static_cast<unsigned>(N), (int)n_ref, (int)n_seq);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    scail::step_cache_finish_kernel<<<1, scail::SC_THREADS, 0, st>>>(partials, ctas, out);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_step_cache_update(const void* h, const void* h1c, float* R, int64_t B, int64_t N, int64_t d, int64_t n_ref,
+                            int64_t n_seq, scail_stream_t stream) {
+    SCAIL_REQUIRE(h && h1c && R, "step_cache_update: null operand");
+    SCAIL_REQUIRE(aligned16(h) && aligned16(h1c) && aligned16(R), "step_cache_update: h, h1c and R must be 16-byte aligned");
+    if (int rc = step_cache_shape("step_cache_update", B, N, d, n_ref, n_seq)) return rc;
+    const int64_t nvec = B * n_seq * (d / 8);
+    scail::step_cache_update_kernel<<<blocks_for(nvec, scail::SC_THREADS), scail::SC_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const uint4*>(h), static_cast<const uint4*>(h1c), reinterpret_cast<float4*>(R), nvec, (int)(d / 8), (int)N,
+        (int)n_ref, (int)n_seq);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_step_cache_apply(void* h, const float* R, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq,
+                           scail_stream_t stream) {
+    SCAIL_REQUIRE(h && R, "step_cache_apply: null operand");
+    SCAIL_REQUIRE(aligned16(h) && aligned16(R), "step_cache_apply: h and R must be 16-byte aligned");
+    if (int rc = step_cache_shape("step_cache_apply", B, N, d, n_ref, n_seq)) return rc;
+    const int64_t nvec = B * n_seq * (d / 8);
+    scail::step_cache_apply_kernel<<<blocks_for(nvec, scail::SC_THREADS), scail::SC_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<uint4*>(h), reinterpret_cast<const float4*>(R), nvec, (int)(d / 8), (int)N, (int)n_ref, (int)n_seq);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

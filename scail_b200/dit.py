@@ -25,7 +25,7 @@ from operator import mul
 import torch
 from torch import nn
 
-from . import ops, rope, sparse
+from . import ops, rope, sparse, step_cache
 
 try:  # when SAT is importable (reference present) be a real BaseMixin so add_mixin / collect_hooks_ accept us
     from sat.model.mixins import BaseMixin as _SatBaseMixin  # type: ignore
@@ -693,7 +693,59 @@ class DiffusionTransformer(nn.Module):
         """x [b,t,16,h,w]; kwargs: ref_concat [1|b,1,16,h,w], concat_smpl_render [1|b,t,16,h/2,w/2],
         image_clip_features [1|b,257,1280], concat_images (gate only, F12), history_mask [1|b,t,4,h,w] (optional: the mask
         channels of x, :1462-1467), chunk_dim (3 | 4 | None: the engine's pre-chunked sequence parallelism,
-        diffusion_video.py:495-552).  Returns [b,t,16,h,w] bf16 (the local chunk when chunk_dim is set)."""
+        diffusion_video.py:495-552), _step_cache (a scail_b200.step_cache.FirstBlockCache, or None: the first-block residual
+        cache decides on this forward whether blocks 1..L-1 run).  Returns [b,t,16,h,w] bf16 (the local chunk when chunk_dim
+        is set)."""
+        sc = kwargs.pop("_step_cache", None)
+        if sc is not None:
+            head = self.step_cache_head(sc, x, timesteps, context, y, **kwargs)
+            head.buffers.indicator(head.h0)
+            skip = sc.decide(head.buffers.read_indicator())
+            out = self.step_cache_tail(head, skip)
+            if not skip:
+                sc.computed()
+            return out
+        hidden, kw, cond = self._tokens(x, timesteps, context, y, kwargs)
+        ad = self.mixins["adaln_layer"]
+        cp = ad.cp
+        chunk_dim = kw.get("chunk_dim")
+        n_layers = int(kwargs.get("_num_layers") or self.num_layers)  # verification hook (bench.py cp_check_rel): first k blocks only
+        if cp is None or cp.size == 1:
+            for l in range(n_layers):
+                hidden = ad.layer_forward(hidden, None, layer_id=l, **kw)
+            return self.mixins["final_layer"].final_forward(hidden, **kw)
+        # ---- context parallel: the CFG branches (independent batch elements) run on separate streams so that one
+        # branch's K/V all-gather overlaps the other branch's GEMMs / attention.  Tokens are either sharded here
+        # (replicated inputs) or already local (chunk_dim: the engine chunked the latents on H/W per rank) ----
+        b, N = x.shape[0], hidden.shape[1]
+        adaln, text, clip = kw["emb"], kw["encoder_outputs"], kw["image_clip_features"]
+        local = hidden if chunk_dim is not None else cp.shard_tokens(hidden)
+        main = torch.cuda.current_stream()
+        streams = cp.branch_streams(b, x.device)
+        if ad.fp8_linear:  # every branch reads the same e4m3 weights: derive them here, before the branch streams wait on main
+            ad.prepare_fp8_weights(n_layers, streams)
+        per = []
+        for i in range(b):
+            kwi = dict(kw, emb=adaln[i:i + 1], encoder_outputs=text[i:i + 1], image_clip_features=clip[i:i + 1])
+            if cond is not None:
+                Lt, Lc = text.shape[1], clip.shape[1]
+                kwi["_xkv_layers"] = [(tk[i * Lt:(i + 1) * Lt], ck[i * Lc:(i + 1) * Lc]) for tk, ck in cond.xkv]
+            per.append([local[i:i + 1].contiguous(), kwi])
+            streams[i].wait_stream(main)
+        for l in range(n_layers):
+            for i in range(b):
+                with torch.cuda.stream(streams[i]):
+                    per[i][0] = ad.layer_forward(per[i][0], None, layer_id=l, **per[i][1])
+        for i in range(b):
+            main.wait_stream(streams[i])
+        hidden = torch.cat([h_ for h_, _ in per], 0)
+        if chunk_dim is None:
+            hidden = cp.gather_tokens(hidden, N)
+        return self.mixins["final_layer"].final_forward(hidden, **kw)
+
+    def _tokens(self, x, timesteps, context, y, kwargs):
+        """The per-step embeddings and the patch embedding of forward(): -> (hidden [b, N, d] in the workspace, the layer
+        kwargs, the Conditioning handle in use or None)."""
         _need_cuda(x)
         assert y is None, "SCAIL's DiT is not class-conditional (num_classes is None)"
         assert kwargs.get("ref_concat") is not None, "must specify ref_concat"
@@ -738,34 +790,38 @@ class DiffusionTransformer(nn.Module):
         # the 16-channel inputs go straight to the gather kernel, which synthesises the mask channels
         hidden = self.mixins["patch_embed"].word_embedding_forward(None, images=xb, ref_concat=ref,
                                                                    concat_smpl_render=pose, _hidden_out=hidden)
-        n_layers = int(kwargs.get("_num_layers") or self.num_layers)  # verification hook (bench.py cp_check_rel): first k blocks only
-        if cp is None or cp.size == 1:
-            for l in range(n_layers):
-                hidden = ad.layer_forward(hidden, None, layer_id=l, **kw)
-            return self.mixins["final_layer"].final_forward(hidden, **kw)
-        # ---- context parallel: the CFG branches (independent batch elements) run on separate streams so that one
-        # branch's K/V all-gather overlaps the other branch's GEMMs / attention.  Tokens are either sharded here
-        # (replicated inputs) or already local (chunk_dim: the engine chunked the latents on H/W per rank) ----
-        local = hidden if chunk_dim is not None else cp.shard_tokens(hidden)
-        main = torch.cuda.current_stream()
-        streams = cp.branch_streams(b, x.device)
-        if ad.fp8_linear:  # every branch reads the same e4m3 weights: derive them here, before the branch streams wait on main
-            ad.prepare_fp8_weights(n_layers, streams)
-        per = []
-        for i in range(b):
-            kwi = dict(kw, emb=adaln[i:i + 1], encoder_outputs=text[i:i + 1], image_clip_features=clip[i:i + 1])
-            if cond is not None:
-                Lt, Lc = text.shape[1], clip.shape[1]
-                kwi["_xkv_layers"] = [(tk[i * Lt:(i + 1) * Lt], ck[i * Lc:(i + 1) * Lc]) for tk, ck in cond.xkv]
-            per.append([local[i:i + 1].contiguous(), kwi])
-            streams[i].wait_stream(main)
-        for l in range(n_layers):
-            for i in range(b):
-                with torch.cuda.stream(streams[i]):
-                    per[i][0] = ad.layer_forward(per[i][0], None, layer_id=l, **per[i][1])
-        for i in range(b):
-            main.wait_stream(streams[i])
-        hidden = torch.cat([h_ for h_, _ in per], 0)
-        if chunk_dim is None:
-            hidden = cp.gather_tokens(hidden, N)
-        return self.mixins["final_layer"].final_forward(hidden, **kw)
+        return hidden, kw, cond
+
+    # -- first-block residual cache (scail_b200.step_cache) ---------------------------------------
+    def step_cache_head(self, sc, x, timesteps=None, context=None, y=None, **kwargs):
+        """Embeddings, patch embedding (h0, left in the workspace) and block 0 on the cache's copy of it (h1).  Refuses what
+        the cache does not cover (step_cache.check_supported).  -> StepCacheHead for the indicator and step_cache_tail."""
+        ad = self.mixins["adaln_layer"]
+        step_cache.check_supported(ad.cp, kwargs.get("chunk_dim"), kwargs.get("_num_layers"))
+        h0, kw, _ = self._tokens(x, timesteps, context, y, kwargs)
+        B, N, d = h0.shape
+        bufs = sc.workspace(B, N, d, kw["ref_length"], kw["seq_length"], h0.device)
+        bufs.h1.copy_(h0)
+        ad.layer_forward(bufs.h1, None, layer_id=0, **kw)  # in place: h1 is contiguous bf16
+        return StepCacheHead(h0, bufs, kw)
+
+    def step_cache_tail(self, head, skip):
+        """skip: the noise rows of h1 become bf16(f32(h1) + R).  Otherwise blocks 1..L-1 run on h1, then R = f32(h_L) - f32(h1)
+        on the noise rows.  Then the final layer.  Changes no host-side cache state (the caller commits a computed step)."""
+        bufs, kw = head.buffers, head.kw
+        if skip:
+            ops.step_cache_apply(bufs.h1, bufs.R, bufs.n_ref)
+        else:
+            ad = self.mixins["adaln_layer"]
+            for l in range(1, self.num_layers):
+                ad.layer_forward(bufs.h1, None, layer_id=l, **kw)
+            ops.step_cache_update(bufs.h1, bufs.h1c, bufs.R, bufs.n_ref)
+        return self.mixins["final_layer"].final_forward(bufs.h1, **kw)
+
+
+class StepCacheHead:
+    """What step_cache_head leaves for the rest of a cached forward: h0 (the patch embedding), the cache's Buffers (h1 holds
+    block 0's output) and the layer kwargs."""
+
+    def __init__(self, h0, buffers, kw):
+        self.h0, self.buffers, self.kw = h0, buffers, kw

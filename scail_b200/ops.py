@@ -439,6 +439,57 @@ def cfg_euler_(x, v, scale, dsigma):
     return x
 
 
+# ---------------------------------------------------------------- first-block residual cache (scail_b200.step_cache)
+STEP_CACHE_PARTIALS = 2048  # fp32 partial sums of step_cache_indicator: 2 per CTA, at most 1024 CTAs
+
+
+def _noise_rows(h, t, n_ref, dtype):
+    """(B, N, d, n_seq) of a contiguous bf16 h [B, N, d] and its contiguous noise-row tensor t [B, n_seq, d] of `dtype`."""
+    _req(h), _req(t, dtype)
+    assert h.dim() == 3 and t.dim() == 3 and h.is_contiguous() and t.is_contiguous()
+    B, N, d = h.shape
+    n_seq = t.shape[1]
+    assert t.shape == (B, n_seq, d) and 0 <= n_ref and n_ref + n_seq <= N, (tuple(h.shape), tuple(t.shape), n_ref)
+    return B, N, d, n_seq
+
+
+def step_cache_indicator(h0, h1, r_ref, r_new, h1c, n_ref, partials, out):
+    """r_new = bf16_rn(f32(h1) - f32(h0)), h1c = h1[:, n_ref:n_ref + n_seq], and out (fp64 [4]) = (sum |r_new - r_ref|,
+    sum |r_ref|, their ratio (+inf for a zero denominator), 0) over all B*N*d elements; h0, h1, r_ref, r_new bf16 [B, N, d],
+    h1c bf16 [B, n_seq, d], partials fp32 [>= STEP_CACHE_PARTIALS] scratch.  Bit-reproducible.  Returns out."""
+    B, N, d, n_seq = _noise_rows(h1, h1c, n_ref, torch.bfloat16)
+    for t in (h0, r_ref, r_new):
+        _req(t)
+        assert t.shape == h1.shape and t.is_contiguous()
+    _req(partials, torch.float32), _req(out, torch.float64)
+    assert partials.is_contiguous() and out.is_contiguous() and out.numel() >= 4
+    _lib.check(_lib.lib().scail_step_cache_indicator(_ptr(h0), _ptr(h1), _ptr(r_ref), _ptr(r_new), _ptr(h1c), _ptr(partials),
+                                                     partials.numel(), _ptr(out), B, N, d, n_ref, n_seq, _stream()),
+               "scail_step_cache_indicator")
+    _count(2)
+    return out
+
+
+def step_cache_update(h, h1c, R, n_ref):
+    """R (fp32 [B, n_seq, d]) = f32(h[:, n_ref:n_ref + n_seq]) - f32(h1c); h bf16 [B, N, d], h1c bf16 [B, n_seq, d]."""
+    B, N, d, n_seq = _noise_rows(h, R, n_ref, torch.float32)
+    _req(h1c)
+    assert h1c.shape == R.shape and h1c.is_contiguous()
+    _lib.check(_lib.lib().scail_step_cache_update(_ptr(h), _ptr(h1c), _ptr(R), B, N, d, n_ref, n_seq, _stream()),
+               "scail_step_cache_update")
+    _count()
+    return R
+
+
+def step_cache_apply(h, R, n_ref):
+    """In place: h[:, n_ref:n_ref + n_seq] = bf16_rn(f32(h[:, n_ref:n_ref + n_seq]) + R); h bf16 [B, N, d], R fp32
+    [B, n_seq, d].  Returns h."""
+    B, N, d, n_seq = _noise_rows(h, R, n_ref, torch.float32)
+    _lib.check(_lib.lib().scail_step_cache_apply(_ptr(h), _ptr(R), B, N, d, n_ref, n_seq, _stream()), "scail_step_cache_apply")
+    _count()
+    return h
+
+
 def cast_bf16(x):
     _req(x, torch.float32)
     out = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16)

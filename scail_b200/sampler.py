@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .step_cache import check_supported
 
 
 def make_flow_timesteps(num_steps=50, shift_scale=5.0, t_start=0.0):
@@ -30,12 +31,16 @@ def prepare_context(cond, uc):
 
 
 def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, plan=None, _x_override=None, _sigma_override=None,
-                 **model_kwargs):
+                 step_cache=None, **model_kwargs):
     """One reference sampler step: x [1,t,16,h,w] fp32 (updated in place and returned).
     cond/uc: dicts with 'crossattn' [1,L,text_dim]; cond also carries ref_concat, concat_smpl_render,
     image_clip_features, concat_images (shared by both CFG branches, guiders.py:50-56).
     plan: an optional scail_b200.parallel.HybridParallel — this rank then runs ONE CFG branch (b = 1) and the two
-    velocities are exchanged between partner ranks before the combine."""
+    velocities are exchanged between partner ranks before the combine.
+    step_cache: an optional scail_b200.step_cache.FirstBlockCache, passed to the forward (single GPU only)."""
+    if step_cache is not None:
+        check_supported(plan=plan)
+        model_kwargs["_step_cache"] = step_cache
     ctx = _ctx if _ctx is not None else prepare_context(cond, uc)
     kw = dict(y=None, ref_concat=cond["ref_concat"], concat_smpl_render=cond["concat_smpl_render"],
               image_clip_features=cond["image_clip_features"], concat_images=cond.get("concat_images"), **model_kwargs)
@@ -52,9 +57,13 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     return ops.cfg_euler_(x, v.contiguous(), scale, float(next_sigma) - float(sigma))
 
 
-def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None):
+def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None, step_cache=None):
     """RFSampler.__call__ (sampling.py:965-982): the full Euler loop.  With `adaln_layer.cache_cross_kv` the step-invariant
-    conditioning (text / CLIP embeddings and all layers' cross-attention K,V) is computed once for this call."""
+    conditioning (text / CLIP embeddings and all layers' cross-attention K,V) is computed once for this call.  step_cache (a
+    scail_b200.step_cache.FirstBlockCache) is reset here and then decides on every step whether blocks 1..L-1 run."""
+    if step_cache is not None:
+        check_supported(plan=plan)
+        step_cache.reset()
     sig = make_flow_timesteps(num_steps, shift_scale)
     ctx = prepare_context(cond, uc)
     cache = getattr(model.mixins["adaln_layer"], "cache_cross_kv", False) if hasattr(model, "mixins") else False
@@ -63,7 +72,7 @@ def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=No
         model.set_conditioning(ctx, cond["image_clip_features"], batch=2)
     try:
         for i in range(num_steps):
-            x = sampler_step(model, x, sig[i], sig[i + 1], cond, uc, scale, _ctx=ctx, plan=plan)
+            x = sampler_step(model, x, sig[i], sig[i + 1], cond, uc, scale, _ctx=ctx, plan=plan, step_cache=step_cache)
     finally:
         if cache:
             model.clear_conditioning()
@@ -142,9 +151,15 @@ class GraphedStep:
     bit-identical to `sampler_step` (same kernels, same order).  Single-GPU path (NCCL collectives are not captured).
     The graph runs in the `fp8_linear`, `fp8_attention` and `attention_window` modes of construction time; a window's tile map
     is held by scail_b200.sparse for the life of the process, so the graph reads it at a fixed address.  With fp8 it reads the e4m3 weight copies in place: every
-    call first re-derives, into the same buffers, the copies of weights that changed since (e.g. after load_state_dict)."""
+    call first re-derives, into the same buffers, the copies of weights that changed since (e.g. after load_state_dict).
+    step_cache (a scail_b200.step_cache.FirstBlockCache): the step runs as three graphs with the host's skip decision between
+    them (bit-identical to sampler_step with the same cache and thresholds).  The cache is reset at construction; when its
+    buffers are dropped or replaced later (reset(), another geometry) the graphs are captured again, and the next step
+    computes."""
 
-    def __init__(self, model, x, cond, uc, scale=4.0):
+    def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None):
+        if step_cache is not None:
+            check_supported(getattr(model.mixins["adaln_layer"], "cp", None))
         if getattr(model.mixins["adaln_layer"], "cp", None) is not None:
             raise NotImplementedError("GraphedStep captures the single-GPU forward; use sampler_step under context parallelism")
         self.model, self.scale = model, scale
@@ -159,6 +174,11 @@ class GraphedStep:
         self.fp8 = getattr(self.adaln, "fp8_linear", False)
         # the e4m3 weights are derived on this stream and held here: the graph replays against these very buffers
         self._fp8_weights = self.adaln.prepare_fp8_weights() if self.fp8 else []
+        self.step_cache = step_cache
+        if step_cache is not None:
+            step_cache.reset()
+            self._capture_cached()
+            return
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():  # warm-up on the capture stream: workspaces and TMA descriptors exist
@@ -174,12 +194,59 @@ class GraphedStep:
     def _forward(self):
         return self.model(torch.cat([self.x, self.x], 0), timesteps=self.ts, context=self.ctx, **self.kw).contiguous()
 
+    def _head(self):
+        return self.model.step_cache_head(self.step_cache, torch.cat([self.x, self.x], 0), timesteps=self.ts, context=self.ctx,
+                                          **self.kw)
+
+    def _capture_cached(self):
+        """The first-block cache's three graphs, sharing one memory pool and replayed in capture order: (1) embeddings, patch
+        embedding and block 0; (2) blocks 1..L-1, the R update and the final layer; (3) the R apply and the final layer.  The
+        indicator runs between (1) and (2) or (3) outside the graphs, because its r_ref / r_new alternate between two buffers
+        and a graph would fix them."""
+        self.graphs = self.head = self.v_run = self.v_skip = None
+        dev = self.x.device
+        if getattr(self, "_side", None) is None:  # one capture stream for every (re)capture: one set of stream workspaces
+            self._side = torch.cuda.Stream(device=dev)
+        side = self._side
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side), torch.no_grad():  # warm-up of every path: workspaces and TMA descriptors exist
+            head = self._head()
+            head.buffers.indicator(head.h0)
+            self.model.step_cache_tail(head, False)
+            self.model.step_cache_tail(head, True)
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.step_cache.has_state = False  # the warm-up overwrote R: the next step computes
+        graphs = [torch.cuda.CUDAGraph() for _ in range(3)]
+        n0 = ops.LAUNCHES
+        with torch.cuda.graph(graphs[0], stream=side), torch.no_grad():
+            self.head = self._head()
+        pool = graphs[0].pool()
+        with torch.cuda.graph(graphs[1], stream=side, pool=pool), torch.no_grad():
+            self.v_run = self.model.step_cache_tail(self.head, False).contiguous()
+        with torch.cuda.graph(graphs[2], stream=side, pool=pool), torch.no_grad():
+            self.v_skip = self.model.step_cache_tail(self.head, True).contiguous()
+        self.graphs = graphs
+        self.kernels_in_graph = ops.LAUNCHES - n0
+
     def __call__(self, sigma, next_sigma):
         if self.fp8:
             self.adaln.prepare_fp8_weights()
         self.ts.fill_(float(sigma) * 1000.0)
-        self.graph.replay()
-        return ops.cfg_euler_(self.x, self.v, self.scale, float(next_sigma) - float(sigma))
+        if self.step_cache is None:
+            self.graph.replay()
+            return ops.cfg_euler_(self.x, self.v, self.scale, float(next_sigma) - float(sigma))
+        sc = self.step_cache
+        if sc.buffers is not self.head.buffers:  # reset() or another geometry since the capture dropped the captured buffers
+            self._capture_cached()
+        self.graphs[0].replay()
+        bufs = self.head.buffers
+        bufs.indicator(self.head.h0)
+        skip = sc.decide(bufs.read_indicator())
+        self.graphs[2 if skip else 1].replay()
+        if not skip:
+            sc.computed()
+        return ops.cfg_euler_(self.x, self.v_skip if skip else self.v_run, self.scale, float(next_sigma) - float(sigma))
 
 
 class HostStep:
