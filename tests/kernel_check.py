@@ -13,7 +13,12 @@ reference's (summation order, approximate exp / rsqrt): those differences are ~1
 largest output.  Composite results (several bf16 roundings in a chain) pass looser `elem_rel` / `elem_abs` and say why at
 the call.
 
-Everything is computed on the tensors' own device (no copy to the host), in fp32."""
+Everything is computed on the tensors' own device (no copy to the host), in fp32.
+
+`recording` finds the launches to check: it wraps entry points of a module while a real workload runs and keeps one entry per
+distinct launch, so that each can be re-run on fresh data against a reference."""
+import contextlib
+import inspect
 from collections import namedtuple
 
 import torch
@@ -54,3 +59,34 @@ def assert_close_bf16(got, want, what, rel_l2=4e-3, elem_rel=ELEM_REL, elem_abs=
                           f"{elem_abs:.3g} max|want| (rel-L2 {c.rel_l2:.3e}); {where}")
     assert c.rel_l2 <= rel_l2, f"{what}: rel-L2 {c.rel_l2:.3e} > {rel_l2:.1e}; {where}"
     return c
+
+
+@contextlib.contextmanager
+def recording(module, names, fields):
+    """Replace module.<name> for each of `names` by a recorder that calls through to the original, and restore them on exit.
+
+    fields(name, arguments) -> (key, value) for one call, where `arguments` maps every parameter to its value (defaults
+    applied): `key` is a dict of what makes two calls the same launch, `value` a number kept as the maximum over the calls
+    with that key.  Yields `seen`, a dict {(name, tuple(key.items())): value} in first-call order."""
+    seen = {}
+    originals = {name: getattr(module, name) for name in names}
+
+    def recorder(name, fn):
+        sig = inspect.signature(fn)
+
+        def rec(*args, **kwargs):
+            b = sig.bind(*args, **kwargs)
+            b.apply_defaults()
+            key, value = fields(name, b.arguments)
+            k = (name, tuple(key.items()))
+            seen[k] = value if k not in seen else max(seen[k], value)
+            return fn(*args, **kwargs)
+        return rec
+
+    try:
+        for name, fn in originals.items():
+            setattr(module, name, recorder(name, fn))
+        yield seen
+    finally:
+        for name, fn in originals.items():
+            setattr(module, name, fn)

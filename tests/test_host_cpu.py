@@ -57,7 +57,8 @@ def test_product_does_not_import_oracle():
 def test_rope_tables_bit_identical_to_oracle():
     from oracle import dit_oracle as O
     from scail_b200 import rope
-    for (T, H, W) in [(3, 4, 6), (4, 8, 8), (21, 32, 32)]:
+    # the token grids of 512x512, 512x896 (landscape and portrait) and 480x832 latents
+    for (T, H, W) in [(3, 4, 6), (4, 8, 8), (21, 32, 32), (21, 32, 56), (21, 56, 32), (21, 30, 52)]:
         c, s = rope.build_tables_cpu(128, T, H, W)
         c2, s2 = O.rope_tables(128, T, H, W, 21, 150, 150)
         assert torch.equal(c, c2) and torch.equal(s, s2)

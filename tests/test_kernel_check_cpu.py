@@ -1,9 +1,12 @@
 """kernel_check.assert_close_bf16 on the CPU: a once-rounded bf16 result passes, and one wrong pixel in a large
-channels-last tensor fails it although rel-L2 alone would let it through (the reason the elementwise bound exists)."""
+channels-last tensor fails it although rel-L2 alone would let it through (the reason the elementwise bound exists).  And
+kernel_check.recording on a fake module."""
+import types
+
 import pytest
 import torch
 
-from kernel_check import assert_close_bf16, measure
+from kernel_check import assert_close_bf16, measure, recording
 
 
 def test_once_rounded_bf16_passes():
@@ -55,3 +58,32 @@ def test_fp32_result_is_not_modified_and_worst_value_is_its_own():
     with pytest.raises(AssertionError, match=f"got {float(got[1, 4, 8, 3]):.6g}, want {float(want[1, 4, 8, 3]):.6g}"):
         assert_close_bf16(got, want, "fp32")
     assert torch.equal(got, got_before)
+
+
+def test_recording_keys_launches_and_restores_the_module():
+    """The launch recorder on a fake module: calls are bound to the signature (positional, keyword and default arguments key
+    alike), distinct keys are kept in first-call order with the maximum value, the originals run and come back on exit, and
+    names not listed are left alone."""
+    calls = []
+
+    def gemm(a, w, out=None, rows_per_batch=0):
+        calls.append((a, w))
+        return a * w
+
+    def other(x):
+        return -x
+
+    fake = types.SimpleNamespace(gemm=gemm, other=other)
+    fields = lambda name, a: (dict(a=a["a"] % 10, rpb=a["rows_per_batch"]), a["w"])
+    with recording(fake, ["gemm"], fields) as seen:
+        assert fake.gemm is not gemm and fake.other is other
+        assert fake.gemm(3, 2) == 6
+        fake.gemm(13, w=5, rows_per_batch=0)  # the same key as the first call: the value becomes the maximum
+        fake.gemm(a=4, w=1, rows_per_batch=7)
+        fake.gemm(13, 1)
+    assert fake.gemm is gemm and fake.other is other
+    assert calls == [(3, 2), (13, 5), (4, 1), (13, 1)]
+    assert list(seen.items()) == [(("gemm", (("a", 3), ("rpb", 0))), 5), (("gemm", (("a", 4), ("rpb", 7))), 1)]
+    with pytest.raises(ValueError), recording(fake, ["gemm", "other"], fields):
+        raise ValueError  # an exception inside the block still restores the module
+    assert fake.gemm is gemm and fake.other is other

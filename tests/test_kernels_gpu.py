@@ -116,8 +116,9 @@ def test_rmsnorm_rope(D, heads):
 
 @pytest.mark.parametrize("M,N,K,epi", [(2048, 2560, 512, 0), (2176, 2304, 640, 2), (4100, 1288, 256, 1), (256, 18944, 128, 3)])
 def test_gemm_cta_pair_kernel(M, N, K, epi):
-    """Shapes with >= 74 tile pairs take the cta_group::2 kernel (256 x 256 tiles over two CTAs): ragged M / N edges,
-    every fused epilogue, against an fp32 reference."""
+    """Shapes with more 128 x 256 output tiles (148 to 198) than the H100 has SMs, so the persistent CTAs each loop over
+    more than one tile: ragged M / N edges (M = 4100, N = 1288), a gate that changes batch every 1024 rows, and the bias,
+    GELU-tanh, gate+residual and residual epilogues, against an fp32 reference."""
     from scail_b200 import ops
     a, w, b = rnd(M, K, seed=1), rnd(N, K, seed=2) * 0.05, rnd(N, seed=3)
     ref = a.float() @ w.float().t() + b.float()

@@ -16,13 +16,12 @@ test_oracle_golden.py): the full-width encoder on a single 480x832 frame, on 5 f
 (row-tile kernel at 96 / 192 / 384 channels) and on one frame followed by zero frames; a single-frame decode (the
 upsample3d T = 1 branch); and the mid-block attention at 64x112 = 7168 tokens."""
 import contextlib
-import inspect
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from kernel_check import assert_close_bf16
+from kernel_check import assert_close_bf16, recording
 
 pytestmark = pytest.mark.gpu
 
@@ -132,26 +131,10 @@ def _fields(name, a):
 def launches():
     """[(op, fields, frames)] of every distinct launch at the production geometries, in first-call order."""
     from scail_b200 import ops
-    seen = {}
-
-    def recorder(name, fn):
-        sig = inspect.signature(fn)
-
-        def rec(*args, **kwargs):
-            b = sig.bind(*args, **kwargs)
-            b.apply_defaults()
-            f, T = _fields(name, b.arguments)
-            key = (name, tuple(f.items()))
-            seen[key] = max(seen.get(key, 0), T)
-            return fn(*args, **kwargs)
-        return rec
-
     vae = _random_vae(0)
     g = torch.Generator(device="cuda").manual_seed(0)
     video = lambda T, H, W: torch.rand(3, T, H, W, device="cuda", generator=g) * 2 - 1
-    with pytest.MonkeyPatch.context() as mp:
-        for name in OPS:
-            mp.setattr(ops, name, recorder(name, getattr(ops, name)))
+    with recording(ops, OPS, _fields) as seen:
         for T, h, w in DECODE_LATENTS:
             vae.decode([torch.randn(16, T, h, w, device="cuda", generator=g)])
         vae.decode([torch.randn(16, *CHUNKED_DECODE, device="cuda", generator=g)], chunk_frames=1)
