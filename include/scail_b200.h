@@ -136,6 +136,36 @@ int scail_attention_sparse(const void* Q, int64_t ldq, const void* K, int64_t ld
                            int64_t kv_batch_rows, int64_t q_rows_total, int64_t kv_rows_total, float scale, int accumulate,
                            const int32_t* kv_tile_ptr, const int32_t* kv_tile_idx, int64_t nnz, scail_stream_t stream);
 
+/* Per-(batch, head) block-sparse self-attention: as scail_attention_sparse, but (b, h) reads its own CSR map, kv_tile_ptr +
+ * (b*H + h) * ptr_stride (ceil(L/128) + 1 entries from 0) and kv_tile_idx + (b*H + h) * idx_stride, with
+ * ptr_stride >= ceil(L/128) + 1 and idx_stride >= ceil(L/128)^2 (the slot capacity).  No host nnz: the maps may be built on
+ * the device (scail_attention_select_tiles), and their contents are trusted. */
+int scail_attention_sparse_bh(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, void* out,
+                              int64_t ldo, int64_t B, int64_t H, int64_t L, int64_t q_batch_rows, int64_t kv_batch_rows,
+                              int64_t q_rows_total, int64_t kv_rows_total, float scale, const int32_t* kv_tile_ptr,
+                              int64_t ptr_stride, const int32_t* kv_tile_idx, int64_t idx_stride, scail_stream_t stream);
+/* Per-(batch, head) form of scail_attention_fp8_sparse: the maps and strides as scail_attention_sparse_bh. */
+int scail_attention_fp8_sparse_bh(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk,
+                                  const float* k_scale, const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B,
+                                  int64_t H, int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
+                                  int64_t ptr_stride, const int32_t* kv_tile_idx, int64_t idx_stride, scail_stream_t stream);
+/* Tile pooling for adaptive tile selection: out fp32 [B, H, ceil(L/128), 128] = the mean over each 128-row tile's valid rows
+ * of one self-attention operand, x [B*L, ldx] with head h at columns [h*128, h*128+128).  fp8 == 0: x is bf16 and x_scale
+ * NULL.  fp8 == 1: x is e4m3 and the value is x * x_scale[b, h, row] with x_scale fp32 [B, H, L_pad]
+ * (scail_rmsnorm_rope_fp8).  Summed in ascending row order in fp64: bit-reproducible. */
+int scail_attention_tile_pool(const void* x, int64_t ldx, const float* x_scale, int fp8, float* out, int64_t B, int64_t H,
+                              int64_t L, int64_t L_pad, scail_stream_t stream);
+/* Adaptive tile selection on the device.  qbar, kbar fp32 [B, H, n, 128] (scail_attention_tile_pool), n = ceil(L/128).
+ * Query tile q of (b, h) lists the key tiles with e_k = n_k exp(s_k - max s), s_k = qbar_q . kbar_k / sqrt(128), n_k the
+ * valid keys of tile k: always k == q and every k < ceil(n_ref/128) (reference tokens), then the others by e_k descending
+ * (ties: lower k) until the listed sum reaches mass * sum_k e_k or max_tiles were taken that way (max_tiles < 0: no cap).
+ * mass >= 1 takes every tile (up to the cap); mass == 0 only the forced ones.  Writes the per-(b, h) maps of
+ * scail_attention_sparse_bh (rows ascending).  scratch: int32, at least B*H*n*(1 + ceil(n/32)) entries (scratch_len).
+ * n <= 2048.  No host synchronisation: the selection can be captured in a CUDA graph. */
+int scail_attention_select_tiles(const float* qbar, const float* kbar, int64_t B, int64_t H, int64_t L, int64_t n_ref, double mass,
+                                 int64_t max_tiles, int32_t* kv_tile_ptr, int64_t ptr_stride, int32_t* kv_tile_idx,
+                                 int64_t idx_stride, int32_t* scratch, int64_t scratch_len, scail_stream_t stream);
+
 /* Context parallelism: attention over a SUBSET of the keys, to be merged later.  Keys are the rows
  * [kv_off0, kv_off0 + kv_len0) and (optionally, kv_len1 > 0) [kv_off1, kv_off1 + kv_len1) of every batch of kv_batch_rows rows
  * ("every shard but mine").  Writes the partial result normalised by its own row sum as float32 o32 [rows, ldo32] and

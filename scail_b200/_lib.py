@@ -41,6 +41,13 @@ SIGNATURES = {
                         c_i64, c_i64, c_f, c_int, c_p],
     "scail_attention_sparse": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                                c_i64, c_i64, c_f, c_int, c_p, c_p, c_i64, c_p],
+    "scail_attention_sparse_bh": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                  c_i64, c_f, c_p, c_i64, c_p, c_i64, c_p],
+    "scail_attention_fp8_sparse_bh": [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                      c_i64, c_f, c_p, c_i64, c_p, c_i64, c_p],
+    "scail_attention_tile_pool": [c_p, c_i64, c_p, c_int, c_p, c_i64, c_i64, c_i64, c_i64, c_p],
+    "scail_attention_select_tiles": [c_p, c_p, c_i64, c_i64, c_i64, c_i64, ctypes.c_double, c_i64, c_p, c_i64, c_p, c_i64,
+                                     c_p, c_i64, c_p],
     "scail_attention_partial": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                                 c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
     "scail_attention_merge": [c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_p],

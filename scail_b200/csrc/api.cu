@@ -14,6 +14,7 @@
 #include <unordered_map>
 
 #include "../../include/scail_b200.h"
+#include "adaptive.cuh"
 #include "attention.cuh"
 #include "conv.cuh"
 #include "gemm.cuh"
@@ -531,7 +532,7 @@ static int check_tile_map(const char* what, const int32_t* kv_tile_ptr, const in
 static int attention_fp8_impl(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
                               const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H,
                               int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
-                              const int32_t* kv_tile_idx, scail_stream_t stream) {
+                              const int32_t* kv_tile_idx, scail_stream_t stream, int64_t ptr_stride = 0, int64_t idx_stride = 0) {
     using namespace scail;
     SCAIL_REQUIRE(Q && q_scale && K && k_scale && vt && v_scale && out, "attention_fp8: null operand");
     SCAIL_REQUIRE(head_dim == ATT_D, "attention_fp8: head_dim=%lld, only 128 is supported", (long long)head_dim);
@@ -555,6 +556,7 @@ static int attention_fp8_impl(const void* Q, int64_t ldq, const float* q_scale, 
     p.L = (int)L; p.L_pad = (int)L_pad; p.heads = (int)H;
     p.scale_log2 = scale * 1.4426950408889634f;
     p.kv_tile_ptr = kv_tile_ptr; p.kv_tile_idx = kv_tile_idx;
+    p.ptr_stride = ptr_stride; p.idx_stride = idx_stride;
     dim3 grid((unsigned)(L_pad / ATT_BQ), (unsigned)H, (unsigned)B);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (kv_tile_ptr) {
@@ -589,7 +591,8 @@ static int attention_impl(const void* Q, int64_t ldq, const void* K, int64_t ldk
                           int64_t ldo, int64_t B, int64_t H, int64_t q_len, int64_t kv_off0, int64_t kv_len0, int64_t kv_off1,
                           int64_t kv_len1, int64_t q_batch_rows, int64_t kv_batch_rows, int64_t q_rows_total,
                           int64_t kv_rows_total, float scale, int accumulate, float* o32, int64_t ldo32, void* state,
-                          const int32_t* kv_tile_ptr, const int32_t* kv_tile_idx, scail_stream_t stream) {
+                          const int32_t* kv_tile_ptr, const int32_t* kv_tile_idx, scail_stream_t stream,
+                          int64_t ptr_stride = 0, int64_t idx_stride = 0) {
     using namespace scail;
     SCAIL_REQUIRE(Q && K && V && (out || o32), "attention: null operand");
     SCAIL_REQUIRE(B > 0 && H > 0 && q_len > 0 && kv_len0 > 0 && kv_len1 >= 0 && kv_off0 >= 0 && kv_off1 >= 0, "attention: bad shape");
@@ -614,6 +617,7 @@ static int attention_impl(const void* Q, int64_t ldq, const void* K, int64_t ldk
     p.scale_log2 = scale * 1.4426950408889634f;
     p.accumulate = accumulate;
     p.kv_tile_ptr = kv_tile_ptr; p.kv_tile_idx = kv_tile_idx;
+    p.ptr_stride = ptr_stride; p.idx_stride = idx_stride;
     dim3 grid(blocks_for(q_len, ATT_BQ), (unsigned)H, (unsigned)B);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (kv_tile_ptr) {
@@ -645,6 +649,95 @@ int scail_attention_sparse(const void* Q, int64_t ldq, const void* K, int64_t ld
     if ((rc = check_tile_map("attention_sparse", kv_tile_ptr, kv_tile_idx, nnz, q_len, kv_len))) return rc;
     return attention_impl(Q, ldq, K, ldk, V, ldv, out, ldo, B, H, q_len, 0, kv_len, 0, 0, q_batch_rows, kv_batch_rows, q_rows_total,
                           kv_rows_total, scale, accumulate, nullptr, 0, nullptr, kv_tile_ptr, kv_tile_idx, stream);
+}
+
+// Host checks of per-(batch, head) maps (scail_attention_sparse_bh, scail_attention_select_tiles): pointers, alignment and
+// strides that give every (b, h) a slot of n_q + 1 row pointers and n_q * n_kv indices.
+static int check_bh_maps(const char* what, const void* kv_tile_ptr, int64_t ptr_stride, const void* kv_tile_idx,
+                         int64_t idx_stride, int64_t L) {
+    SCAIL_REQUIRE(kv_tile_ptr && kv_tile_idx, "%s: null tile map", what);
+    SCAIL_REQUIRE(aligned4(kv_tile_ptr) && aligned4(kv_tile_idx), "%s: kv_tile_ptr and kv_tile_idx must be 4-byte aligned int32", what);
+    SCAIL_REQUIRE(L > 0, "%s: L=%lld must be positive", what, (long long)L);
+    const int64_t n = (L + scail::ATT_BKV - 1) / scail::ATT_BKV;
+    SCAIL_REQUIRE(ptr_stride >= n + 1, "%s: ptr_stride=%lld must be >= n_q_tiles + 1 = %lld", what, (long long)ptr_stride,
+                  (long long)(n + 1));
+    SCAIL_REQUIRE(idx_stride >= n * n, "%s: idx_stride=%lld must be >= n_q_tiles * n_kv_tiles = %lld", what, (long long)idx_stride,
+                  (long long)(n * n));
+    return 0;
+}
+
+int scail_attention_sparse_bh(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, void* out,
+                              int64_t ldo, int64_t B, int64_t H, int64_t L, int64_t q_batch_rows, int64_t kv_batch_rows,
+                              int64_t q_rows_total, int64_t kv_rows_total, float scale, const int32_t* kv_tile_ptr,
+                              int64_t ptr_stride, const int32_t* kv_tile_idx, int64_t idx_stride, scail_stream_t stream) {
+    int rc;
+    if ((rc = check_bh_maps("attention_sparse_bh", kv_tile_ptr, ptr_stride, kv_tile_idx, idx_stride, L))) return rc;
+    return attention_impl(Q, ldq, K, ldk, V, ldv, out, ldo, B, H, L, 0, L, 0, 0, q_batch_rows, kv_batch_rows, q_rows_total,
+                          kv_rows_total, scale, 0, nullptr, 0, nullptr, kv_tile_ptr, kv_tile_idx, stream, ptr_stride, idx_stride);
+}
+
+int scail_attention_fp8_sparse_bh(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk,
+                                  const float* k_scale, const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B,
+                                  int64_t H, int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
+                                  int64_t ptr_stride, const int32_t* kv_tile_idx, int64_t idx_stride, scail_stream_t stream) {
+    int rc;
+    if ((rc = check_bh_maps("attention_fp8_sparse_bh", kv_tile_ptr, ptr_stride, kv_tile_idx, idx_stride, L))) return rc;
+    return attention_fp8_impl(Q, ldq, q_scale, K, ldk, k_scale, vt, v_scale, out, ldo, B, H, head_dim, L, L_pad, scale,
+                              kv_tile_ptr, kv_tile_idx, stream, ptr_stride, idx_stride);
+}
+
+int scail_attention_tile_pool(const void* x, int64_t ldx, const float* x_scale, int fp8, float* out, int64_t B, int64_t H,
+                              int64_t L, int64_t L_pad, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(x && out, "attention_tile_pool: null operand");
+    SCAIL_REQUIRE(fp8 == 0 || fp8 == 1, "attention_tile_pool: fp8=%d must be 0 (bf16) or 1 (e4m3 with scales)", fp8);
+    SCAIL_REQUIRE(fp8 == (x_scale != nullptr), "attention_tile_pool: x_scale must be given exactly when fp8 == 1");
+    SCAIL_REQUIRE(B > 0 && H > 0 && L > 0 && B <= 65535 && H <= 65535,
+                  "attention_tile_pool: bad shape B=%lld H=%lld L=%lld", (long long)B, (long long)H, (long long)L);
+    SCAIL_REQUIRE(ldx >= H * ATT_D, "attention_tile_pool: ldx=%lld must be >= H*128 = %lld", (long long)ldx, (long long)(H * ATT_D));
+    SCAIL_REQUIRE(!fp8 || (L_pad % 128 == 0 && L <= L_pad), "attention_tile_pool: L_pad=%lld must be a multiple of 128 and >= L=%lld",
+                  (long long)L_pad, (long long)L);
+    SCAIL_REQUIRE(aligned4(out) && aligned4(x_scale) && (fp8 || (reinterpret_cast<uintptr_t>(x) & 1) == 0),
+                  "attention_tile_pool: out and x_scale must be 4-byte aligned, a bf16 x 2-byte aligned");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    dim3 grid(blocks_for(L, ATT_BKV), (unsigned)H, (unsigned)B);
+    if (fp8) tile_pool_kernel<true><<<grid, ATT_D, 0, st>>>(x, ldx, x_scale, out, (int)L, (int)L_pad, (int)H);
+    else tile_pool_kernel<false><<<grid, ATT_D, 0, st>>>(x, ldx, nullptr, out, (int)L, 0, (int)H);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_attention_select_tiles(const float* qbar, const float* kbar, int64_t B, int64_t H, int64_t L, int64_t n_ref, double mass,
+                                 int64_t max_tiles, int32_t* kv_tile_ptr, int64_t ptr_stride, int32_t* kv_tile_idx,
+                                 int64_t idx_stride, int32_t* scratch, int64_t scratch_len, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(qbar && kbar && scratch, "attention_select_tiles: null operand");
+    SCAIL_REQUIRE(aligned16(qbar) && aligned16(kbar) && aligned4(scratch),
+                  "attention_select_tiles: qbar and kbar must be 16-byte aligned, scratch 4-byte aligned");
+    int rc;
+    if ((rc = check_bh_maps("attention_select_tiles", kv_tile_ptr, ptr_stride, kv_tile_idx, idx_stride, L))) return rc;
+    const int64_t n = (L + ATT_BKV - 1) / ATT_BKV, words = (n + 31) / 32;
+    SCAIL_REQUIRE(B > 0 && H > 0 && B <= 65535 && H <= 65535 && B * H <= 65535 && n <= ADA_MAX_TILES,
+                  "attention_select_tiles: bad shape B=%lld H=%lld L=%lld (B*H <= 65535, ceil(L/128) <= %d)", (long long)B,
+                  (long long)H, (long long)L, ADA_MAX_TILES);
+    SCAIL_REQUIRE(n_ref >= 0 && n_ref <= L, "attention_select_tiles: n_ref=%lld must lie in [0, L=%lld]", (long long)n_ref, (long long)L);
+    SCAIL_REQUIRE(mass >= 0.0 && mass <= 1.0, "attention_select_tiles: mass=%g must lie in [0, 1]", mass);
+    SCAIL_REQUIRE(max_tiles >= -1, "attention_select_tiles: max_tiles=%lld must be >= 0, or -1 for no cap", (long long)max_tiles);
+    SCAIL_REQUIRE(scratch_len >= B * H * n * (1 + words), "attention_select_tiles: scratch holds %lld int32, this shape needs %lld",
+                  (long long)scratch_len, (long long)(B * H * n * (1 + words)));
+    SelectParams p;
+    p.qbar = qbar; p.kbar = kbar;
+    p.heads = (int)H; p.L = (int)L; p.n_t = (int)n; p.n_ref_tiles = (int)((n_ref + ATT_BKV - 1) / ATT_BKV);
+    p.mass = mass; p.max_tiles = (int)(max_tiles < n ? max_tiles : n); p.words = (int)words;
+    p.counts = scratch; p.bits = reinterpret_cast<uint32_t*>(scratch + B * H * n);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int smem = (int)n * (2 * sizeof(double) + sizeof(int));
+    select_tiles_kernel<<<dim3((unsigned)n, (unsigned)H, (unsigned)B), ADA_SELECT_THREADS, smem, st>>>(p);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    compact_tiles_kernel<<<dim3((unsigned)n, (unsigned)(B * H)), 32, 0, st>>>(scratch, p.bits, (int)n, (int)words, kv_tile_ptr,
+                                                                              ptr_stride, kv_tile_idx, idx_stride);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 int scail_attention_partial(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* V, int64_t ldv, float* o32,

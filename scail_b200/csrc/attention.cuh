@@ -45,11 +45,13 @@ struct AttnParams {
     int accumulate;      // out += result (second cross-attention pass, dit_video_crossattn_sc_xc.py:1197)
     const int* kv_tile_ptr;  // block-sparse map (attention_fwd_kernel<true> only, one range, kv_off = 0): query tile t attends
     const int* kv_tile_idx;  // the key tiles kv_tile_idx[kv_tile_ptr[t] .. kv_tile_ptr[t + 1]), strictly ascending
+    int64_t ptr_stride;      // per-(batch, head) maps: (b, h) reads kv_tile_ptr + (b H + h) ptr_stride and kv_tile_idx +
+    int64_t idx_stride;      // (b H + h) idx_stride; both 0: one map serves every (batch, head)
 };
 
 
-// kSparse: the CTA's key tiles are the row blockIdx.x of the block-sparse map (AttnParams::kv_tile_ptr / kv_tile_idx) instead
-// of every tile of the key ranges.  Only the tile list changes: tile j of the row is loaded from key row 128 kv_tile_idx[j],
+// kSparse: the CTA's key tiles are the row blockIdx.x of the block-sparse map (AttnParams::kv_tile_ptr / kv_tile_idx; with
+// non-zero strides, the map of the CTA's own (batch, head)) instead of every tile of the key ranges.  Only the tile list changes: tile j of the row is loaded from key row 128 kv_tile_idx[j],
 // its valid-key mask is taken from that global start, and the turns run over the row's n_kv tiles exactly as below.
 template <bool kSparse>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
@@ -77,8 +79,10 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     const int head = blockIdx.y;
     const int batch = blockIdx.z;
     const int q0 = blockIdx.x * ATT_BQ;
-    const int* kv_tiles = kSparse ? p.kv_tile_idx + p.kv_tile_ptr[blockIdx.x] : nullptr;
-    const int n_kv0 = kSparse ? p.kv_tile_ptr[blockIdx.x + 1] - p.kv_tile_ptr[blockIdx.x] : (p.kv_len + ATT_BKV - 1) / ATT_BKV;
+    const int64_t bh_map = kSparse ? static_cast<int64_t>(batch) * p.heads + head : 0;  // this (b, h)'s map
+    const int* tile_ptr = kSparse ? p.kv_tile_ptr + bh_map * p.ptr_stride : nullptr;
+    const int* kv_tiles = kSparse ? p.kv_tile_idx + bh_map * p.idx_stride + tile_ptr[blockIdx.x] : nullptr;
+    const int n_kv0 = kSparse ? tile_ptr[blockIdx.x + 1] - tile_ptr[blockIdx.x] : (p.kv_len + ATT_BKV - 1) / ATT_BKV;
     const int n_kv = kSparse ? n_kv0 : n_kv0 + (p.kv_len1 + ATT_BKV - 1) / ATT_BKV;
 
     if (warp == 0 && lane == 0) {
@@ -318,6 +322,7 @@ struct Attn8Params {
     float scale_log2;       // softmax scale * log2(e)
     const int* kv_tile_ptr;  // block-sparse map (attention_fp8_kernel<true> only), as AttnParams
     const int* kv_tile_idx;
+    int64_t ptr_stride, idx_stride;  // per-(batch, head) maps, as AttnParams (0: shared)
 };
 
 // kSparse: the block-sparse map selects the CTA's key tiles, as in attention_fwd_kernel<true>; tile j's K rows, K scales
@@ -349,10 +354,11 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     const int head = blockIdx.y;
     const int batch = blockIdx.z;
     const int q0 = blockIdx.x * ATT_BQ;
-    const int* kv_tiles = kSparse ? p.kv_tile_idx + p.kv_tile_ptr[blockIdx.x] : nullptr;
-    const int n_kv = kSparse ? p.kv_tile_ptr[blockIdx.x + 1] - p.kv_tile_ptr[blockIdx.x] : (p.L + ATT_BKV - 1) / ATT_BKV;
-    auto kv_start = [&](int j) { return (kSparse ? kv_tiles[j] : j) * ATT_BKV; };  // first key of the CTA's tile j
     const int64_t bh = static_cast<int64_t>(batch) * p.heads + head;
+    const int* tile_ptr = kSparse ? p.kv_tile_ptr + bh * p.ptr_stride : nullptr;  // this (b, h)'s map
+    const int* kv_tiles = kSparse ? p.kv_tile_idx + bh * p.idx_stride + tile_ptr[blockIdx.x] : nullptr;
+    const int n_kv = kSparse ? tile_ptr[blockIdx.x + 1] - tile_ptr[blockIdx.x] : (p.L + ATT_BKV - 1) / ATT_BKV;
+    auto kv_start = [&](int j) { return (kSparse ? kv_tiles[j] : j) * ATT_BKV; };  // first key of the CTA's tile j
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_q);

@@ -297,7 +297,7 @@ class AdaLNMixin(BaseMixin):
     def __init__(self, hidden_size, num_layers, time_embed_dim, compressed_num_frames, transformer_args, qk_ln=True,
                  qk_ln_affine=None, hidden_size_head=None, params_dtype=torch.float, device=torch.device("cpu"),
                  elementwise_affine=True, share_adaln=False, use_i2v_clip=False, fp8_linear=False, fp8_attention=False,
-                 attention_window=None):
+                 attention_window=None, attention_adaptive=None):
         super().__init__()
         if not (qk_ln and share_adaln and use_i2v_clip) or hidden_size_head != hidden_size:
             raise NotImplementedError("scail_b200 implements qk_ln=True over the full hidden width, share_adaln=True, use_i2v_clip=True")
@@ -335,6 +335,13 @@ class AdaLNMixin(BaseMixin):
         # keys within w frames of its own (the ref rows and the ref keys stay dense), through the sparse forms of whichever
         # self-attention kernel runs (bf16 or fp8_attention).  A plain attribute, toggled between forwards like fp8_attention.
         self.attention_window = None if attention_window is None else sparse.check_window(attention_window)
+        # Opt-in content-adaptive block-sparse self-attention (scail_b200.sparse.AdaptiveTiles): None is dense; otherwise every
+        # layer and forward chooses per-(batch, head) tile maps on the device from tile-pooled Q and K, and the per-(batch,
+        # head) sparse form of whichever self-attention kernel runs.  Not combinable with attention_window.  A plain
+        # attribute, toggled between forwards like attention_window.
+        self.attention_adaptive = sparse.check_adaptive(attention_adaptive)
+        if self.attention_window is not None and self.attention_adaptive is not None:
+            raise ValueError("attention_window and attention_adaptive cannot be combined: set one of them")
 
     # -- fp8 linears ---------------------------------------------------------------------------
     FP8_LINEARS = ("attention.query_key_value", "attention.dense", "cross_attention.query", "cross_attention.dense",
@@ -470,13 +477,17 @@ class AdaLNMixin(BaseMixin):
             self._linear(h2, a.query_key_value, _fp8_scale, out=qkv)
             tiles = self._attention_tiles(dev, N, kw_args)
             if self.fp8_attention:
-                self._self_attention_fp8(qkv, B, N, d, H, wq, wk, cos, sin, ctx, tiles)
+                self._self_attention_fp8(qkv, B, N, d, H, wq, wk, cos, sin, ctx, tiles, kw_args.get("ref_length"))
             else:
                 ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon)
-                if tiles is None:
-                    ops.attention(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, N)
+                q, k, v = qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:]
+                if self.attention_adaptive is not None:
+                    ptr, idx = self.attention_adaptive.select(q, k, B, H, N, self._n_ref(N, kw_args), self._ws(dev))
+                    ops.attention_sparse_bh(q, k, v, ctx, B, H, N, ptr, idx)
+                elif tiles is None:
+                    ops.attention(q, k, v, ctx, B, H, N, N)
                 else:
-                    ops.attention_sparse(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ctx, B, H, N, tiles)
+                    ops.attention_sparse(q, k, v, ctx, B, H, N, tiles)
         else:
             self._refuse_fp8_attention_cp()
             # engine-style sequence parallelism (diffusion_video.py:495-552): the latents arrive pre-chunked on H or W, so the
@@ -492,12 +503,27 @@ class AdaLNMixin(BaseMixin):
         when attention_window is None."""
         if self.attention_window is None:
             return None
+        if self.attention_adaptive is not None:
+            raise ValueError("attention_window and attention_adaptive cannot be combined: set one of them")
         g = sparse.geometry(**kw)
         if g.ref_length + g.seq_length + g.pose_length != N:
             raise ValueError(f"attention_window: the token layout {g} does not add up to the sequence length {N}")
         return sparse.tile_map(g, self.attention_window, dev)
 
-    def _self_attention_fp8(self, qkv, B, N, d, H, wq, wk, cos, sin, ctx, tiles=None):
+    @staticmethod
+    def _n_ref(N, kw):
+        """The reference-token count of this forward's ref || noise || pose layout (attention_adaptive keeps their key tiles)."""
+        n_ref = int(kw["ref_length"])
+        if not 0 <= n_ref <= N:
+            raise ValueError(f"attention_adaptive: ref_length={n_ref} does not fit the sequence length {N}")
+        return n_ref
+
+    @staticmethod
+    def _ws(dev):
+        """The per-stream workspace as a buf(name, shape, dtype) callable (AdaptiveTiles.select)."""
+        return lambda name, shape, dtype: _WS.get(name, shape, dev, dtype)
+
+    def _self_attention_fp8(self, qkv, B, N, d, H, wq, wk, cos, sin, ctx, tiles=None, n_ref=None):
         """Self-attention of the fused QKV buffer in e4m3: RMSNorm+RoPE writes quantised Q and K, the V slab is transposed and
         quantised per channel, then attention_fp8 writes the merged-head context into ctx.  Buffers: per-stream workspace."""
         dev, f32 = qkv.device, torch.float32
@@ -507,7 +533,12 @@ class AdaLNMixin(BaseMixin):
         ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon, out_fp8=[q8, k8])
         vt, vs = ops.quant_vt_fp8(qkv[:, 2 * d:], B, H, N, _WS.get("vt8", (B, H, 128, Lp), dev, ops.FP8),
                                   _WS.get("vt8_scale", (B, H, 128), dev, f32), _WS.get("vt8_amax", (B, d), dev, torch.int32))
-        ops.attention_fp8(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, tiles=tiles)
+        if self.attention_adaptive is not None:
+            ptr, idx = self.attention_adaptive.select(q8[0], k8[0], B, H, N, self._n_ref(N, {"ref_length": n_ref}), self._ws(dev),
+                                                      q_scale=q8[1], k_scale=k8[1])
+            ops.attention_fp8_sparse_bh(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, ptr, idx)
+        else:
+            ops.attention_fp8(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, tiles=tiles)
 
     def _refuse_fp8_attention_cp(self):
         if self.fp8_attention and self.cp is not None and self.cp.size > 1:
@@ -516,6 +547,9 @@ class AdaLNMixin(BaseMixin):
         if self.attention_window is not None and self.cp is not None and self.cp.size > 1:
             raise NotImplementedError("attention_window is not implemented under context parallelism (a ContextParallel of "
                                       f"size {self.cp.size}); set attention_window to None or run without context parallelism")
+        if self.attention_adaptive is not None and self.cp is not None and self.cp.size > 1:
+            raise NotImplementedError("attention_adaptive is not implemented under context parallelism (a ContextParallel of "
+                                      f"size {self.cp.size}); set attention_adaptive to None or run without context parallelism")
 
     def cross_attention_forward(self, hidden_states, cross_attention_mask, encoder_outputs, _ctx_out=None, _fp8_scale=None,
                                 **kw_args):
@@ -591,7 +625,7 @@ class DiffusionTransformer(nn.Module):
                  text_dim=4096, num_layers=40, num_attention_heads=40, elementwise_affine=False, time_freq_dim=256,
                  time_embed_dim=None, modules=None, share_adaln=True, use_SwiGLU=False, use_RMSNorm=False,
                  layernorm_epsilon=1e-6, inner_hidden_size=None, use_i2v_clip=True, dtype="bf16", fp8_linear=False,
-                 fp8_attention=False, attention_window=None, **kwargs):
+                 fp8_attention=False, attention_window=None, attention_adaptive=None, **kwargs):
         super().__init__()
         if use_SwiGLU or use_RMSNorm:
             raise NotImplementedError("SCAIL-14B uses the non-gated GELU-tanh MLP and LayerNorm (yaml:42-43)")
@@ -627,7 +661,8 @@ class DiffusionTransformer(nn.Module):
         self.add_mixin("adaln_layer", AdaLNMixin(d, num_layers, self.time_embed_dim, frames, targs, qk_ln=True,
                                                  qk_ln_affine=True, hidden_size_head=d, elementwise_affine=elementwise_affine,
                                                  share_adaln=True, use_i2v_clip=True, fp8_linear=fp8_linear,
-                                                 fp8_attention=fp8_attention, attention_window=attention_window))
+                                                 fp8_attention=fp8_attention, attention_window=attention_window,
+                                                 attention_adaptive=attention_adaptive))
         self.add_mixin("final_layer", FinalLayerMixin(d, self.time_embed_dim, self.patch_size, out_channels,
                                                       elementwise_affine, layernorm_epsilon, True))
         object.__setattr__(self.mixins["adaln_layer"], "_pos_embed", self.mixins["pos_embed"])

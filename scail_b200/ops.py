@@ -341,6 +341,122 @@ def attention_fp8_sparse(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, ti
     return attention_fp8(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, scale=scale, tiles=tiles)
 
 
+def _bh_maps(ptr, idx, B, H, L, device):
+    """(ptr_stride, idx_stride) of per-(batch, head) maps: int32 ptr [B, H, >= n + 1] and idx [B, H, >= n * n], contiguous."""
+    n = -(-int(L) // ATT_TILE)
+    for t, want, what in ((ptr, n + 1, "kv_tile_ptr"), (idx, n * n, "kv_tile_idx")):
+        _req(t, torch.int32)
+        if t.dim() != 3 or tuple(t.shape[:2]) != (B, H) or t.shape[2] < want or not t.is_contiguous():
+            raise ValueError(f"per-(batch, head) {what} must be a contiguous int32 [B={B}, H={H}, >= {want}], got "
+                             f"{tuple(t.shape)}")
+        if t.device != device:
+            raise ValueError(f"{what} lives on {t.device}, the operands on {device}")
+    return ptr.shape[2], idx.shape[2]
+
+
+def attention_sparse_bh(q, k, v, out, B, H, L, ptr, idx, q_batch_rows=None, kv_batch_rows=None, scale=None):
+    """Block-sparse bf16 self-attention with one map per (batch, head): (b, h) attends as attention_sparse under the CSR map
+    ptr[b, h] (int32 [B, H, >= n + 1], n = ceil(L / 128)) and idx[b, h] (int32 [B, H, >= n * n]).  The maps' contents are
+    not read on the host (select_tiles builds them on the device)."""
+    for t in (q, k, v, out):
+        _req(t)
+        assert t.dim() == 2 and t.stride(1) == 1
+    ps, ids = _bh_maps(ptr, idx, B, H, L, q.device)
+    q_batch_rows = L if q_batch_rows is None else q_batch_rows
+    kv_batch_rows = L if kv_batch_rows is None else kv_batch_rows
+    scale = 1.0 / math.sqrt(128) if scale is None else scale
+    ev = None
+    if ATTN_EVENTS is not None and L > 1024:
+        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+        ev[0].record()
+    _lib.check(_lib.lib().scail_attention_sparse_bh(_ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
+                                                    out.stride(0), B, H, L, q_batch_rows, kv_batch_rows, q.shape[0], k.shape[0],
+                                                    scale, _ptr(ptr), ps, _ptr(idx), ids, _stream()), "scail_attention_sparse_bh")
+    if ev is not None:
+        ev[1].record()
+        ATTN_EVENTS.append(ev)
+    _count()
+    return out
+
+
+def attention_fp8_sparse_bh(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, ptr, idx, scale=None):
+    """FP8 self-attention (operands as attention_fp8) with one block-sparse map per (batch, head), as attention_sparse_bh."""
+    for t in (q8, k8):
+        _req(t, FP8)
+        assert t.dim() == 2 and t.stride(1) == 1 and t.shape == (B * L, H * 128)
+    Lp = fp8_pad(L)
+    for s in (q_scale, k_scale):
+        _req(s, torch.float32)
+        assert s.is_contiguous() and s.shape == (B, H, Lp)
+    _req(vt, FP8), _req(v_scale, torch.float32), _req(out)
+    assert vt.is_contiguous() and vt.shape == (B, H, 128, Lp) and v_scale.is_contiguous() and v_scale.shape == (B, H, 128)
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape == (B * L, H * 128)
+    ps, ids = _bh_maps(ptr, idx, B, H, L, q8.device)
+    scale = 1.0 / math.sqrt(128) if scale is None else scale
+    ev = None
+    if ATTN_EVENTS is not None and L > 1024:
+        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+        ev[0].record()
+    _lib.check(_lib.lib().scail_attention_fp8_sparse_bh(_ptr(q8), q8.stride(0), _ptr(q_scale), _ptr(k8), k8.stride(0),
+                                                        _ptr(k_scale), _ptr(vt), _ptr(v_scale), _ptr(out), out.stride(0), B, H, 128,
+                                                        L, Lp, scale, _ptr(ptr), ps, _ptr(idx), ids, _stream()),
+               "scail_attention_fp8_sparse_bh")
+    if ev is not None:
+        ev[1].record()
+        ATTN_EVENTS.append(ev)
+    _count()
+    return out
+
+
+def tile_pool(x, B, H, L, out=None, x_scale=None):
+    """Tile means of one self-attention operand: x [B*L, H*128] (2-D row-strided view) bf16, or e4m3 with its per-token
+    scales x_scale [B, H, L_pad] -> out fp32 [B, H, ceil(L/128), 128], the mean of each 128-row tile's valid rows (of x *
+    scale for e4m3).  Bit-reproducible."""
+    fp8 = x_scale is not None
+    _req(x, FP8 if fp8 else torch.bfloat16)
+    assert x.dim() == 2 and x.stride(1) == 1 and x.shape == (B * L, H * 128)
+    n = -(-L // ATT_TILE)
+    Lp = fp8_pad(L)
+    if fp8:
+        _req(x_scale, torch.float32)
+        assert x_scale.is_contiguous() and x_scale.shape == (B, H, Lp)
+    if out is None:
+        out = torch.empty(B, H, n, 128, device=x.device, dtype=torch.float32)
+    _req(out, torch.float32)
+    assert out.is_contiguous() and out.shape == (B, H, n, 128)
+    _lib.check(_lib.lib().scail_attention_tile_pool(_ptr(x), x.stride(0), _ptr(x_scale), 1 if fp8 else 0, _ptr(out), B, H, L,
+                                                    Lp if fp8 else 0, _stream()), "scail_attention_tile_pool")
+    _count()
+    return out
+
+
+def select_scratch_len(B, H, L):
+    """int32 entries of the scratch select_tiles needs: B H n (1 + ceil(n / 32)), n = ceil(L / 128)."""
+    n = -(-int(L) // ATT_TILE)
+    return B * H * n * (1 + -(-n // 32))
+
+
+def select_tiles(qbar, kbar, B, H, L, n_ref, mass, max_tiles, ptr, idx, scratch):
+    """Per-(batch, head) tile maps chosen on the device from the tile means qbar, kbar (fp32 [B, H, n, 128], tile_pool):
+    query tile q lists its diagonal tile, every key tile holding one of the n_ref reference tokens, then the key tiles of
+    largest estimated softmax mass e_k = n_k exp(s_k - max s), s_k = qbar_q . kbar_k / sqrt(128) (ties: lower index), until
+    the listed mass reaches `mass` of the total or max_tiles (None: no cap) were taken that way.  Writes ptr, idx (int32
+    [B, H, n + 1] and [B, H, n * n] or wider); scratch int32 [>= select_scratch_len(B, H, L)].  No host synchronisation."""
+    n = -(-int(L) // ATT_TILE)
+    for t in (qbar, kbar):
+        _req(t, torch.float32)
+        assert t.is_contiguous() and t.shape == (B, H, n, 128)
+    ps, ids = _bh_maps(ptr, idx, B, H, L, qbar.device)
+    _req(scratch, torch.int32)
+    assert scratch.is_contiguous()
+    _lib.check(_lib.lib().scail_attention_select_tiles(_ptr(qbar), _ptr(kbar), B, H, L, n_ref, float(mass),
+                                                       -1 if max_tiles is None else int(max_tiles), _ptr(ptr), ps, _ptr(idx),
+                                                       ids, _ptr(scratch), scratch.numel(), _stream()),
+               "scail_attention_select_tiles")
+    _count(2)
+    return ptr, idx
+
+
 def attention_partial(q, k, v, o32, state, B, H, q_len, ranges, q_batch_rows=None, kv_batch_rows=None, scale=None):
     """Attention of q over the key rows `ranges` = [(off0, len0)] or [(off0, len0), (off1, len1)] of every batch (offsets inside a
     batch of kv_batch_rows rows).  o32: fp32 [rows, H*128] (normalised partial result), state: fp32 [rows, H, 2] = (max, sum)."""

@@ -149,8 +149,10 @@ class GraphedStep:
     instead of ~780, and none of the reference's per-layer host syncs (sat/transformer_defaults.py:56-57) by construction.
     The latent `x`, the timestep vector and the conditioning tensors are static buffers owned by this object; results are
     bit-identical to `sampler_step` (same kernels, same order).  Single-GPU path (NCCL collectives are not captured).
-    The graph runs in the `fp8_linear`, `fp8_attention` and `attention_window` modes of construction time; a window's tile map
-    is held by scail_b200.sparse for the life of the process, so the graph reads it at a fixed address.  With fp8 it reads the e4m3 weight copies in place: every
+    The graph runs in the `fp8_linear`, `fp8_attention`, `attention_window` and `attention_adaptive` modes of construction
+    time; a window's tile map is held by scail_b200.sparse for the life of the process, so the graph reads it at a fixed
+    address.  attention_adaptive selects its maps on the device on every replay (tile pooling and selection are captured
+    kernels writing the per-stream workspace), so they follow the replayed step's Q and K.  With fp8 it reads the e4m3 weight copies in place: every
     call first re-derives, into the same buffers, the copies of weights that changed since (e.g. after load_state_dict).
     step_cache (a scail_b200.step_cache.FirstBlockCache): the step runs as three graphs with the host's skip decision between
     them (bit-identical to sampler_step with the same cache and thresholds).  The cache is reset at construction; when its

@@ -12,7 +12,14 @@ tokens.  Key tile k is listed for query tile q when
   (c) some frame of q and some frame of k differ by at most `window`, a tile's frames being the span from its lowest to
       its highest frame (see frame_window_tiles).
 A tile that straddles a segment or frame boundary therefore takes part with all its tokens.  window >= T - 1 lists every
-tile (the dense map)."""
+tile (the dense map).
+
+The module also holds the content-adaptive policy (AdaptiveTiles): per forward, per layer and per (batch, head), each query
+tile keeps the key tiles that carry a chosen share of the softmax mass estimated from tile-pooled Q and K, always with its
+diagonal tile and the tiles holding reference tokens.  Those maps are chosen on the device (ops.tile_pool,
+ops.select_tiles) and run through the per-(batch, head) sparse kernels."""
+import math
+import numbers
 import threading
 from collections import namedtuple
 
@@ -102,3 +109,63 @@ def tile_map(g, window, device):
             m.density = density
             _CACHE[key] = m
     return m
+
+
+# ---------------------------------------------------------------- content-adaptive tiles
+RECORD = None  # a list to collect (kv_tile_ptr, kv_tile_idx) copies of every map AdaptiveTiles.select builds (tests)
+
+
+class AdaptiveTiles:
+    """Content-adaptive block-sparse self-attention.  mass in [0, 1]: per query tile, the key tiles are listed by estimated
+    softmax mass e_k = n_k exp(s_k - max s), s_k = mean(Q over the query tile) . mean(K over key tile k) / sqrt(128), n_k the
+    valid keys of tile k, until the listed share of sum_k e_k reaches `mass` (1: every tile; 0: only the forced tiles, the
+    diagonal tile and those holding reference tokens).  max_tiles: None, or an int >= 0 capping the tiles taken by mass
+    (forced tiles do not count).  1 - mass estimates the attention mass dropped; it says nothing about visual quality."""
+
+    def __init__(self, mass, max_tiles=None):
+        if isinstance(mass, bool) or not isinstance(mass, numbers.Real) or math.isnan(float(mass)) or not 0.0 <= float(mass) <= 1.0:
+            raise ValueError(f"AdaptiveTiles: mass must be a float in [0, 1], got {mass!r}")
+        if max_tiles is not None and (isinstance(max_tiles, bool) or not isinstance(max_tiles, (int, np.integer)) or
+                                      max_tiles < 0):
+            raise ValueError(f"AdaptiveTiles: max_tiles must be None or an int >= 0, got {max_tiles!r}")
+        self.mass = float(mass)
+        self.max_tiles = None if max_tiles is None else int(max_tiles)
+
+    def __repr__(self):
+        return f"AdaptiveTiles(mass={self.mass!r}, max_tiles={self.max_tiles!r})"
+
+    def __eq__(self, other):
+        return isinstance(other, AdaptiveTiles) and (self.mass, self.max_tiles) == (other.mass, other.max_tiles)
+
+    def __hash__(self):
+        return hash((self.mass, self.max_tiles))
+
+    def select(self, q, k, B, H, L, n_ref, buf, q_scale=None, k_scale=None):
+        """Pool the self-attention operands q, k ([B*L, H*128] slabs: bf16, or e4m3 with their [B, H, L_pad] scales) and
+        choose this forward's maps on the device.  buf(name, shape, dtype) supplies the buffers (the model's per-stream
+        workspace, so a captured graph reads fixed addresses).  -> (kv_tile_ptr int32 [B, H, n + 1], kv_tile_idx int32
+        [B, H, n * n]) for ops.attention_sparse_bh / attention_fp8_sparse_bh."""
+        import torch
+        n = -(-int(L) // TILE)
+        f32, i32 = torch.float32, torch.int32
+        qbar = ops.tile_pool(q, B, H, L, buf("ada_qbar", (B, H, n, 128), f32), x_scale=q_scale)
+        kbar = ops.tile_pool(k, B, H, L, buf("ada_kbar", (B, H, n, 128), f32), x_scale=k_scale)
+        ptr, idx = buf("ada_ptr", (B, H, n + 1), i32), buf("ada_idx", (B, H, n * n), i32)
+        ops.select_tiles(qbar, kbar, B, H, L, n_ref, self.mass, self.max_tiles, ptr, idx,
+                         buf("ada_scratch", (ops.select_scratch_len(B, H, L),), i32))
+        if RECORD is not None:
+            RECORD.append((ptr.clone(), idx.clone()))
+        return ptr, idx
+
+
+def check_adaptive(adaptive):
+    """The attention_adaptive setting: None or an AdaptiveTiles."""
+    if adaptive is not None and not isinstance(adaptive, AdaptiveTiles):
+        raise ValueError(f"attention_adaptive must be None or a scail_b200.sparse.AdaptiveTiles, got {adaptive!r}")
+    return adaptive
+
+
+def bh_maps_host(ptr, idx):
+    """Per-(batch, head) device maps -> {(b, h): (kv_tile_ptr, kv_tile_idx)} numpy int32, each trimmed to its own nnz."""
+    p, i = ptr.cpu().numpy(), idx.cpu().numpy()
+    return {(b, h): (p[b, h].copy(), i[b, h, :p[b, h, -1]].copy()) for b in range(p.shape[0]) for h in range(p.shape[1])}

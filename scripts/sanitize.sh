@@ -34,3 +34,13 @@ timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$O
     > "$OUT/memcheck_fp8_attention_pytest.log" 2>&1
 echo "sanitizer exit code $?" >> "$OUT/memcheck_fp8_attention_pytest.log"
 tail -3 "$OUT/memcheck_fp8_attention_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_fp8_attention.log" | head -5
+# adaptive tile selection at small shapes: tile pooling (bf16, e4m3 + scales, ragged last tile), device selection and
+# compaction, and the per-(batch, head) sparse attention kernels; memcheck, then racecheck for the shared-memory selection
+for tool in memcheck racecheck; do
+    timeout 900 compute-sanitizer --tool $tool --error-exitcode 99 --log-file "$OUT/${tool}_adaptive.log" \
+        python -m pytest tests/test_adaptive_attention_gpu.py -q -x --timeout 600 \
+        -k "tile_pool and not 27904 or selection and 1000 or per_head and 1000 or mass_one_is and not 27904 or planted or refuses" \
+        > "$OUT/${tool}_adaptive_pytest.log" 2>&1
+    echo "sanitizer exit code $?" >> "$OUT/${tool}_adaptive_pytest.log"
+    tail -3 "$OUT/${tool}_adaptive_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds|hazard" "$OUT/${tool}_adaptive.log" | head -5
+done
