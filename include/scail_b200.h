@@ -230,6 +230,18 @@ int scail_step_cache_update(const void* h, const void* h1c, float* R, int64_t B,
                             int64_t n_seq, scail_stream_t stream);
 int scail_step_cache_apply(void* h, const float* R, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq,
                            scail_stream_t stream);
+/* Taylor forecast of the skipped blocks' residual (FirstBlockCache(order >= 1)).  R_slots holds n_slots (1..3) fp32
+ * [B, n_seq, d] slots, slot s at R_slots + s * slot_stride floats (slot_stride >= B*n_seq*d, a multiple of 4).  The slot
+ * index and the coefficients are read from device memory when the kernel runs, so one captured graph serves every step.
+ * scail_step_cache_update_slot: R_slots[*slot] = f32(h[noise rows]) - f32(h1c); a *slot outside [0, n_slots) writes nothing.
+ * scail_step_cache_apply_forecast: in place on the noise rows of h, t = c0*R0, t = t + c1*R1, t = t + c2*R2 (slot order,
+ * each product and sum rounded separately), then h = bf16_rn(f32(h) + t).  A slot with coef[s] == 0 is neither read nor
+ * added; with every coefficient 0, h is left unchanged. */
+int scail_step_cache_update_slot(const void* h, const void* h1c, float* R_slots, int64_t slot_stride, int64_t n_slots,
+                                 const int* slot, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq,
+                                 scail_stream_t stream);
+int scail_step_cache_apply_forecast(void* h, const float* R_slots, int64_t slot_stride, int64_t n_slots, const float* coef,
+                                    int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq, scail_stream_t stream);
 
 /* ---- Wan2.1 VAE decode (sgm/models/wan_vae.py); activations channels-last bf16 [T, H, W, C] ---- */
 enum { SCAIL_CONV_EPI_BIAS = 0, SCAIL_CONV_EPI_BIAS_RES = 1, SCAIL_CONV_EPI_HEAD_CLAMP = 2 };

@@ -66,6 +66,8 @@ SIGNATURES = {
     "scail_step_cache_indicator": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_update": [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_apply": [c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
+    "scail_step_cache_update_slot": [c_p, c_p, c_p, c_i64, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
+    "scail_step_cache_apply_forecast": [c_p, c_p, c_i64, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_conv3d_cl": [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_i64, c_int, c_int, c_int, c_p, c_p, c_i64, c_p, c_i64,
                         c_i64, c_int, c_int, c_p, c_p, c_p],
     "scail_conv3d_strided_cl": [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_i64, c_int, c_int, c_int, c_p, c_p, c_i64, c_i64,

@@ -886,6 +886,51 @@ int scail_step_cache_apply(void* h, const float* R, int64_t B, int64_t N, int64_
     return 0;
 }
 
+// Slot checks shared by the two forecast entry points: 1 <= n_slots <= 3, and every slot is a whole, 16-byte aligned
+// [B, n_seq, d] fp32 tensor that does not overlap the next one.
+static int step_cache_slots(const char* what, int64_t slot_stride, int64_t n_slots, int64_t B, int64_t n_seq, int64_t d) {
+    SCAIL_REQUIRE(n_slots >= 1 && n_slots <= scail::SC_MAX_SLOTS, "%s: need 1 <= n_slots <= %d (got %lld)", what,
+                  scail::SC_MAX_SLOTS, (long long)n_slots);
+    SCAIL_REQUIRE(slot_stride >= B * n_seq * d, "%s: slot_stride = %lld floats must be >= B * n_seq * d = %lld", what,
+                  (long long)slot_stride, (long long)(B * n_seq * d));
+    SCAIL_REQUIRE(slot_stride % 4 == 0, "%s: slot_stride = %lld floats must be a multiple of 4 so that every slot is 16-byte "
+                  "aligned", what, (long long)slot_stride);
+    return 0;
+}
+
+int scail_step_cache_update_slot(const void* h, const void* h1c, float* R_slots, int64_t slot_stride, int64_t n_slots,
+                                 const int* slot, int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq,
+                                 scail_stream_t stream) {
+    SCAIL_REQUIRE(h && h1c && R_slots && slot, "step_cache_update_slot: null operand");
+    SCAIL_REQUIRE(aligned16(h) && aligned16(h1c) && aligned16(R_slots),
+                  "step_cache_update_slot: h, h1c and R_slots must be 16-byte aligned");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(slot) & 3) == 0, "step_cache_update_slot: slot must be 4-byte aligned");
+    if (int rc = step_cache_shape("step_cache_update_slot", B, N, d, n_ref, n_seq)) return rc;
+    if (int rc = step_cache_slots("step_cache_update_slot", slot_stride, n_slots, B, n_seq, d)) return rc;
+    const int64_t nvec = B * n_seq * (d / 8);
+    scail::step_cache_update_slot_kernel<<<blocks_for(nvec, scail::SC_THREADS), scail::SC_THREADS, 0,
+                                           static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const uint4*>(h), static_cast<const uint4*>(h1c), R_slots, slot_stride, (int)n_slots, slot, nvec,
+        (int)(d / 8), (int)N, (int)n_ref, (int)n_seq);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_step_cache_apply_forecast(void* h, const float* R_slots, int64_t slot_stride, int64_t n_slots, const float* coef,
+                                    int64_t B, int64_t N, int64_t d, int64_t n_ref, int64_t n_seq, scail_stream_t stream) {
+    SCAIL_REQUIRE(h && R_slots && coef, "step_cache_apply_forecast: null operand");
+    SCAIL_REQUIRE(aligned16(h) && aligned16(R_slots), "step_cache_apply_forecast: h and R_slots must be 16-byte aligned");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(coef) & 3) == 0, "step_cache_apply_forecast: coef must be 4-byte aligned");
+    if (int rc = step_cache_shape("step_cache_apply_forecast", B, N, d, n_ref, n_seq)) return rc;
+    if (int rc = step_cache_slots("step_cache_apply_forecast", slot_stride, n_slots, B, n_seq, d)) return rc;
+    const int64_t nvec = B * n_seq * (d / 8);
+    scail::step_cache_apply_forecast_kernel<<<blocks_for(nvec, scail::SC_THREADS), scail::SC_THREADS, 0,
+                                              static_cast<cudaStream_t>(stream)>>>(
+        static_cast<uint4*>(h), R_slots, slot_stride, (int)n_slots, coef, nvec, (int)(d / 8), (int)N, (int)n_ref, (int)n_seq);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 int scail_conv3d_cl(const void* x, int64_t T, int64_t H, int64_t W, int64_t Cin, const void* w2, int64_t Cout, int KT,
                     int KH, int KW, const void* bias, const void* residual, int64_t ldr, void* out, int64_t ldo,
                     int64_t ocols, int fmul, int epilogue, const void* norm_gamma, void* out2, scail_stream_t stream) {

@@ -143,4 +143,66 @@ __global__ void __launch_bounds__(SC_THREADS) step_cache_apply_kernel(uint4* __r
     h[dst] = sc_pack(f);
 }
 
+// ---- Taylor forecast (FirstBlockCache(order >= 1)): n_slots fp32 residual slots [B, n_seq, d], slot s at R + s * slot_stride.
+// The slot index and the coefficients are read from device memory, so one captured graph serves every step.
+constexpr int SC_MAX_SLOTS = 3;
+
+// R[*slot] = f32(h[noise rows]) - f32(h1c) (step_cache_update's arithmetic); a slot outside [0, n_slots) writes nothing.
+__global__ void __launch_bounds__(SC_THREADS) step_cache_update_slot_kernel(const uint4* __restrict__ h,
+                                                                            const uint4* __restrict__ h1c, float* __restrict__ R,
+                                                                            int64_t slot_stride, int n_slots,
+                                                                            const int* __restrict__ slot, int64_t nvec, int vpr,
+                                                                            int N, int n_ref, int n_seq) {
+    const int s = *slot;
+    const int64_t v = static_cast<int64_t>(blockIdx.x) * SC_THREADS + threadIdx.x;
+    if (s < 0 || s >= n_slots || v >= nvec) return;
+    float4* Rs = reinterpret_cast<float4*>(R + s * slot_stride);
+    float fh[8], fc[8];
+    sc_unpack(h[sc_noise_to_full(v, vpr, n_seq, N, n_ref)], fh);
+    sc_unpack(h1c[v], fc);
+    Rs[2 * v] = make_float4(fh[0] - fc[0], fh[1] - fc[1], fh[2] - fc[2], fh[3] - fc[3]);
+    Rs[2 * v + 1] = make_float4(fh[4] - fc[4], fh[5] - fc[5], fh[6] - fc[6], fh[7] - fc[7]);
+}
+
+// In place on the noise rows: t = c0*R0, t = t + c1*R1, t = t + c2*R2 (slot order, every product and sum rounded on its
+// own: no FMA contraction), then h = bf16_rn(f32(h) + t).  A slot whose coefficient is exactly 0 is neither read nor
+// added, so stale or NaN slots cannot leak in and c = (1, 0, 0) is step_cache_apply bit for bit; with no active slot h
+// is left as it is.
+__global__ void __launch_bounds__(SC_THREADS) step_cache_apply_forecast_kernel(uint4* __restrict__ h, const float* __restrict__ R,
+                                                                               int64_t slot_stride, int n_slots,
+                                                                               const float* __restrict__ coef, int64_t nvec,
+                                                                               int vpr, int N, int n_ref, int n_seq) {
+    const int64_t v = static_cast<int64_t>(blockIdx.x) * SC_THREADS + threadIdx.x;
+    if (v >= nvec) return;
+    float c[SC_MAX_SLOTS];
+    bool any = false;
+#pragma unroll
+    for (int s = 0; s < SC_MAX_SLOTS; ++s) {
+        c[s] = s < n_slots ? coef[s] : 0.f;
+        any = any || c[s] != 0.f;
+    }
+    if (!any) return;
+    float t[8];
+    bool first = true;
+#pragma unroll
+    for (int s = 0; s < SC_MAX_SLOTS; ++s) {
+        if (c[s] == 0.f) continue;
+        const float4* Rs = reinterpret_cast<const float4*>(R + s * slot_stride);
+        const float4 r0 = Rs[2 * v], r1 = Rs[2 * v + 1];
+        const float r[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const float p = __fmul_rn(c[s], r[i]);
+            t[i] = first ? p : __fadd_rn(t[i], p);
+        }
+        first = false;
+    }
+    const int64_t dst = sc_noise_to_full(v, vpr, n_seq, N, n_ref);
+    float f[8];
+    sc_unpack(h[dst], f);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) f[i] = __fadd_rn(f[i], t[i]);
+    h[dst] = sc_pack(f);
+}
+
 }  // namespace scail

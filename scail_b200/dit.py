@@ -733,9 +733,11 @@ class DiffusionTransformer(nn.Module):
         is set)."""
         sc = kwargs.pop("_step_cache", None)
         if sc is not None:
+            sc.begin()  # the sampler's sigma of this step (required at order >= 1)
             head = self.step_cache_head(sc, x, timesteps, context, y, **kwargs)
             head.buffers.indicator(head.h0)
             skip = sc.decide(head.buffers.read_indicator())
+            sc.stage(skip)
             out = self.step_cache_tail(head, skip)
             if not skip:
                 sc.computed()
@@ -842,15 +844,23 @@ class DiffusionTransformer(nn.Module):
 
     def step_cache_tail(self, head, skip):
         """skip: the noise rows of h1 become bf16(f32(h1) + R).  Otherwise blocks 1..L-1 run on h1, then R = f32(h_L) - f32(h1)
-        on the noise rows.  Then the final layer.  Changes no host-side cache state (the caller commits a computed step)."""
+        on the noise rows.  Then the final layer.  Changes no host-side cache state (the caller commits a computed step).
+        At order >= 1 the forecast kernels take the place of R: the apply adds the coefficients' combination of the slots,
+        the update writes one slot; both read the slot and coefficients from the control block (FirstBlockCache.stage)."""
         bufs, kw = head.buffers, head.kw
         if skip:
-            ops.step_cache_apply(bufs.h1, bufs.R, bufs.n_ref)
+            if bufs.R_slots is None:
+                ops.step_cache_apply(bufs.h1, bufs.R, bufs.n_ref)
+            else:
+                ops.step_cache_apply_forecast(bufs.h1, bufs.R_slots, bufs.ctl_coef, bufs.n_ref)
         else:
             ad = self.mixins["adaln_layer"]
             for l in range(1, self.num_layers):
                 ad.layer_forward(bufs.h1, None, layer_id=l, **kw)
-            ops.step_cache_update(bufs.h1, bufs.h1c, bufs.R, bufs.n_ref)
+            if bufs.R_slots is None:
+                ops.step_cache_update(bufs.h1, bufs.h1c, bufs.R, bufs.n_ref)
+            else:
+                ops.step_cache_update_slot(bufs.h1, bufs.h1c, bufs.R_slots, bufs.ctl_slot, bufs.n_ref)
         return self.mixins["final_layer"].final_forward(bufs.h1, **kw)
 
 

@@ -606,6 +606,39 @@ def step_cache_apply(h, R, n_ref):
     return h
 
 
+def _slots(h, R_slots, n_ref):
+    """(B, N, d, n_seq, n_slots, slot_stride) of h bf16 [B, N, d] and its forecast slots R_slots fp32 [n_slots, B, n_seq, d]."""
+    _req(R_slots, torch.float32)
+    assert R_slots.dim() == 4 and R_slots.is_contiguous() and 1 <= R_slots.shape[0] <= 3, tuple(R_slots.shape)
+    B, N, d, n_seq = _noise_rows(h, R_slots[0], n_ref, torch.float32)
+    return B, N, d, n_seq, R_slots.shape[0], R_slots[0].numel()
+
+
+def step_cache_update_slot(h, h1c, R_slots, slot, n_ref):
+    """R_slots[slot] (fp32 [B, n_seq, d]) = f32(h[:, n_ref:n_ref + n_seq]) - f32(h1c), where slot is an int32 device tensor
+    (read by the kernel when it runs; a slot outside [0, n_slots) writes nothing); R_slots fp32 [n_slots, B, n_seq, d]."""
+    B, N, d, n_seq, n_slots, stride = _slots(h, R_slots, n_ref)
+    _req(h1c), _req(slot, torch.int32)
+    assert h1c.shape == (B, n_seq, d) and h1c.is_contiguous() and slot.numel() >= 1
+    _lib.check(_lib.lib().scail_step_cache_update_slot(_ptr(h), _ptr(h1c), _ptr(R_slots), stride, n_slots, _ptr(slot), B, N, d,
+                                                       n_ref, n_seq, _stream()), "scail_step_cache_update_slot")
+    _count()
+    return R_slots
+
+
+def step_cache_apply_forecast(h, R_slots, coef, n_ref):
+    """In place on h[:, n_ref:n_ref + n_seq]: t = c0*R0, t = t + c1*R1, t = t + c2*R2 (each product and sum rounded on its own;
+    slots with c == 0 are not read), h = bf16_rn(f32(h) + t).  coef: fp32 device tensor of n_slots coefficients, read by the
+    kernel when it runs; R_slots fp32 [n_slots, B, n_seq, d].  Returns h."""
+    B, N, d, n_seq, n_slots, stride = _slots(h, R_slots, n_ref)
+    _req(coef, torch.float32)
+    assert coef.numel() >= n_slots and coef.is_contiguous()
+    _lib.check(_lib.lib().scail_step_cache_apply_forecast(_ptr(h), _ptr(R_slots), stride, n_slots, _ptr(coef), B, N, d, n_ref,
+                                                          n_seq, _stream()), "scail_step_cache_apply_forecast")
+    _count()
+    return h
+
+
 def cast_bf16(x):
     _req(x, torch.float32)
     out = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16)

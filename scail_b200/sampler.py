@@ -37,9 +37,11 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     image_clip_features, concat_images (shared by both CFG branches, guiders.py:50-56).
     plan: an optional scail_b200.parallel.HybridParallel — this rank then runs ONE CFG branch (b = 1) and the two
     velocities are exchanged between partner ranks before the combine.
-    step_cache: an optional scail_b200.step_cache.FirstBlockCache, passed to the forward (single GPU only)."""
+    step_cache: an optional scail_b200.step_cache.FirstBlockCache, passed to the forward with this step's sigma (single GPU
+    only)."""
     if step_cache is not None:
         check_supported(plan=plan)
+        step_cache.set_sigma(sigma if _sigma_override is None else _sigma_override)
         model_kwargs["_step_cache"] = step_cache
     ctx = _ctx if _ctx is not None else prepare_context(cond, uc)
     kw = dict(y=None, ref_concat=cond["ref_concat"], concat_smpl_render=cond["concat_smpl_render"],
@@ -157,7 +159,8 @@ class GraphedStep:
     step_cache (a scail_b200.step_cache.FirstBlockCache): the step runs as three graphs with the host's skip decision between
     them (bit-identical to sampler_step with the same cache and thresholds).  The cache is reset at construction; when its
     buffers are dropped or replaced later (reset(), another geometry) the graphs are captured again, and the next step
-    computes."""
+    computes.  At order >= 1, graphs (2) and (3) hold the forecast kernels, which read the slot and coefficients from the
+    cache's control block: the host writes it between graph (1) and the tail, so the same graphs serve every step."""
 
     def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None):
         if step_cache is not None:
@@ -239,12 +242,15 @@ class GraphedStep:
             self.graph.replay()
             return ops.cfg_euler_(self.x, self.v, self.scale, float(next_sigma) - float(sigma))
         sc = self.step_cache
+        sc.set_sigma(sigma)
+        sc.begin()
         if sc.buffers is not self.head.buffers:  # reset() or another geometry since the capture dropped the captured buffers
             self._capture_cached()
         self.graphs[0].replay()
         bufs = self.head.buffers
         bufs.indicator(self.head.h0)
         skip = sc.decide(bufs.read_indicator())
+        sc.stage(skip)
         self.graphs[2 if skip else 1].replay()
         if not skip:
             sc.computed()
