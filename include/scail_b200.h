@@ -212,6 +212,17 @@ int scail_unpatchify(const void* lin, void* out, int64_t B, int64_t T, int64_t H
 /* x (fp32, n elements) += dsigma * (v_u + scale*(v_c - v_u)), v bf16 [2, n]
  * (guiders.py:41-45, sampling_utils.py:7-10, sampling.py:960-963) */
 int scail_cfg_euler(float* x, const void* v, int64_t n, float scale, float dsigma, scail_stream_t stream);
+/* One UniPC solver step (scail_b200/unipc.py), in place, one pass over n fp32 elements (n % 4 == 0).  v is the bf16 CFG
+ * pair [2, n] as scail_cfg_euler reads it; slots holds n_slots (1..3) fp32 model outputs of n elements, slot s at
+ * slots + s * slot_stride floats (slot_stride >= n, a multiple of 4); x, x_last, v and slots are 16-byte aligned.
+ * coef is a host array of 10 floats {a_x, a_0, a_1, a_2, a_m, b_y, b_0, b_1, b_2, b_m}, passed to the kernel by value;
+ * the coefficients of slots >= n_slots must be 0.  Per element, each product and sum rounded separately (no FMA):
+ * g = u + scale*(c - u); m = x - sigma*g; y = a_x*x_last + a_s*M_s (slot order) + a_m*m if correct, else y = x;
+ * z = b_y*y + b_s*M_s (slot order) + b_m*m; then x = z, x_last = y, slot write_slot = m.  A slot whose coefficients are 0
+ * is neither read nor added; all reads precede the writes, so write_slot may be a slot the step reads. */
+int scail_unipc_step(float* x, float* x_last, const void* v, float* slots, int64_t slot_stride, int64_t n_slots,
+                     int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                     scail_stream_t stream);
 int scail_cast_f32_bf16(const float* x, void* out, int64_t n, scail_stream_t stream);
 
 /* First-block residual cache (scail_b200/step_cache.py).  Token tensors are bf16 [B, N, d] (ref || noise || pose rows of

@@ -19,6 +19,7 @@
 #include "conv.cuh"
 #include "gemm.cuh"
 #include "rowops.cuh"
+#include "solver.cuh"
 #include "step_cache.cuh"
 
 namespace {
@@ -815,6 +816,39 @@ int scail_cfg_euler(float* x, const void* v, int64_t n, float scale, float dsigm
     SCAIL_REQUIRE(x && v, "cfg_euler: null operand");
     scail::cfg_euler_kernel<<<blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         x, static_cast<const __nv_bfloat16*>(v), n, scale, dsigma);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_unipc_step(float* x, float* x_last, const void* v, float* slots, int64_t slot_stride, int64_t n_slots,
+                     int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                     scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && v && slots && coef, "unipc_step: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(v) && aligned16(slots),
+                  "unipc_step: x, x_last, v and slots must be 16-byte aligned");
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "unipc_step: need n a positive multiple of 4 (got n=%lld)", (long long)n);
+    SCAIL_REQUIRE(n_slots >= 1 && n_slots <= scail::UNIPC_MAX_SLOTS, "unipc_step: need 1 <= n_slots <= %d (got %lld)",
+                  scail::UNIPC_MAX_SLOTS, (long long)n_slots);
+    SCAIL_REQUIRE(write_slot >= 0 && write_slot < n_slots, "unipc_step: write_slot = %lld must be in [0, n_slots = %lld)",
+                  (long long)write_slot, (long long)n_slots);
+    SCAIL_REQUIRE(slot_stride >= n && slot_stride % 4 == 0, "unipc_step: slot_stride = %lld floats must be >= n = %lld and a "
+                  "multiple of 4 so that every slot is whole and 16-byte aligned", (long long)slot_stride, (long long)n);
+    scail::UnipcCoef k;
+    k.a_x = coef[0];
+    k.a_m = coef[4];
+    k.b_y = coef[5];
+    k.b_m = coef[9];
+    for (int s = 0; s < scail::UNIPC_MAX_SLOTS; ++s) {
+        k.a[s] = coef[1 + s];
+        k.b[s] = coef[6 + s];
+        SCAIL_REQUIRE(s < n_slots || (k.a[s] == 0.f && k.b[s] == 0.f),
+                      "unipc_step: the coefficients of slot %d must be 0 with n_slots = %lld", s, (long long)n_slots);
+    }
+    const int64_t nvec = n / 4;
+    scail::unipc_step_kernel<<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
+                               static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(v), slots, slot_stride,
+        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

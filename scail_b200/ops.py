@@ -1,5 +1,6 @@
 """Thin torch-tensor wrappers over the C ABI (one function per entry point).  All tensors must be
 CUDA tensors; there is no CPU path.  Launches go to torch.cuda.current_stream()."""
+import ctypes
 import math
 
 import torch
@@ -551,6 +552,25 @@ def cfg_euler_(x, v, scale, dsigma):
     _req(x, torch.float32), _req(v)
     assert x.is_contiguous() and v.is_contiguous() and v.numel() == 2 * x.numel()
     _lib.check(_lib.lib().scail_cfg_euler(_ptr(x), _ptr(v), x.numel(), float(scale), float(dsigma), _stream()), "scail_cfg_euler")
+    _count()
+    return x
+
+
+def unipc_step_(x, x_last, v, slots, write_slot, scale, sigma, coef, correct):
+    """One fused UniPC step (scail_b200.unipc), in place: g = v[0] + scale*(v[1] - v[0]); m = x - sigma*g; y = a_x*x_last +
+    a_k*slots[k] (slot order) + a_m*m if `correct`, else y = x; x = b_y*y + b_k*slots[k] + b_m*m; x_last = y;
+    slots[write_slot] = m.  Each product and sum rounded on its own; slots with zero coefficients are not read.
+    x, x_last fp32 (same shape, contiguous), v bf16 [2, ...], slots fp32 [n_slots, x.numel()]; coef: 10 floats
+    (a_x, a_0, a_1, a_2, a_m, b_y, b_0, b_1, b_2, b_m), passed by value.  Returns x."""
+    _req(x, torch.float32), _req(x_last, torch.float32), _req(v), _req(slots, torch.float32)
+    assert x.is_contiguous() and x_last.is_contiguous() and x_last.shape == x.shape
+    assert v.is_contiguous() and v.numel() == 2 * x.numel()
+    assert slots.dim() == 2 and slots.is_contiguous() and slots.shape[1] == x.numel(), tuple(slots.shape)
+    assert len(coef) == 10
+    c = (ctypes.c_float * 10)(*coef)
+    _lib.check(_lib.lib().scail_unipc_step(_ptr(x), _ptr(x_last), _ptr(v), _ptr(slots), slots.stride(0), slots.shape[0],
+                                           int(write_slot), x.numel(), float(scale), float(sigma), int(bool(correct)),
+                                           ctypes.addressof(c), _stream()), "scail_unipc_step")
     _count()
     return x
 

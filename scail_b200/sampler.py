@@ -31,14 +31,18 @@ def prepare_context(cond, uc):
 
 
 def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, plan=None, _x_override=None, _sigma_override=None,
-                 step_cache=None, **model_kwargs):
+                 step_cache=None, solver=None, **model_kwargs):
     """One reference sampler step: x [1,t,16,h,w] fp32 (updated in place and returned).
     cond/uc: dicts with 'crossattn' [1,L,text_dim]; cond also carries ref_concat, concat_smpl_render,
     image_clip_features, concat_images (shared by both CFG branches, guiders.py:50-56).
     plan: an optional scail_b200.parallel.HybridParallel — this rank then runs ONE CFG branch (b = 1) and the two
     velocities are exchanged between partner ranks before the combine.
     step_cache: an optional scail_b200.step_cache.FirstBlockCache, passed to the forward with this step's sigma (single GPU
-    only)."""
+    only).
+    solver: an optional scail_b200.unipc.UniPC with a bound schedule; its step replaces the Euler update.  (sigma, next_sigma)
+    must be the solver's next pair and x its latent, else ValueError before anything runs."""
+    if solver is not None:
+        solver.check_step(x, sigma, next_sigma)
     if step_cache is not None:
         check_supported(plan=plan)
         step_cache.set_sigma(sigma if _sigma_override is None else _sigma_override)
@@ -56,17 +60,22 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
         b = plan.branch
         ts = torch.full((1,), c_noise, device=x.device, dtype=torch.float32)
         v = plan.gather_branches(model(x_in, timesteps=ts, context=ctx[b:b + 1], **kw))
+    if solver is not None:
+        return solver.step(x, v.contiguous(), scale, sigma, next_sigma)
     return ops.cfg_euler_(x, v.contiguous(), scale, float(next_sigma) - float(sigma))
 
 
-def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None, step_cache=None):
+def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None, step_cache=None, solver=None):
     """RFSampler.__call__ (sampling.py:965-982): the full Euler loop.  With `adaln_layer.cache_cross_kv` the step-invariant
     conditioning (text / CLIP embeddings and all layers' cross-attention K,V) is computed once for this call.  step_cache (a
-    scail_b200.step_cache.FirstBlockCache) is reset here and then decides on every step whether blocks 1..L-1 run."""
+    scail_b200.step_cache.FirstBlockCache) is reset here and then decides on every step whether blocks 1..L-1 run.
+    solver (a scail_b200.unipc.UniPC) is bound to this call's schedule here and replaces the Euler update on every step."""
     if step_cache is not None:
         check_supported(plan=plan)
         step_cache.reset()
     sig = make_flow_timesteps(num_steps, shift_scale)
+    if solver is not None:
+        solver.begin(sig)
     ctx = prepare_context(cond, uc)
     cache = getattr(model.mixins["adaln_layer"], "cache_cross_kv", False) if hasattr(model, "mixins") else False
     cache = cache and plan is None  # (a CFG-parallel rank feeds its own row of ctx: a different tensor object)
@@ -74,7 +83,8 @@ def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=No
         model.set_conditioning(ctx, cond["image_clip_features"], batch=2)
     try:
         for i in range(num_steps):
-            x = sampler_step(model, x, sig[i], sig[i + 1], cond, uc, scale, _ctx=ctx, plan=plan, step_cache=step_cache)
+            x = sampler_step(model, x, sig[i], sig[i + 1], cond, uc, scale, _ctx=ctx, plan=plan, step_cache=step_cache,
+                             solver=solver)
     finally:
         if cache:
             model.clear_conditioning()
@@ -160,14 +170,17 @@ class GraphedStep:
     them (bit-identical to sampler_step with the same cache and thresholds).  The cache is reset at construction; when its
     buffers are dropped or replaced later (reset(), another geometry) the graphs are captured again, and the next step
     computes.  At order >= 1, graphs (2) and (3) hold the forecast kernels, which read the slot and coefficients from the
-    cache's control block: the host writes it between graph (1) and the tail, so the same graphs serve every step."""
+    cache's control block: the host writes it between graph (1) and the tail, so the same graphs serve every step.
+    solver (a scail_b200.unipc.UniPC, with a schedule bound by solver.begin): its step runs eagerly after the replay, in
+    place of CFG+Euler, with its coefficients passed by value, so no graph depends on it; the step is validated before
+    anything runs."""
 
-    def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None):
+    def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None, solver=None):
         if step_cache is not None:
             check_supported(getattr(model.mixins["adaln_layer"], "cp", None))
         if getattr(model.mixins["adaln_layer"], "cp", None) is not None:
             raise NotImplementedError("GraphedStep captures the single-GPU forward; use sampler_step under context parallelism")
-        self.model, self.scale = model, scale
+        self.model, self.scale, self.solver = model, scale, solver
         self.x = x  # fp32 [1,t,16,h,w], updated in place every step
         dev = x.device
         self.ts = torch.zeros(2, device=dev, dtype=torch.float32)
@@ -234,13 +247,20 @@ class GraphedStep:
         self.graphs = graphs
         self.kernels_in_graph = ops.LAUNCHES - n0
 
+    def _update(self, v, sigma, next_sigma):
+        if self.solver is not None:
+            return self.solver.step(self.x, v, self.scale, sigma, next_sigma)
+        return ops.cfg_euler_(self.x, v, self.scale, float(next_sigma) - float(sigma))
+
     def __call__(self, sigma, next_sigma):
+        if self.solver is not None:
+            self.solver.check_step(self.x, sigma, next_sigma)
         if self.fp8:
             self.adaln.prepare_fp8_weights()
         self.ts.fill_(float(sigma) * 1000.0)
         if self.step_cache is None:
             self.graph.replay()
-            return ops.cfg_euler_(self.x, self.v, self.scale, float(next_sigma) - float(sigma))
+            return self._update(self.v, sigma, next_sigma)
         sc = self.step_cache
         sc.set_sigma(sigma)
         sc.begin()
@@ -254,7 +274,7 @@ class GraphedStep:
         self.graphs[2 if skip else 1].replay()
         if not skip:
             sc.computed()
-        return ops.cfg_euler_(self.x, self.v_skip if skip else self.v_run, self.scale, float(next_sigma) - float(sigma))
+        return self._update(self.v_skip if skip else self.v_run, sigma, next_sigma)
 
 
 class HostStep:
