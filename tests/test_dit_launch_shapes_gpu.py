@@ -5,16 +5,28 @@ random weights) runs sampler.sampler_step on latents 21x64x64 (N = 27 904), 21x6
 last tile, n_ref = 1560) and 21x64x112 (N = 48 832, 64 keys in the last tile) with the CFG batch of two 512-token text
 contexts, in bf16, with fp8 linears + fp8 attention, and with the window-2 block-sparse attention (bf16 and fp8); the
 per-rank b = 1 forward of the 2-GPU CFG split at 21x64x112; and two steps of FirstBlockCache(inf) at the two ragged
-geometries (the first computes, the second skips).  Every DiT entry point of scail_b200.ops is wrapped by
-kernel_check.recording; each distinct launch (shapes, row strides and slab offsets of every operand, batch-row counts,
-epilogue, RoPE geometry, tile map, ...) is re-run on fresh seeded data with the recorded views inside wider buffers whose
-other elements are sentinels (checked bit for bit after the launch), against an fp32 reference on the GPU (TF32 off).
+geometries (the first computes, the second skips).  Also at every geometry the content-adaptive attention
+AdaptiveTiles(0.9, max_tiles=40), in bf16 and with fp8 linears + fp8 attention; at the two ragged geometries
+FirstBlockCache(order=1) and (order=2) over four steps with thresholds 0, 0, 0, inf (three computed steps fill the
+forecast slots, the fourth skips and forecasts from 2 or 3 of them); and at 21x64x112 sampler.sample with UniPC(3) over
+make_flow_timesteps(4) (predictor orders 1, 2, 2, 1, the corrector from the second step on).  Every DiT entry point of
+scail_b200.ops is wrapped by kernel_check.recording; each distinct launch (shapes, row strides and slab offsets of every
+operand, batch-row counts, epilogue, RoPE geometry, tile map, map strides, slot counts, ...) is re-run on fresh seeded data
+with the recorded views inside wider buffers whose other elements are sentinels (checked bit for bit after the launch),
+against an fp32 reference on the GPU (TF32 off), or a float64 / bit-exact restatement where the kernel promises one: tile
+pooling against the float64 tile mean, tile selection against its float64 restatement (tests/adaptive_oracle.py) on the
+kernel's own pooled tiles, the forecast kernels against tests/forecast_oracle.py at every slot index and every coefficient
+pattern the cache can pass (dead slots full of NaN), and the UniPC step against test_unipc_gpu.step_ref at the recorded
+coefficients (unread slots full of NaN).
 
 Attention data can fail: q, k give scaled logits with std ~3, and planted keys dominate chosen rows of batch 0 (key 0, the
 last valid key, keys on both sides of a 128-key tile edge, and for sparse maps a key in an unlisted tile, which must have no
 effect, and one in a listed tile).  Where batch 0's last key tile overhangs into batch 1 (kv_len % 128 != 0), batch 0's last
 query row gets a winning key among batch 1's first rows: the TMA box of that tile reads it and only the mask keeps it out.
-A leaked mask or a skipped tile moves such a row by the scale of V, not by a rounding.
+A leaked mask or a skipped tile moves such a row by the scale of V, not by a rounding.  The per-(batch, head) kernels run
+under maps from a real select_tiles run that differ across heads and batch elements; in both batch elements, at heads 0,
+H/2 and H - 1, a row gets a key in a tile its own map omits but the next head's map lists (no effect), and one in a tile
+its map lists.
 
 test_full_width_block_at_480x832_cfg_batch_vs_oracle: one full-width block plus the embeddings and the final layer at
 21x60x104, b = 2 (two different text contexts), against oracle/dit_oracle.py in fp32 on the GPU, next to the
@@ -22,16 +34,23 @@ reference-style bf16 library chain."""
 import math
 import time
 
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from adaptive_oracle import select_reference
+from forecast_oracle import apply_forecast_ref
 from kernel_check import assert_close_bf16, measure, recording
 from step_cache_oracle import apply_ref, indicator_sums, update_ref
+from test_adaptive_attention_gpu import bh_dense, masked_chain_fp8_bh, pool_ref, upload_maps
 from test_fp8_attention_gpu import qk_ref, vt_ref
 from test_fp8_gpu import deq, quant_ref
 from test_scale_gpu import sdpa_fp32_chunked
+from test_sparse_attention_gpu import heads
+from test_step_cache_forecast_gpu import sentinel_slots, slot_tensor
 from test_step_cache_gpu import operands as step_cache_operands, scratch as step_cache_scratch
+from test_unipc_gpu import sentinel as unipc_sentinel, step_ref
 
 pytestmark = pytest.mark.gpu
 FP8 = torch.float8_e4m3fn
@@ -39,12 +58,17 @@ BF = torch.bfloat16
 
 OPS = ("gemm", "gemm_fp8", "quant_rows_fp8", "quant_vt_fp8", "ln_modulate", "rmsnorm_rope", "attention", "attention_sparse",
        "attention_fp8", "adaln_modulation", "silu", "timestep_embedding", "patchify", "unpatchify", "cfg_euler_", "cast_bf16",
-       "step_cache_indicator", "step_cache_update", "step_cache_apply")
+       "step_cache_indicator", "step_cache_update", "step_cache_apply", "tile_pool", "select_tiles", "attention_sparse_bh",
+       "attention_fp8_sparse_bh", "step_cache_update_slot", "step_cache_apply_forecast", "unipc_step_")
 GEOMETRIES = {"512x512": (21, 64, 64), "480x832": (21, 60, 104), "512x896": (21, 64, 112)}
+ADAPTIVE = (0.9, 40)  # AdaptiveTiles(mass, max_tiles) of the adaptive modes
 MODES = {"bf16": dict(), "fp8": dict(fp8_linear=True, fp8_attention=True), "window 2": dict(attention_window=2),
-         "window 2, fp8 attention": dict(attention_window=2, fp8_attention=True)}
+         "window 2, fp8 attention": dict(attention_window=2, fp8_attention=True), "adaptive": dict(attention_adaptive=True),
+         "adaptive, fp8": dict(attention_adaptive=True, fp8_linear=True, fp8_attention=True)}
 CACHED = ("480x832", "512x896")
 B1 = "512x896"
+FORECAST_THRESHOLDS = (0.0, 0.0, 0.0, math.inf)  # three computed steps fill the slots, the fourth skips and forecasts
+N_REF = {(1 + t) * (h // 2) * (w // 2) + t * (h // 4) * (w // 4): (h // 2) * (w // 2) for t, h, w in GEOMETRIES.values()}
 
 GELU_TANH_ABS = 2.0 ** -11  # tanh.approx slack, as in test_gemm_tiles_gpu.py
 ATT_ELEM = dict(elem_rel=2.0 ** -7, elem_abs=2.0 ** -8)  # as test_sparse_attention_gpu.py: P enters PV as bf16, then the output
@@ -179,14 +203,43 @@ def _fields(name, a):
         return dict(shape=tuple(a["h1"].shape), n_ref=a["n_ref"], n_seq=a["h1c"].shape[1]), 1
     if name in ("step_cache_update", "step_cache_apply"):
         return dict(shape=tuple(a["h"].shape), n_ref=a["n_ref"], n_seq=a["R"].shape[1]), 1
+    if name == "tile_pool":
+        xs = a["x_scale"]
+        return dict(B=a["B"], H=a["H"], L=a["L"], x=_view(a["x"]), fp8=xs is not None,
+                    L_pad=None if xs is None else xs.shape[-1]), 1
+    if name == "select_tiles":
+        return dict(B=a["B"], H=a["H"], L=a["L"], n_ref=a["n_ref"], mass=float(a["mass"]), max_tiles=a["max_tiles"],
+                    ptr_stride=a["ptr"].shape[2], idx_stride=a["idx"].shape[2]), 1
+    if name == "attention_sparse_bh":
+        L = a["L"]
+        return dict(B=a["B"], H=a["H"], L=L, q_rows=L if a["q_batch_rows"] is None else a["q_batch_rows"],
+                    kv_rows=L if a["kv_batch_rows"] is None else a["kv_batch_rows"], q=_view(a["q"]), k=_view(a["k"]),
+                    v=_view(a["v"]), out=_view(a["out"]), q_total=a["q"].shape[0], kv_total=a["k"].shape[0],
+                    scale=float(a["scale"] or 1.0 / math.sqrt(128)), ptr_stride=a["ptr"].shape[2],
+                    idx_stride=a["idx"].shape[2]), 1
+    if name == "attention_fp8_sparse_bh":
+        return dict(B=a["B"], H=a["H"], L=a["L"], q=_view(a["q8"]), k=_view(a["k8"]), out=_view(a["out"]),
+                    L_pad=a["q_scale"].shape[-1], scale=float(a["scale"] or 1.0 / math.sqrt(128)),
+                    ptr_stride=a["ptr"].shape[2], idx_stride=a["idx"].shape[2]), 1
+    if name in ("step_cache_update_slot", "step_cache_apply_forecast"):
+        # the slot index and the coefficients live on the device: the check runs every value of them
+        R = a["R_slots"]
+        return dict(shape=tuple(a["h"].shape), n_ref=a["n_ref"], n_seq=R.shape[2], n_slots=R.shape[0],
+                    slot_stride=R[0].numel()), 1
+    if name == "unipc_step_":
+        coef = tuple(float(c) for c in a["coef"])
+        return dict(shape=tuple(a["x"].shape), n_slots=a["slots"].shape[0], slot_stride=a["slots"].stride(0),
+                    write_slot=int(a["write_slot"]), correct=bool(a["correct"]), active=tuple(c != 0.0 for c in coef),
+                    coef=coef, scale=float(a["scale"]), sigma=float(a["sigma"])), 1
     raise KeyError(name)
 
 
 @pytest.fixture(scope="module")
 def launches():
     """[(op, key)] of every distinct DiT launch of the cases in the module docstring, in first-call order."""
-    from scail_b200 import dit, ops, sampler
+    from scail_b200 import dit, ops, sampler, sparse
     from scail_b200.step_cache import FirstBlockCache
+    from scail_b200.unipc import UniPC
     m = full_width_model(2)
     ad = m.mixins["adaln_layer"]
     sig = sampler.make_flow_timesteps(50, 5.0)
@@ -196,19 +249,30 @@ def launches():
             for mode in MODES.values():
                 ad.fp8_linear, ad.fp8_attention = mode.get("fp8_linear", False), mode.get("fp8_attention", False)
                 ad.attention_window = mode.get("attention_window")
+                ad.attention_adaptive = sparse.AdaptiveTiles(*ADAPTIVE) if mode.get("attention_adaptive") else None
                 sampler.sampler_step(m, x0.clone(), sig[0], sig[1], cond, uc, 4.0)
             ad.fp8_linear = ad.fp8_attention = False
-            ad.attention_window = None
+            ad.attention_window = ad.attention_adaptive = None
             if geo in CACHED:  # the first step computes, the second skips: indicator, update and apply all launch
                 c, x = FirstBlockCache(math.inf), x0.clone()
                 sampler.sampler_step(m, x, sig[0], sig[1], cond, uc, 4.0, step_cache=c)
                 sampler.sampler_step(m, x, sig[1], sig[2], cond, uc, 4.0, step_cache=c)
                 assert [s for _, s in c.history] == [False, True]
                 del c
+                for order in (1, 2):  # computed steps write slots 0, 1, 0 (order 1) or 0, 1, 2; the skip reads 2 or 3
+                    c, x = FirstBlockCache(0.0, order=order), x0.clone()
+                    for j, threshold in enumerate(FORECAST_THRESHOLDS):
+                        c.threshold = threshold
+                        sampler.sampler_step(m, x, sig[j], sig[j + 1], cond, uc, 4.0, step_cache=c)
+                    assert [s for _, s in c.history] == [False, False, False, True]
+                    assert sum(cf != 0.0 for cf in c.buffers.ctl_coef.tolist()) == order + 1
+                    del c
             if geo == B1:  # one rank of the 2-GPU CFG split: the conditional branch alone
                 m(x0, timesteps=torch.full((1,), float(sig[0]) * 1000.0, device="cuda"), context=cond["crossattn"],
                   ref_concat=cond["ref_concat"], concat_smpl_render=cond["concat_smpl_render"],
                   image_clip_features=cond["image_clip_features"])
+                # UniPC(3) over make_flow_timesteps(4): predictor orders 1, 2, 2, 1; the corrector on from the second step
+                sampler.sample(m, x0.clone(), cond, uc, num_steps=4, solver=UniPC(3))
     torch.cuda.synchronize()
     del m, ad
     dit._WS.bufs.clear()
@@ -458,8 +522,9 @@ def _tile_matrix(key):
 
 def _attention_ref(q, k, v, B, H, q_len, kv_len, scale, tiles=None, chain=False):
     """fp32 softmax(scale q k^T) v per batch and head over [B * len, H * 128] operands, queries chunked; tiles: the key tiles
-    each 128-query tile may see.  chain: the restated fp8 chain of test_fp8_attention_gpu.chain_fp8 (dequantised per-token
-    Q, K and per-channel V, P^ = e4m3(2^8 p) against the row max over the allowed keys, l the sum of the unquantised 2^8 p)."""
+    each 128-query tile may see, bool [n_q_tiles, n_kv_tiles] for every (batch, head) or [B, H, n_q_tiles, n_kv_tiles] per
+    (batch, head).  chain: the restated fp8 chain of test_fp8_attention_gpu.chain_fp8 (dequantised per-token Q, K and
+    per-channel V, P^ = e4m3(2^8 p) against the row max over the allowed keys, l the sum of the unquantised 2^8 p)."""
     out = torch.empty(B * q_len, H * 128, device="cuda")
     chunk = min(4096, max(128, (2 ** 29 // (H * kv_len)) // 128 * 128))
     for b in range(B):
@@ -472,10 +537,10 @@ def _attention_ref(q, k, v, B, H, q_len, kv_len, scale, tiles=None, chain=False)
         kt = kh.transpose(1, 2)
         for i in range(0, q_len, chunk):
             s = (qh[:, i:i + chunk] @ kt) * scale
-            if tiles is not None:
+            if tiles is not None:  # s: [H, rows, kv_len]
                 qt = torch.arange(i, i + s.shape[1], device="cuda") // 128
-                allowed = tiles[qt].repeat_interleave(128, 1)[:, :kv_len]
-                s.masked_fill_(~allowed[None], float("-inf"))
+                allowed = (tiles[qt] if tiles.dim() == 2 else tiles[b][:, qt]).repeat_interleave(128, -1)[..., :kv_len]
+                s.masked_fill_(~(allowed if allowed.dim() == 3 else allowed[None]), float("-inf"))
             if chain:
                 p = torch.exp(s - s.amax(-1, keepdim=True)) * 256.0
                 o = (p.to(FP8).float() @ vh) / p.sum(-1, keepdim=True)
@@ -563,16 +628,22 @@ def check_attention_fp8(ops, f, g):
     torch.cuda.synchronize()
     for s in (Q, K, out):
         s.check("attention_fp8")
-    got = out.v
-    assert torch.isfinite(got.float()).all()
     want = _attention_ref(q, k, v, B, H, L, L, f["scale"], tiles)
     chain = _attention_ref(q, k, v, B, H, L, L, f["scale"], tiles, chain=True)
+    return _fp8_verdict(out.v, want, chain, B, H, L, planted, "attention_fp8")
+
+
+def _fp8_verdict(got, want, chain, B, H, L, planted, what):
+    """The e4m3 attention output got against the fp32 reference want, bounded by the restated fp8 chain's own error: overall
+    rel-L2, the worst (batch, 128-query tile, head) block, and every planted row (global row, head, whether its key is
+    visible)."""
+    assert torch.isfinite(got.float()).all()
     e, e_chain = rel(got, want), rel(chain, want)
-    assert e <= 1.25 * e_chain + 1e-3, f"attention_fp8: rel-L2 {e:.3e} > 1.25 x chain {e_chain:.3e} + 1e-3"
+    assert e <= 1.25 * e_chain + 1e-3, f"{what}: rel-L2 {e:.3e} > 1.25 x chain {e_chain:.3e} + 1e-3"
     blk, blk_chain = _block_rel(got, want, B, H, L), _block_rel(chain, want, B, H, L)
     worst, worst_chain = float(blk.max()), float(blk_chain.max())
     at = tuple(int(i) for i in torch.unravel_index(blk.argmax(), blk.shape))
-    assert worst <= 2 * worst_chain + 1e-3, (f"attention_fp8: worst (batch, 128-query tile, head) block {at} rel-L2 {worst:.3e} "
+    assert worst <= 2 * worst_chain + 1e-3, (f"{what}: worst (batch, 128-query tile, head) block {at} rel-L2 {worst:.3e} "
                                              f"> 2 x the chain's worst block {worst_chain:.3e} + 1e-3")
     for row, h, visible in planted:
         # a visible planted key takes the whole weight: P^ = 2^8 there in both, so the row matches the chain closely.  A
@@ -580,11 +651,277 @@ def check_attention_fp8(ops, f, g):
         # leaked in, it would take the whole weight and move the row by the scale of V (rel-L2 ~1).
         c = slice(h * 128, h * 128 + 128)
         e_row, bound = rel(got[row, c], chain[row, c]), 1e-2 if visible else 0.1
-        assert e_row < bound, (f"attention_fp8: planted row {row}, head {h} ({'visible' if visible else 'masked'} key): "
+        assert e_row < bound, (f"{what}: planted row {row}, head {h} ({'visible' if visible else 'masked'} key): "
                                f"rel-L2 vs the chain {e_row:.3e} >= {bound}")
     ratio = worst / (2 * worst_chain + 1e-3)
     return (f"rel-L2 {e:.2e} (chain {e_chain:.2e}); worst block {worst:.2e} at {at} vs chain's worst {worst_chain:.2e}: "
             f"block ratio {worst / worst_chain:.2f}, {len(planted)} planted rows"), ratio
+
+
+# ---------------------------------------------------------------- content-adaptive attention
+def _flat(data):
+    """A Slab of a contiguous tensor taken as rows of its last dimension: two sentinel rows before and after it, and a view
+    that is contiguous again.  -> (slab, the view in data's shape)."""
+    s = Slab(data.reshape(-1, data.shape[-1]), (data.shape[-1], 0, True))
+    return s, s.v.view(data.shape)
+
+
+def check_tile_pool(ops, f, g):
+    """Tile means against float64 within 1e-6 relative (as test_adaptive_attention_gpu), the ragged last tile included; in
+    e4m3 the codes times per-(token, head) scales that differ from token to token, with NaN past L (never read)."""
+    B, H, L = f["B"], f["H"], f["L"]
+    n = -(-L // 128)
+    x = _rand(g, B * L, H * 128, scale=2.0) + _rand(g, B * L, 1)  # rows with a mean of their own
+    slabs = []
+    if f["fp8"]:
+        codes, sc = qk_ref(x, B, H, L)
+        assert sc.shape[-1] == f["L_pad"]
+        sc[:, :, L:] = math.nan
+        X = Slab(codes, f["x"])
+        S, scale = _flat(sc)
+        slabs.append(S)
+        x64 = (codes.float().double().view(B, L, H, 128) * sc[:, :, :L].permute(0, 2, 1).double()[..., None]).view(B * L, H * 128)
+    else:
+        X, scale, x64 = Slab(x, f["x"]), None, x.double()
+    O, out = _flat(torch.zeros(B, H, n, 128, device="cuda"))
+    slabs += [X, O]
+    ops.tile_pool(X.v, B, H, L, out, x_scale=scale)
+    torch.cuda.synchronize()
+    for s in slabs:
+        s.check("tile_pool")
+    del x
+    want = pool_ref(x64, B, H, L)
+    del x64
+    ratio = float(((out.double() - want).abs() / (1e-6 * want.abs() + 1e-30)).max())
+    assert ratio <= 1, f"tile_pool: worst |d| / (1e-6 |float64 mean|) = {ratio:.3g}"
+    return f"worst |d| / (1e-6 |mean|) {ratio:.2f}; last tile {L - 128 * (n - 1)} rows", ratio
+
+
+def _structured(g, B, L, H, amp=3.0):
+    """test_adaptive_attention_gpu.structured() generated on the GPU: tiles that share a component of amplitude amp plus
+    token noise (at B = 2, L = 48 832 the host version holds ~2 GB)."""
+    d, n = H * 128, -(-L // 128)
+    base = (torch.randn(B, n, 1, d, device="cuda", generator=g) * amp).expand(B, n, 128, d).reshape(B, n * 128, d)[:, :L]
+    return (base + torch.randn(B, L, d, device="cuda", generator=g)).reshape(B * L, d).to(BF)
+
+
+def _select(ops, f, qbar, kbar):
+    """select_tiles at the recorded arguments into maps with sentinels around them -> (slabs, ptr, idx)."""
+    B, H, L = f["B"], f["H"], f["L"]
+    P, ptr = _flat(torch.zeros(B, H, f["ptr_stride"], device="cuda", dtype=torch.int32))
+    I, idx = _flat(torch.zeros(B, H, f["idx_stride"], device="cuda", dtype=torch.int32))
+    scratch = torch.empty(ops.select_scratch_len(B, H, L), device="cuda", dtype=torch.int32)
+    ops.select_tiles(qbar, kbar, B, H, L, f["n_ref"], f["mass"], f["max_tiles"], ptr, idx, scratch)
+    return [P, I], ptr, idx
+
+
+def check_select_tiles(ops, f, g):
+    """Maps chosen from the kernel's own pooled tiles of structured Q, K: every (b, h) map valid, the forced tiles (the
+    diagonal and every tile holding a reference token) listed, and the rows equal to the float64 restatement except rows
+    within rounding of their cutoff, which must stay <= 1e-3 of all rows (as test_adaptive_attention_gpu)."""
+    B, H, L, n_ref = f["B"], f["H"], f["L"], f["n_ref"]
+    n = -(-L // 128)
+    q = _structured(g, B, L, H)
+    Qb, qbar = _flat(ops.tile_pool(q, B, H, L))
+    del q
+    k = _structured(g, B, L, H)
+    Kb, kbar = _flat(ops.tile_pool(k, B, H, L))
+    del k
+    slabs, ptr, idx = _select(ops, f, qbar, kbar)
+    torch.cuda.synchronize()
+    for s in [Qb, Kb] + slabs:
+        s.check("select_tiles")
+    got = bh_dense(ptr, idx).numpy()  # checks every (b, h) map with ops.check_tile_map
+    n_ref_t = -(-n_ref // 128)
+    missing = np.argwhere(~got[..., :n_ref_t])
+    assert missing.size == 0, f"select_tiles: reference tiles not listed at (b, h, q tile, k tile) {missing[:5].tolist()}"
+    assert got[..., np.arange(n), np.arange(n)].all(), "select_tiles: a diagonal tile not listed"
+    want, near = select_reference(qbar.cpu().numpy(), kbar.cpu().numpy(), L, n_ref, f["mass"], f["max_tiles"], band=1e-5)
+    diff = (got != want).any(-1)
+    bad = np.argwhere(diff & ~near)
+    assert bad.size == 0, f"select_tiles: {len(bad)} rows differ from the float64 restatement, e.g. (b, h, q tile) {bad[:5].tolist()}"
+    assert near.mean() <= 1e-3, f"select_tiles: {near.mean():.2e} of the rows sit at their cutoff"
+    return (f"density {got.mean():.3f}, {n_ref_t} reference tiles forced, {int(diff.sum())} of {diff.size} rows differ "
+            f"(all within rounding of the cutoff, {int(near.sum())} rows there)"), 0.0
+
+
+def _adaptive_data(ops, g, f):
+    """q, k, v bf16 [B * L, H * 128] (logit std ~3), per-(b, h) maps tm (bool [B, H, n, n] on the host) from a real
+    select_tiles run on q, k at the adaptive mode's settings, and planted keys -> (q, k, v, tm, [(global query row, head,
+    whether the row may see its planted key)]).  In both batch elements, at heads 0, H/2 and H - 1, a query tile gets a key
+    in a tile its own map omits but the next head's map lists (no effect), and one in a listed tile (batch 0: the last
+    valid key, in the ragged last tile); where batch 0's last key tile overhangs into batch 1, batch 0's last query row gets
+    a winning key among batch 1's first rows (as _attention_data)."""
+    B, H, L = f["B"], f["H"], f["L"]
+    n = -(-L // 128)
+    s = LOGIT_STD ** 0.5
+    q, k, v = _rand(g, B * L, H * 128, scale=s), _rand(g, B * L, H * 128, scale=s), _rand(g, B * L, H * 128)
+    sel = dict(B=B, H=H, L=L, n_ref=N_REF[L], mass=ADAPTIVE[0], max_tiles=ADAPTIVE[1], ptr_stride=n + 1, idx_stride=n * n)
+    _, ptr, idx = _select(ops, sel, ops.tile_pool(q, B, H, L), ops.tile_pool(k, B, H, L))
+    tm = bh_dense(ptr, idx)
+    assert not torch.equal(tm[0, 0], tm[0, 1]) and not torch.equal(tm[0, 0], tm[1, 0]), "maps that do not differ"
+    plants = []
+    for b in range(B):
+        for j, h in enumerate((0, H // 2, H - 1)):
+            t = (n // 3 + 5 * j + 11 * b) % n
+            unlisted = [u for u in torch.nonzero(~tm[b, h, t]).flatten().tolist() if u != n - 1]
+            u = unlisted[len(unlisted) // 2]
+            w = n - 1 if b == 0 else unlisted[0]
+            assert u != w
+            tm[b, (h + 1) % H, t, u] = True  # another head's map lists the tile
+            tm[b, h, t, w] = True
+            plants += [(b, h, 128 * t + 5, 128 * u + 7, 1.0), (b, h, 128 * t + 6, L - 1 if w == n - 1 else 128 * w + 9, 0.5)]
+            if b == 0 and B > 1 and L % 128:  # batch 1's key 5 lies inside batch 0's last key tile (listed: the diagonal)
+                plants.append((0, h, L - 1, L + 5, 1.0))
+    rows = []
+    for b, h, row, key, alpha in plants:
+        c = slice(h * 128, h * 128 + 128)
+        q[b * L + row, c] = (alpha * k[b * L + key, c].float()).to(BF)
+        rows.append((b * L + row, h, key < L and bool(tm[b, h, row // 128, key // 128])))
+    return q, k, v, tm, rows
+
+
+def check_attention_sparse_bh(ops, f, g):
+    B, H, L = f["B"], f["H"], f["L"]
+    assert f["q_rows"] == L and f["kv_rows"] == L and f["q_total"] == B * L and f["kv_total"] == B * L
+    q, k, v, tm, planted = _adaptive_data(ops, g, f)
+    Q, K, V = Slab(q, f["q"]), Slab(k, f["k"]), Slab(v, f["v"])
+    out = Slab(torch.zeros(B * L, H * 128, device="cuda", dtype=BF), f["out"])
+    maps = [_flat(t) for t in upload_maps(tm)]
+    assert [m.shape[2] for _, m in maps] == [f["ptr_stride"], f["idx_stride"]]
+    ops.attention_sparse_bh(Q.v, K.v, V.v, out.v, B, H, L, maps[0][1], maps[1][1], scale=f["scale"])
+    torch.cuda.synchronize()
+    for s in [Q, K, V, out] + [s for s, _ in maps]:
+        s.check("attention_sparse_bh")
+    want = _attention_ref(q, k, v, B, H, L, L, f["scale"], tm.cuda())
+    c = assert_close_bf16(out.v, want, "attention_sparse_bh", **ATT_ELEM)
+    return _report(c) + f", density {tm.float().mean():.3f}, {len(planted)} planted rows", c.worst_ratio
+
+
+def check_attention_fp8_sparse_bh(ops, f, g):
+    B, H, L = f["B"], f["H"], f["L"]
+    assert f["scale"] == 1.0 / math.sqrt(128)  # masked_chain_fp8_bh's scale
+    q, k, v, tm, planted = _adaptive_data(ops, g, f)
+    (q8, qs), (k8, ks), (vt, vs) = qk_ref(q, B, H, L), qk_ref(k, B, H, L), vt_ref(v, B, H, L)
+    assert qs.shape[-1] == f["L_pad"]
+    Q, K = Slab(q8, f["q"]), Slab(k8, f["k"])
+    scales = [_flat(t) for t in (qs, ks, vt.view(FP8), vs)]
+    out = Slab(torch.zeros(B * L, H * 128, device="cuda", dtype=BF), f["out"])
+    maps = [_flat(t) for t in upload_maps(tm)]
+    assert [m.shape[2] for _, m in maps] == [f["ptr_stride"], f["idx_stride"]]
+    (_, qsv), (_, ksv), (_, vtv), (_, vsv) = scales
+    ops.attention_fp8_sparse_bh(Q.v, qsv, K.v, ksv, vtv, vsv, out.v, B, H, L, maps[0][1], maps[1][1], scale=f["scale"])
+    torch.cuda.synchronize()
+    for s in [Q, K, out] + [s for s, _ in scales + maps]:
+        s.check("attention_fp8_sparse_bh")
+    del q8, k8, vt, scales, Q, K
+    tmc = tm.cuda()
+    want = _attention_ref(q, k, v, B, H, L, L, f["scale"], tmc)
+    chain = masked_chain_fp8_bh(heads(q, B, L, H), heads(k, B, L, H), heads(v, B, L, H), tmc, chunk=128)
+    chain = chain.transpose(1, 2).reshape(B * L, H * 128)
+    return _fp8_verdict(out.v, want, chain, B, H, L, planted, "attention_fp8_sparse_bh")
+
+
+# ---------------------------------------------------------------- forecast cache and UniPC
+def check_step_cache_update_slot(ops, f, g):
+    """Every slot value -1 .. n_slots - 1 on the recorded [B, N, d] and slots: the named slot equals update_ref bit for bit;
+    the others, NaN-patterned sentinels, keep their bits (slot -1: all of them)."""
+    (B, N, d), n_ref, n_seq, n_slots = f["shape"], f["n_ref"], f["n_seq"], f["n_slots"]
+    assert f["slot_stride"] == B * n_seq * d
+    Hs, h = _flat(_rand(g, B, N, d, scale=4.0))
+    Cs, h1c = _flat(_rand(g, B, n_seq, d))
+    want = update_ref(h, h1c, n_ref)
+    before = sentinel_slots(n_slots, B, n_seq, d)
+    for s in range(-1, n_slots):
+        Rs, R = _flat(before)
+        ops.step_cache_update_slot(h, h1c, R, slot_tensor(s), n_ref)
+        torch.cuda.synchronize()
+        for slab in (Hs, Cs, Rs):
+            slab.check(f"step_cache_update_slot, slot {s}")
+        for k in range(n_slots):
+            if k == s:
+                _exact(R[k], want, f"step_cache_update_slot: slot {s}")
+            else:
+                _exact(R[k], before[k], f"step_cache_update_slot: slot {k} while writing slot {s}")
+        del Rs, R
+    return f"exact, slots -1 .. {n_slots - 1}, slot {n_slots - 1} ends {4 * n_slots * f['slot_stride'] / 2**30:.2f} GiB in", 0.0
+
+
+def _forecast_patterns(n_slots):
+    """(coefficients, the slot filled with NaN or None) for what the cache can pass: every slot active, one slot dead (its
+    coefficient 0, its contents NaN: it must not be read), none active (h unchanged), and one slot at exactly 1 (which is
+    step_cache_apply of that slot)."""
+    out = [({2: [2.0, -1.0], 3: [3.0, -3.0, 1.0]}[n_slots], None)]  # linear and quadratic extrapolation, evenly spaced
+    for dead in range(n_slots):
+        c = [0.5, -1.25, 1.75][:n_slots]
+        c[dead] = 0.0
+        out.append((c, dead))
+    out.append(([0.0] * n_slots, None))
+    out += [([1.0 if k == s else 0.0 for k in range(n_slots)], None) for s in range(n_slots)]
+    return out
+
+
+def check_step_cache_apply_forecast(ops, f, g):
+    """Bit for bit apply_forecast_ref for every coefficient pattern of _forecast_patterns (a coefficient past n_slots is NaN:
+    never read); (1 at slot s) also equals step_cache_apply of slot s; the ref and pose rows and the slots are untouched."""
+    (B, N, d), n_ref, n_seq, n_slots = f["shape"], f["n_ref"], f["n_seq"], f["n_slots"]
+    assert f["slot_stride"] == B * n_seq * d
+    h0 = _rand(g, B, N, d, scale=2.0)
+    slots = torch.randn(n_slots, B, n_seq, d, device="cuda", generator=g) * 0.5
+    Rs, R = _flat(slots)
+    outside = torch.ones(N, dtype=torch.bool, device="cuda")
+    outside[n_ref:n_ref + n_seq] = False
+    for coef, dead in _forecast_patterns(n_slots):
+        what = f"step_cache_apply_forecast, coefficients {coef}" + ("" if dead is None else f", slot {dead} NaN")
+        if dead is not None:
+            R[dead].fill_(math.nan)
+        Hs, h = _flat(h0)
+        c = torch.tensor(coef + [math.nan] * (3 - n_slots), device="cuda")
+        ops.step_cache_apply_forecast(h, R, c, n_ref)
+        torch.cuda.synchronize()
+        Hs.check(what), Rs.check(what)
+        want = apply_forecast_ref(h0, slots, coef, n_ref)
+        _exact(h, want, what)
+        _exact(h[:, outside], h0[:, outside], what + ": ref and pose rows")
+        if coef.count(1.0) == 1 and coef.count(0.0) == n_slots - 1:
+            s = coef.index(1.0)
+            plain = h0.clone()
+            ops.step_cache_apply(plain, slots[s].contiguous(), n_ref)
+            _exact(h, plain, what + ": step_cache_apply")
+        if dead is not None:
+            R[dead].copy_(slots[dead])
+        _exact(R, slots, what + ": the slots (only read)")
+        del Hs, h
+    return f"exact for {len(_forecast_patterns(n_slots))} coefficient patterns over {n_slots} slots", 0.0
+
+
+def check_unipc_step_(ops, f, g):
+    """Bit for bit step_ref at the recorded coefficients, scale and sigma: x, x_last and the written slot; every slot with
+    zero coefficients holds NaN-patterned sentinels (not read, and kept bit for bit unless written), and so does x_last
+    when the corrector is off."""
+    shape, n_slots, write, correct, coef = f["shape"], f["n_slots"], f["write_slot"], f["correct"], list(f["coef"])
+    n = math.prod(shape)
+    assert f["slot_stride"] == n
+    x0 = torch.randn(*shape, device="cuda", generator=g)
+    xl0 = torch.randn(*shape, device="cuda", generator=g) if correct else unipc_sentinel(1, n).view(shape).clone()
+    v = (torch.randn(2, *shape[1:], device="cuda", generator=g) * 2.0).to(BF)
+    before = unipc_sentinel(n_slots, n).clone()
+    live = [s for s in range(n_slots) if coef[1 + s] != 0.0 or coef[6 + s] != 0.0]
+    for s in live:
+        before[s] = torch.randn(n, device="cuda", generator=g)
+    z, y, m = step_ref(x0, xl0, v, before, f["scale"], f["sigma"], coef, correct)
+    (X, x), (XL, xl), (V, vv), (S, slots) = _flat(x0), _flat(xl0), _flat(v), _flat(before)
+    ops.unipc_step_(x, xl, vv, slots, write, f["scale"], f["sigma"], coef, correct)
+    torch.cuda.synchronize()
+    for s in (X, XL, V, S):
+        s.check("unipc_step_")
+    _exact(x.view(-1), z, "unipc_step_: x")
+    _exact(xl.view(-1), y, "unipc_step_: x_last")
+    _exact(slots[write], m, f"unipc_step_: slot {write}")
+    for s in range(n_slots):
+        if s != write:
+            _exact(slots[s], before[s], f"unipc_step_: slot {s} (not written)")
+    return f"exact; live slots {live}, write slot {write}, corrector {'on' if correct else 'off'}", 0.0
 
 
 # ---------------------------------------------------------------- small kernels
@@ -762,6 +1099,17 @@ def test_recorded_launches_cover_the_production_cases(launches):
             for op in ("step_cache_indicator", "step_cache_update", "step_cache_apply")),
         "patchify with Br = Bp = 1 < B = 2": has("patchify", B=2, Br=1, Bp=1),
         "patch-embed GEMM writing a row range of hidden": has("gemm", K=80, out=lambda v: v[0] == 5120 and v[2]),
+        "adaptive pooling (bf16 and fp8), selection and both per-(b, h) kernels at B = 2, H = 40, bf16 Q/K/V with ld 15360, "
+        "at every geometry": all(
+            has("tile_pool", B=2, H=40, L=N, fp8=False, x=ld(15360)) and has("tile_pool", B=2, H=40, L=N, fp8=True) and
+            has("select_tiles", B=2, H=40, L=N, n_ref=n_ref[geo], mass=ADAPTIVE[0], max_tiles=ADAPTIVE[1]) and
+            has("attention_sparse_bh", B=2, H=40, L=N, q=ld(15360), k=ld(15360), v=ld(15360)) and
+            has("attention_fp8_sparse_bh", B=2, H=40, L=N) for geo, N in Ns.items()),
+        "forecast update_slot and apply_forecast with 2 and 3 slots at ragged N": all(
+            has(op, shape=lambda s, N=Ns[geo]: s[:2] == (2, N), n_slots=k) for geo in CACHED for k in (2, 3)
+            for op in ("step_cache_update_slot", "step_cache_apply_forecast")),
+        "UniPC(3) steps with and without the corrector on the 512x896 latent": all(
+            has("unipc_step_", shape=(1, 21, 16, 64, 112), n_slots=3, correct=c) for c in (False, True)),
     }
     print("\n" + "\n".join(f"{'ok' if ok else 'MISSING'}: {what}" for what, ok in cases.items()))
     assert all(cases.values()), [what for what, ok in cases.items() if not ok]
