@@ -224,6 +224,24 @@ int scail_unipc_step(float* x, float* x_last, const void* v, float* slots, int64
                      int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
                      scail_stream_t stream);
 int scail_cast_f32_bf16(const float* x, void* out, int64_t n, scail_stream_t stream);
+/* CFG cache (scail_b200/cfg_cache.py).  n fp32 elements (n % 4 == 0); every pointer below is 16-byte aligned except
+ * partials (4) and out (8).
+ * scail_cfg_cache_delta: from the bf16 CFG pair v [2, n] (as scail_cfg_euler reads it), d_new = f32(c) - f32(u) (one
+ * subtraction, rounded once) and out = {sum |d_new - d_ref|, sum |d_ref|, ratio, 0} (fp64; ratio = +inf when the
+ * denominator is 0).  fp32 partial sums per CTA over a fixed partition of the elements (partials: at least 2 * 1024
+ * floats), then one CTA adds them in fp64 in a fixed order: bit-reproducible, no floating-point atomics.  Two launches.
+ * scail_cfg_euler_cached: the conditional-only Euler step from c, bf16 [n], and delta: per element, each product and sum
+ * rounded separately (no FMA), u = c - delta; g = u + scale*(c - u); x = x + dsigma*g.
+ * scail_unipc_step_cached: scail_unipc_step with u = f32(c) - delta in place of the pair's u (c bf16 [n], delta fp32 [n]);
+ * the same checks and every later instruction shared, so where delta = f32(c) - f32(u) is exact the two agree bit for
+ * bit. */
+int scail_cfg_cache_delta(const void* v, const float* d_ref, float* d_new, float* partials, int64_t partials_len, double* out,
+                          int64_t n, scail_stream_t stream);
+int scail_cfg_euler_cached(float* x, const void* c, const float* delta, int64_t n, float scale, float dsigma,
+                           scail_stream_t stream);
+int scail_unipc_step_cached(float* x, float* x_last, const void* c, const float* delta, float* slots, int64_t slot_stride,
+                            int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma, int correct,
+                            const float* coef, scail_stream_t stream);
 
 /* First-block residual cache (scail_b200/step_cache.py).  Token tensors are bf16 [B, N, d] (ref || noise || pose rows of
  * each batch element); the noise rows are rows [n_ref, n_ref + n_seq) of each element.  d % 8 == 0, B*N*d/8 < 2^31, and

@@ -16,6 +16,7 @@
 #include "../../include/scail_b200.h"
 #include "adaptive.cuh"
 #include "attention.cuh"
+#include "cfg_cache.cuh"
 #include "conv.cuh"
 #include "gemm.cuh"
 #include "rowops.cuh"
@@ -820,35 +821,93 @@ int scail_cfg_euler(float* x, const void* v, int64_t n, float scale, float dsigm
     return 0;
 }
 
+// Slot and coefficient checks shared by the two UniPC entry points; fills k.  Returns 0 or the fail() code.
+static int unipc_coef(const char* what, int64_t slot_stride, int64_t n_slots, int64_t write_slot, int64_t n,
+                      const float* coef, scail::UnipcCoef* k) {
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "%s: need n a positive multiple of 4 (got n=%lld)", what, (long long)n);
+    SCAIL_REQUIRE(n_slots >= 1 && n_slots <= scail::UNIPC_MAX_SLOTS, "%s: need 1 <= n_slots <= %d (got %lld)", what,
+                  scail::UNIPC_MAX_SLOTS, (long long)n_slots);
+    SCAIL_REQUIRE(write_slot >= 0 && write_slot < n_slots, "%s: write_slot = %lld must be in [0, n_slots = %lld)", what,
+                  (long long)write_slot, (long long)n_slots);
+    SCAIL_REQUIRE(slot_stride >= n && slot_stride % 4 == 0, "%s: slot_stride = %lld floats must be >= n = %lld and a "
+                  "multiple of 4 so that every slot is whole and 16-byte aligned", what, (long long)slot_stride, (long long)n);
+    k->a_x = coef[0];
+    k->a_m = coef[4];
+    k->b_y = coef[5];
+    k->b_m = coef[9];
+    for (int s = 0; s < scail::UNIPC_MAX_SLOTS; ++s) {
+        k->a[s] = coef[1 + s];
+        k->b[s] = coef[6 + s];
+        SCAIL_REQUIRE(s < n_slots || (k->a[s] == 0.f && k->b[s] == 0.f),
+                      "%s: the coefficients of slot %d must be 0 with n_slots = %lld", what, s, (long long)n_slots);
+    }
+    return 0;
+}
+
 int scail_unipc_step(float* x, float* x_last, const void* v, float* slots, int64_t slot_stride, int64_t n_slots,
                      int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
                      scail_stream_t stream) {
     SCAIL_REQUIRE(x && x_last && v && slots && coef, "unipc_step: null operand");
     SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(v) && aligned16(slots),
                   "unipc_step: x, x_last, v and slots must be 16-byte aligned");
-    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "unipc_step: need n a positive multiple of 4 (got n=%lld)", (long long)n);
-    SCAIL_REQUIRE(n_slots >= 1 && n_slots <= scail::UNIPC_MAX_SLOTS, "unipc_step: need 1 <= n_slots <= %d (got %lld)",
-                  scail::UNIPC_MAX_SLOTS, (long long)n_slots);
-    SCAIL_REQUIRE(write_slot >= 0 && write_slot < n_slots, "unipc_step: write_slot = %lld must be in [0, n_slots = %lld)",
-                  (long long)write_slot, (long long)n_slots);
-    SCAIL_REQUIRE(slot_stride >= n && slot_stride % 4 == 0, "unipc_step: slot_stride = %lld floats must be >= n = %lld and a "
-                  "multiple of 4 so that every slot is whole and 16-byte aligned", (long long)slot_stride, (long long)n);
     scail::UnipcCoef k;
-    k.a_x = coef[0];
-    k.a_m = coef[4];
-    k.b_y = coef[5];
-    k.b_m = coef[9];
-    for (int s = 0; s < scail::UNIPC_MAX_SLOTS; ++s) {
-        k.a[s] = coef[1 + s];
-        k.b[s] = coef[6 + s];
-        SCAIL_REQUIRE(s < n_slots || (k.a[s] == 0.f && k.b[s] == 0.f),
-                      "unipc_step: the coefficients of slot %d must be 0 with n_slots = %lld", s, (long long)n_slots);
-    }
+    if (int rc = unipc_coef("unipc_step", slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
     const int64_t nvec = n / 4;
-    scail::unipc_step_kernel<<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
-                               static_cast<cudaStream_t>(stream)>>>(
+    scail::unipc_step_kernel<false><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
+                                      static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(v), slots, slot_stride,
-        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k);
+        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, nullptr);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_unipc_step_cached(float* x, float* x_last, const void* c, const float* delta, float* slots, int64_t slot_stride,
+                            int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma, int correct,
+                            const float* coef, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && c && delta && slots && coef, "unipc_step_cached: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(c) && aligned16(delta) && aligned16(slots),
+                  "unipc_step_cached: x, x_last, c, delta and slots must be 16-byte aligned");
+    scail::UnipcCoef k;
+    if (int rc = unipc_coef("unipc_step_cached", slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
+    const int64_t nvec = n / 4;
+    scail::unipc_step_kernel<true><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
+                                     static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(c), slots, slot_stride,
+        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, reinterpret_cast<const float4*>(delta));
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_cfg_cache_delta(const void* v, const float* d_ref, float* d_new, float* partials, int64_t partials_len, double* out,
+                          int64_t n, scail_stream_t stream) {
+    SCAIL_REQUIRE(v && d_ref && d_new && partials && out, "cfg_cache_delta: null operand");
+    SCAIL_REQUIRE(aligned16(v) && aligned16(d_ref) && aligned16(d_new),
+                  "cfg_cache_delta: v, d_ref and d_new must be 16-byte aligned");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0,
+                  "cfg_cache_delta: partials must be 4-byte and out 8-byte aligned");
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "cfg_cache_delta: need n a positive multiple of 4 (got n=%lld)", (long long)n);
+    const int64_t nvec = n / 4;
+    const int ctas = static_cast<int>(std::min<int64_t>(scail::SC_MAX_CTAS, (nvec + scail::SC_THREADS - 1) / scail::SC_THREADS));
+    SCAIL_REQUIRE(partials_len >= 2 * ctas, "cfg_cache_delta: partials holds %lld floats, this size needs %d",
+                  (long long)partials_len, 2 * ctas);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    scail::cfg_cache_delta_kernel<<<ctas, scail::SC_THREADS, 0, st>>>(
+        static_cast<const uint2*>(v), reinterpret_cast<const float4*>(d_ref), reinterpret_cast<float4*>(d_new), partials, nvec);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    scail::step_cache_finish_kernel<<<1, scail::SC_THREADS, 0, st>>>(partials, ctas, out);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_cfg_euler_cached(float* x, const void* c, const float* delta, int64_t n, float scale, float dsigma,
+                           scail_stream_t stream) {
+    SCAIL_REQUIRE(x && c && delta, "cfg_euler_cached: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(c) && aligned16(delta), "cfg_euler_cached: x, c and delta must be 16-byte aligned");
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "cfg_euler_cached: need n a positive multiple of 4 (got n=%lld)", (long long)n);
+    const int64_t nvec = n / 4;
+    scail::cfg_euler_cached_kernel<<<blocks_for(nvec, scail::CFGC_THREADS), scail::CFGC_THREADS, 0,
+                                     static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<float4*>(x), static_cast<const uint2*>(c), reinterpret_cast<const float4*>(delta), nvec, scale, dsigma);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

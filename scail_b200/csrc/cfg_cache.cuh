@@ -1,0 +1,77 @@
+// CFG cache (scail_b200/cfg_cache.py): the two HBM-bound passes around a conditional-only sampler step.  A full step keeps
+// delta = f32(c) - f32(u) of its CFG pair (fp32, one subtraction rounded once) and measures how far it moved since the last
+// full step; a conditional-only step rebuilds u = f32(c) - delta.  Every thread moves 4 elements: 16-byte vectors of the
+// fp32 tensors and 8-byte vectors of bf16, as the UniPC step does.
+#pragma once
+#include <cuda_bf16.h>
+
+#include "solver.cuh"      // unipc_unpack4, unipc_load
+#include "step_cache.cuh"  // SC_THREADS, SC_MAX_CTAS, step_cache_finish_kernel, warp_sum
+
+namespace scail {
+
+constexpr int CFGC_THREADS = 256;
+
+// Pass 1 of the delta.  d_new = f32(c) - f32(u) from the pair v = [u; c] (bf16 [2, nvec * 4], cfg_euler's layout); this
+// CTA's fp32 partial sums of |d_new - d_ref| and |d_ref| -> partials[blockIdx.x] and partials[gridDim.x + blockIdx.x].  The
+// grid is a function of the size only and every thread walks the same grid-stride vectors in the same order, so the
+// partials do not depend on the device, the stream or timing.  Pass 2 is step_cache_finish_kernel.
+__global__ void __launch_bounds__(SC_THREADS) cfg_cache_delta_kernel(const uint2* __restrict__ v, const float4* __restrict__ d_ref,
+                                                                     float4* __restrict__ d_new, float* __restrict__ partials,
+                                                                     int64_t nvec) {
+    float s_diff = 0.f, s_ref = 0.f;
+    const int64_t stride = static_cast<int64_t>(gridDim.x) * SC_THREADS;
+    for (int64_t i = static_cast<int64_t>(blockIdx.x) * SC_THREADS + threadIdx.x; i < nvec; i += stride) {
+        float fu[4], fc[4], fr[4], fd[4];
+        unipc_unpack4(v[i], fu);
+        unipc_unpack4(v[nvec + i], fc);
+        unipc_load(d_ref, i, fr);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            fd[j] = __fsub_rn(fc[j], fu[j]);
+            s_diff = __fadd_rn(s_diff, fabsf(__fsub_rn(fd[j], fr[j])));
+            s_ref = __fadd_rn(s_ref, fabsf(fr[j]));
+        }
+        d_new[i] = make_float4(fd[0], fd[1], fd[2], fd[3]);
+    }
+    __shared__ float red[2][SC_THREADS / 32];
+    s_diff = warp_sum(s_diff);
+    s_ref = warp_sum(s_ref);
+    if ((threadIdx.x & 31) == 0) {
+        red[0][threadIdx.x >> 5] = s_diff;
+        red[1][threadIdx.x >> 5] = s_ref;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float a = 0.f, b = 0.f;
+#pragma unroll
+        for (int w = 0; w < SC_THREADS / 32; ++w) {
+            a += red[0][w];
+            b += red[1][w];
+        }
+        partials[blockIdx.x] = a;
+        partials[gridDim.x + blockIdx.x] = b;
+    }
+}
+
+// The conditional-only Euler step, per element in this order, each product and sum rounded on its own (no FMA):
+// u = c - delta; g = u + scale*(c - u); x = x + dsigma*g.  c is the conditional output alone (bf16 [nvec * 4]).
+__global__ void __launch_bounds__(CFGC_THREADS) cfg_euler_cached_kernel(float4* __restrict__ x, const uint2* __restrict__ c,
+                                                                        const float4* __restrict__ delta, int64_t nvec,
+                                                                        float scale, float dsigma) {
+    const int64_t i = static_cast<int64_t>(blockIdx.x) * CFGC_THREADS + threadIdx.x;
+    if (i >= nvec) return;
+    float fx[4], fc[4], fd[4];
+    unipc_load(x, i, fx);
+    unipc_unpack4(c[i], fc);
+    unipc_load(delta, i, fd);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float u = __fsub_rn(fc[j], fd[j]);
+        const float g = __fadd_rn(u, __fmul_rn(scale, __fsub_rn(fc[j], u)));
+        fx[j] = __fadd_rn(fx[j], __fmul_rn(dsigma, g));
+    }
+    x[i] = make_float4(fx[0], fx[1], fx[2], fx[3]);
+}
+
+}  // namespace scail

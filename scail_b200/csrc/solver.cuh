@@ -38,17 +38,30 @@ __device__ __forceinline__ void unipc_axpy(float (&acc)[4], float c, const float
 // `correct`, else y = x; z = b_y*y + b[k]*M_k (slot order) + b_m*m.  Writes x = z, x_last = y and slot `write_slot` = m.
 // A slot whose a[k] and b[k] are both exactly 0 is not read, and a term with a zero slot coefficient is not added, so stale
 // or NaN slots cannot leak.  Every thread reads all it needs before it writes, so the write slot may be one it reads.
+// kCached = false: v is the bf16 CFG pair [2, nvec * 4] and `delta` is not read.  kCached = true (the CFG cache's
+// conditional-only step, scail_b200/cfg_cache.py): v is the conditional output alone [nvec * 4] and u = f32(c) - delta;
+// every instruction after that is shared.  `delta` is the last parameter, so the pair instantiation's parameters keep their
+// offsets.
+template <bool kCached>
 __global__ void __launch_bounds__(UNIPC_THREADS) unipc_step_kernel(float4* __restrict__ x, float4* __restrict__ x_last,
                                                                    const uint2* __restrict__ v, float* __restrict__ slots,
                                                                    int64_t slot_stride, int n_slots, int write_slot,
                                                                    int64_t nvec, float scale, float sigma, int correct,
-                                                                   UnipcCoef k) {
+                                                                   UnipcCoef k, const float4* __restrict__ delta) {
     const int64_t i = static_cast<int64_t>(blockIdx.x) * UNIPC_THREADS + threadIdx.x;
     if (i >= nvec) return;
     float fx[4], fu[4], fc[4], m[4], y[4], z[4];
     unipc_load(x, i, fx);
-    unipc_unpack4(v[i], fu);
-    unipc_unpack4(v[nvec + i], fc);
+    if constexpr (kCached) {
+        float fd[4];
+        unipc_unpack4(v[i], fc);
+        unipc_load(delta, i, fd);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) fu[j] = __fsub_rn(fc[j], fd[j]);
+    } else {
+        unipc_unpack4(v[i], fu);
+        unipc_unpack4(v[nvec + i], fc);
+    }
     float M[UNIPC_MAX_SLOTS][4];
 #pragma unroll
     for (int s = 0; s < UNIPC_MAX_SLOTS; ++s)

@@ -161,10 +161,39 @@ class Conditioning:
         self.versions = (context._version, clip_feats._version)
         self.text = self.clip = None
         self.xkv = []  # per layer: (tkv [B*Lt, 2d], ckv [B*Lc, 2d])
+        self._rows = {}  # batch row -> its handle (row())
 
     def matches(self, context, clip_feats, batch):
         return (context is self.context and clip_feats is self.clip_feats and batch == self.batch
                 and (context._version, clip_feats._version) == self.versions)
+
+    def lookup(self, context, clip_feats, batch):
+        """This handle when it matches; else, when `context` is one batch row of this handle's context (a view
+        `context[i:i + 1]` of that very tensor object, as the CFG cache's conditional-only forward passes it) with the same
+        `clip_feats`, the handle of row i; else None."""
+        if self.matches(context, clip_feats, batch):
+            return self
+        base = self.context
+        if (batch != 1 or context._base is not base or clip_feats is not self.clip_feats
+                or (context._version, clip_feats._version) != self.versions or context.shape[0] != 1
+                or context.shape[1:] != base.shape[1:] or context.stride() != base.stride()):
+            return None
+        off = context.storage_offset() - base.storage_offset()
+        i = off // base.stride(0)
+        if off % base.stride(0) or not 0 <= i < self.batch:
+            return None
+        return self.row(i)
+
+    def row(self, i):
+        """The handle of batch row i: rows of text, clip and every layer's K,V, sliced as the context-parallel path slices
+        them (views: nothing is recomputed or copied)."""
+        r = self._rows.get(i)
+        if r is None:
+            r = self._rows[i] = Conditioning(self.context, self.clip_feats, 1)
+            r.text, r.clip = self.text[i:i + 1], self.clip[i:i + 1]
+            Lt, Lc = self.text.shape[1], self.clip.shape[1]
+            r.xkv = [(tk[i * Lt:(i + 1) * Lt], ck[i * Lc:(i + 1) * Lc]) for tk, ck in self.xkv]
+        return r
 
 
 def _need_cuda(t):
@@ -799,8 +828,8 @@ class DiffusionTransformer(nn.Module):
             ref = torch.cat([rep(ref), torch.ones(b, 1, 4, h, w, device=x.device, dtype=bf)], 2).contiguous()
             pose = torch.cat([rep(pose), torch.ones(b, t, 4, h // 2, w // 2, device=x.device, dtype=bf)], 2).contiguous()
         cond = getattr(self, "_conditioning", None)
-        if cond is not None and not cond.matches(context, kwargs["image_clip_features"], b):
-            cond = None  # different prompt / image tensors: compute everything (never reuse by address)
+        if cond is not None:  # different prompt / image tensors: compute everything (never reuse by address)
+            cond = cond.lookup(context, kwargs["image_clip_features"], b)
         text, clip, emb, adaln = self._embeddings(timesteps, context, kwargs["image_clip_features"], b, cond)
         pp = reduce(mul, self.patch_size)
         kw = dict(seq_length=t * h * w // pp, pose_length=t * (h // 2) * (w // 2) // pp, ref_length=h * w // pp,

@@ -575,6 +575,50 @@ def unipc_step_(x, x_last, v, slots, write_slot, scale, sigma, coef, correct):
     return x
 
 
+# ---------------------------------------------------------------- CFG cache (scail_b200.cfg_cache)
+def cfg_cache_delta(v, d_ref, d_new, partials, out):
+    """d_new = f32(v[1]) - f32(v[0]) (fp32, one subtraction rounded once) and out (fp64 [4]) = (sum |d_new - d_ref|,
+    sum |d_ref|, their ratio (+inf for a zero denominator), 0); v bf16 [2, ...] (the CFG pair as cfg_euler_ reads it),
+    d_ref, d_new fp32 with v[0]'s element count, partials fp32 [>= STEP_CACHE_PARTIALS] scratch.  Bit-reproducible.
+    Returns out."""
+    _req(v), _req(d_ref, torch.float32), _req(d_new, torch.float32), _req(partials, torch.float32), _req(out, torch.float64)
+    n = d_new.numel()
+    assert v.is_contiguous() and v.numel() == 2 * n and d_ref.is_contiguous() and d_new.is_contiguous() and d_ref.numel() == n
+    assert partials.is_contiguous() and out.is_contiguous() and out.numel() >= 4
+    _lib.check(_lib.lib().scail_cfg_cache_delta(_ptr(v), _ptr(d_ref), _ptr(d_new), _ptr(partials), partials.numel(), _ptr(out),
+                                                n, _stream()), "scail_cfg_cache_delta")
+    _count(2)
+    return out
+
+
+def cfg_euler_cached_(x, c, delta, scale, dsigma):
+    """The conditional-only Euler step, in place on x (fp32): u = c - delta; g = u + scale*(c - u); x = x + dsigma*g, each
+    product and sum rounded on its own.  c bf16 (the conditional output alone), delta fp32, both with x's element count."""
+    _req(x, torch.float32), _req(c), _req(delta, torch.float32)
+    assert x.is_contiguous() and c.is_contiguous() and delta.is_contiguous() and c.numel() == x.numel() == delta.numel()
+    _lib.check(_lib.lib().scail_cfg_euler_cached(_ptr(x), _ptr(c), _ptr(delta), x.numel(), float(scale), float(dsigma),
+                                                 _stream()), "scail_cfg_euler_cached")
+    _count()
+    return x
+
+
+def unipc_step_cached_(x, x_last, c, delta, slots, write_slot, scale, sigma, coef, correct):
+    """unipc_step_ with u = f32(c) - delta in place of the pair's u: c bf16 (the conditional output alone), delta fp32, both
+    with x's element count; everything else as unipc_step_.  Returns x."""
+    _req(x, torch.float32), _req(x_last, torch.float32), _req(c), _req(delta, torch.float32), _req(slots, torch.float32)
+    assert x.is_contiguous() and x_last.is_contiguous() and x_last.shape == x.shape
+    assert c.is_contiguous() and delta.is_contiguous() and c.numel() == x.numel() == delta.numel()
+    assert slots.dim() == 2 and slots.is_contiguous() and slots.shape[1] == x.numel(), tuple(slots.shape)
+    assert len(coef) == 10
+    k = (ctypes.c_float * 10)(*coef)
+    _lib.check(_lib.lib().scail_unipc_step_cached(_ptr(x), _ptr(x_last), _ptr(c), _ptr(delta), _ptr(slots), slots.stride(0),
+                                                  slots.shape[0], int(write_slot), x.numel(), float(scale), float(sigma),
+                                                  int(bool(correct)), ctypes.addressof(k), _stream()),
+               "scail_unipc_step_cached")
+    _count()
+    return x
+
+
 # ---------------------------------------------------------------- first-block residual cache (scail_b200.step_cache)
 STEP_CACHE_PARTIALS = 2048  # fp32 partial sums of step_cache_indicator: 2 per CTA, at most 1024 CTAs
 

@@ -10,7 +10,8 @@ The latent stays fp32 across steps (diffusion_video.py:470); the DiT consumes/pr
 import numpy as np
 import torch
 
-from . import ops
+from . import cfg_cache as cfgc
+from . import dit, ops
 from .step_cache import check_supported
 
 
@@ -30,8 +31,19 @@ def prepare_context(cond, uc):
     return torch.cat((u, c), 0)
 
 
+def _adaln(model):
+    return model.mixins["adaln_layer"] if hasattr(model, "mixins") else None
+
+
+def _check_cfg_cache(model, cfg_cache, plan=None, model_kwargs=None):
+    """Validate a cfg_cache argument and refuse what it does not cover (scail_b200.cfg_cache.check_supported)."""
+    if cfgc.check_cache(cfg_cache) is not None:
+        mk = model_kwargs or {}
+        cfgc.check_supported(getattr(_adaln(model), "cp", None), mk.get("chunk_dim"), mk.get("_num_layers"), plan)
+
+
 def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, plan=None, _x_override=None, _sigma_override=None,
-                 step_cache=None, solver=None, **model_kwargs):
+                 step_cache=None, solver=None, cfg_cache=None, **model_kwargs):
     """One reference sampler step: x [1,t,16,h,w] fp32 (updated in place and returned).
     cond/uc: dicts with 'crossattn' [1,L,text_dim]; cond also carries ref_concat, concat_smpl_render,
     image_clip_features, concat_images (shared by both CFG branches, guiders.py:50-56).
@@ -40,11 +52,17 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     step_cache: an optional scail_b200.step_cache.FirstBlockCache, passed to the forward with this step's sigma (single GPU
     only).
     solver: an optional scail_b200.unipc.UniPC with a bound schedule; its step replaces the Euler update.  (sigma, next_sigma)
-    must be the solver's next pair and x its latent, else ValueError before anything runs."""
+    must be the solver's next pair and x its latent, else ValueError before anything runs.
+    cfg_cache: an optional scail_b200.cfg_cache.CFGCache (single GPU only).  It decides before the forward whether this step
+    runs the conditional branch alone (b = 1, on the cache's stream) and rebuilds u = c - delta for the update; the
+    first-block cache then sits the step out."""
+    _check_cfg_cache(model, cfg_cache, plan, model_kwargs)
     if solver is not None:
         solver.check_step(x, sigma, next_sigma)
     if step_cache is not None:
         check_supported(plan=plan)
+    cond_only = cfg_cache is not None and cfg_cache.begin_step(x)
+    if step_cache is not None and not cond_only:
         step_cache.set_sigma(sigma if _sigma_override is None else _sigma_override)
         model_kwargs["_step_cache"] = step_cache
     ctx = _ctx if _ctx is not None else prepare_context(cond, uc)
@@ -52,6 +70,12 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
               image_clip_features=cond["image_clip_features"], concat_images=cond.get("concat_images"), **model_kwargs)
     x_in = x if _x_override is None else _x_override          # guided_velocity(): forward on x_in, accumulate into a zero latent
     c_noise = float(sigma if _sigma_override is None else _sigma_override) * 1000.0  # RFScaling: c_noise = 1000 sigma
+    if cond_only:
+        ts = torch.full((1,), c_noise, device=x.device, dtype=torch.float32)
+        c = cfg_cache.cond_forward(model, x_in, ts, ctx[1:2], kw)
+        if solver is not None:
+            return solver.step(x, c, scale, sigma, next_sigma, delta=cfg_cache.delta)
+        return ops.cfg_euler_cached_(x, c, cfg_cache.delta, scale, float(next_sigma) - float(sigma))
     if plan is None:
         x2 = torch.cat([x_in, x_in], 0)
         ts = torch.full((2,), c_noise, device=x.device, dtype=torch.float32)
@@ -60,16 +84,23 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
         b = plan.branch
         ts = torch.full((1,), c_noise, device=x.device, dtype=torch.float32)
         v = plan.gather_branches(model(x_in, timesteps=ts, context=ctx[b:b + 1], **kw))
+    if cfg_cache is not None:
+        cfg_cache.full_step(v.contiguous())
     if solver is not None:
         return solver.step(x, v.contiguous(), scale, sigma, next_sigma)
     return ops.cfg_euler_(x, v.contiguous(), scale, float(next_sigma) - float(sigma))
 
 
-def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None, step_cache=None, solver=None):
+def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None, step_cache=None, solver=None, cfg_cache=None):
     """RFSampler.__call__ (sampling.py:965-982): the full Euler loop.  With `adaln_layer.cache_cross_kv` the step-invariant
     conditioning (text / CLIP embeddings and all layers' cross-attention K,V) is computed once for this call.  step_cache (a
     scail_b200.step_cache.FirstBlockCache) is reset here and then decides on every step whether blocks 1..L-1 run.
-    solver (a scail_b200.unipc.UniPC) is bound to this call's schedule here and replaces the Euler update on every step."""
+    solver (a scail_b200.unipc.UniPC) is bound to this call's schedule here and replaces the Euler update on every step.
+    cfg_cache (a scail_b200.cfg_cache.CFGCache) is reset here and then decides on every step whether only the conditional
+    branch runs; with cache_cross_kv that forward reads the cond row of this call's conditioning."""
+    _check_cfg_cache(model, cfg_cache, plan)
+    if cfg_cache is not None:
+        cfg_cache.reset()
     if step_cache is not None:
         check_supported(plan=plan)
         step_cache.reset()
@@ -84,7 +115,7 @@ def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=No
     try:
         for i in range(num_steps):
             x = sampler_step(model, x, sig[i], sig[i + 1], cond, uc, scale, _ctx=ctx, plan=plan, step_cache=step_cache,
-                             solver=solver)
+                             solver=solver, cfg_cache=cfg_cache)
     finally:
         if cache:
             model.clear_conditioning()
@@ -173,9 +204,14 @@ class GraphedStep:
     cache's control block: the host writes it between graph (1) and the tail, so the same graphs serve every step.
     solver (a scail_b200.unipc.UniPC, with a schedule bound by solver.begin): its step runs eagerly after the replay, in
     place of CFG+Euler, with its coefficients passed by value, so no graph depends on it; the step is validated before
-    anything runs."""
+    anything runs.
+    cfg_cache (a scail_b200.cfg_cache.CFGCache, reset at construction): the conditional-only forward (b = 1 on the cond
+    row) is one more graph, captured on a stream of this object's own so that it has its own workspace; the host decides
+    before each step which graphs replay.  Every graph's workspace tensors are held here (_workspace_of).  The delta kernel and the updates run eagerly after the replay (delta_ref and delta_new
+    alternate between two buffers, which a graph would fix)."""
 
-    def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None, solver=None):
+    def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None, solver=None, cfg_cache=None):
+        _check_cfg_cache(model, cfg_cache)
         if step_cache is not None:
             check_supported(getattr(model.mixins["adaln_layer"], "cp", None))
         if getattr(model.mixins["adaln_layer"], "cp", None) is not None:
@@ -192,7 +228,10 @@ class GraphedStep:
         self.fp8 = getattr(self.adaln, "fp8_linear", False)
         # the e4m3 weights are derived on this stream and held here: the graph replays against these very buffers
         self._fp8_weights = self.adaln.prepare_fp8_weights() if self.fp8 else []
-        self.step_cache = step_cache
+        self.step_cache, self.cfg_cache = step_cache, cfg_cache
+        if cfg_cache is not None:
+            cfg_cache.reset()
+            self._capture_cond()
         if step_cache is not None:
             step_cache.reset()
             self._capture_cached()
@@ -208,9 +247,30 @@ class GraphedStep:
         with torch.cuda.graph(self.graph, stream=side), torch.no_grad():
             self.v = self._forward()
         self.kernels_in_graph = ops.LAUNCHES - n0
+        self._ws = _workspace_of(side)
 
     def _forward(self):
         return self.model(torch.cat([self.x, self.x], 0), timesteps=self.ts, context=self.ctx, **self.kw).contiguous()
+
+    def _capture_cond(self):
+        """The conditional-only forward as one graph on a capture stream of its own (so its b = 1 workspace is not the b = 2
+        graph's): x itself (b = 1), timesteps [1] and the cond row of the context."""
+        dev = self.x.device
+        self.ts1 = torch.zeros(1, device=dev, dtype=torch.float32)
+        self.ctx1 = self.ctx[1:2]
+        side, main = torch.cuda.Stream(device=dev), torch.cuda.current_stream(dev)
+        fwd = lambda: self.model(self.x, timesteps=self.ts1, context=self.ctx1, **self.kw).contiguous()
+        side.wait_stream(main)
+        with torch.cuda.stream(side), torch.no_grad():  # warm-up: the capture stream's workspace and TMA descriptors exist
+            fwd()
+        main.wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.graph1 = torch.cuda.CUDAGraph()
+        n0 = ops.LAUNCHES
+        with torch.cuda.graph(self.graph1, stream=side), torch.no_grad():
+            self.v1 = fwd()
+        self.kernels_in_graph1 = ops.LAUNCHES - n0
+        self._ws1 = _workspace_of(side)
 
     def _head(self):
         return self.model.step_cache_head(self.step_cache, torch.cat([self.x, self.x], 0), timesteps=self.ts, context=self.ctx,
@@ -246,10 +306,13 @@ class GraphedStep:
             self.v_skip = self.model.step_cache_tail(self.head, True).contiguous()
         self.graphs = graphs
         self.kernels_in_graph = ops.LAUNCHES - n0
+        self._ws = _workspace_of(side)
 
-    def _update(self, v, sigma, next_sigma):
+    def _update(self, v, sigma, next_sigma, delta=None):
         if self.solver is not None:
-            return self.solver.step(self.x, v, self.scale, sigma, next_sigma)
+            return self.solver.step(self.x, v, self.scale, sigma, next_sigma, delta=delta)
+        if delta is not None:
+            return ops.cfg_euler_cached_(self.x, v, delta, self.scale, float(next_sigma) - float(sigma))
         return ops.cfg_euler_(self.x, v, self.scale, float(next_sigma) - float(sigma))
 
     def __call__(self, sigma, next_sigma):
@@ -257,10 +320,22 @@ class GraphedStep:
             self.solver.check_step(self.x, sigma, next_sigma)
         if self.fp8:
             self.adaln.prepare_fp8_weights()
+        cc = self.cfg_cache
+        if cc is not None and cc.begin_step(self.x):
+            self.ts1.fill_(float(sigma) * 1000.0)
+            self.graph1.replay()
+            return self._update(self.v1, sigma, next_sigma, cc.delta)
+        v = self._full(sigma)
+        if cc is not None:
+            cc.full_step(v)
+        return self._update(v, sigma, next_sigma)
+
+    def _full(self, sigma):
+        """Replay the b = 2 forward (with the first-block cache's decision between its graphs) -> the CFG pair."""
         self.ts.fill_(float(sigma) * 1000.0)
         if self.step_cache is None:
             self.graph.replay()
-            return self._update(self.v, sigma, next_sigma)
+            return self.v
         sc = self.step_cache
         sc.set_sigma(sigma)
         sc.begin()
@@ -274,7 +349,15 @@ class GraphedStep:
         self.graphs[2 if skip else 1].replay()
         if not skip:
             sc.computed()
-        return self._update(self.v_skip if skip else self.v_run, sigma, next_sigma)
+        return self.v_skip if skip else self.v_run
+
+
+def _workspace_of(stream):
+    """The DiT workspace tensors of `stream`, which a graph just captured on it reads and writes.  GraphedStep holds them:
+    stream handles come from a pool and recur, so another forward on a stream with the same handle may later replace the
+    workspace entries (dit._Workspace frees a buffer whose shape changes), and the graph must keep its memory."""
+    h = stream.cuda_stream
+    return [b for k, b in dit._WS.bufs.items() if k[0][1] == h]
 
 
 class HostStep:

@@ -34,13 +34,14 @@ import torch
 from . import ops
 
 
-def check_threshold(threshold):
-    """A float >= 0 (inf allowed).  Raises TypeError for bools and non-numbers, ValueError for NaN and negatives."""
+def check_threshold(threshold, what="step cache"):
+    """A float >= 0 (inf allowed).  Raises TypeError for bools and non-numbers, ValueError for NaN and negatives; the
+    messages name `what`."""
     if isinstance(threshold, bool) or not isinstance(threshold, numbers.Real):
-        raise TypeError(f"step cache threshold must be a real number >= 0 (inf allowed), got {threshold!r}")
+        raise TypeError(f"{what} threshold must be a real number >= 0 (inf allowed), got {threshold!r}")
     t = float(threshold)
     if math.isnan(t) or t < 0:
-        raise ValueError(f"step cache threshold must be >= 0 (inf allowed), got {threshold!r}")
+        raise ValueError(f"{what} threshold must be >= 0 (inf allowed), got {threshold!r}")
     return t
 
 
@@ -54,14 +55,15 @@ def check_order(order):
     return int(order)
 
 
-def check_max_skips(max_skips):
-    """None (no cap) or an int >= 0.  Raises TypeError for bools and non-ints, ValueError for negatives."""
+def check_max_skips(max_skips, what="step cache"):
+    """None (no cap) or an int >= 0.  Raises TypeError for bools and non-ints, ValueError for negatives; the messages name
+    `what`."""
     if max_skips is None:
         return None
     if isinstance(max_skips, bool) or not isinstance(max_skips, numbers.Integral):
-        raise TypeError(f"step cache max_skips must be None or an int >= 0, got {max_skips!r}")
+        raise TypeError(f"{what} max_skips must be None or an int >= 0, got {max_skips!r}")
     if int(max_skips) < 0:
-        raise ValueError(f"step cache max_skips must be None or an int >= 0, got {max_skips!r}")
+        raise ValueError(f"{what} max_skips must be None or an int >= 0, got {max_skips!r}")
     return int(max_skips)
 
 

@@ -226,8 +226,10 @@ class UniPC:
             raise ValueError(f"solver: the latent {tuple(x.shape)} {x.dtype} on {x.device} is not the latent "
                              f"{self._key[0]} {self._key[1]} on {self._key[2]} the solver's state was built for")
 
-    def step(self, x, v, scale, sigma, next_sigma):
-        """One solver step in place on x (fp32), from the CFG pair v (bf16 [2, ...], as cfg_euler_ reads it).  Returns x."""
+    def step(self, x, v, scale, sigma, next_sigma, delta=None):
+        """One solver step in place on x (fp32), from the CFG pair v (bf16 [2, ...], as cfg_euler_ reads it).  With `delta`
+        (fp32, x's element count: a scail_b200.cfg_cache.CFGCache's held c - u), v is the conditional output alone (bf16
+        [1, ...]) and u = f32(c) - delta; the coefficients and the state are those of the pair step.  Returns x."""
         self.check_step(x, sigma, next_sigma)
         i = self._i
         if i == 0:
@@ -241,6 +243,10 @@ class UniPC:
         k = step_coefficients(self._sigmas, i, self._order)
         pad = [0.0] * (3 - self._order)
         coef = [k.x_last_c, *k.slot_c, *pad, k.m_c, k.y_c, *k.slot_p, *pad, k.m_p]
-        ops.unipc_step_(x, self.x_last, v, self.slots, k.write, scale, self._sigmas[i], [_f32(c) for c in coef], k.correct)
+        coef = [_f32(c) for c in coef]
+        if delta is None:
+            ops.unipc_step_(x, self.x_last, v, self.slots, k.write, scale, self._sigmas[i], coef, k.correct)
+        else:
+            ops.unipc_step_cached_(x, self.x_last, v, delta, self.slots, k.write, scale, self._sigmas[i], coef, k.correct)
         self._i = i + 1
         return x
