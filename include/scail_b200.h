@@ -242,6 +242,25 @@ int scail_cfg_euler_cached(float* x, const void* c, const float* delta, int64_t 
 int scail_unipc_step_cached(float* x, float* x_last, const void* c, const float* delta, float* slots, int64_t slot_stride,
                             int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma, int correct,
                             const float* coef, scail_stream_t stream);
+/* CFG cache forecast (CFGCache(order >= 1)): n_slots (1..3) fp32 delta slots of n elements, slot s at slots + s*slot_stride
+ * floats (slot_stride >= n, a multiple of 4), and coef: 3 host floats, the forecast coefficient of each slot (0 for every
+ * slot s >= n_slots).  The forecast is t = c0*S0, then t = t + c1*S1, then t = t + c2*S2, each product and sum rounded on
+ * its own (no FMA); a slot whose coefficient is exactly 0 is not read, and with no active slot t = 0.
+ * scail_cfg_cache_delta_forecast: slot write_slot = f32(c) - f32(u) from the pair v [2, n] and out = {sum |d_new - t|,
+ * sum |t|, ratio, 0}, in scail_cfg_cache_delta's partition and order (bit-reproducible; with coef = 1 on one slot alone
+ * its sums are scail_cfg_cache_delta's with d_ref = that slot, bit for bit).  The write slot may be one t reads.
+ * scail_cfg_euler_cached_forecast: scail_cfg_euler_cached with delta = t.
+ * scail_unipc_step_cached_forecast: scail_unipc_step_cached with delta = t of the delta slots (dslots, dslot_stride,
+ * n_dslots, dcoef); the UniPC slots and coefficients as scail_unipc_step. */
+int scail_cfg_cache_delta_forecast(const void* v, float* slots, int64_t slot_stride, int64_t n_slots, int64_t write_slot,
+                                   const float* coef, float* partials, int64_t partials_len, double* out, int64_t n,
+                                   scail_stream_t stream);
+int scail_cfg_euler_cached_forecast(float* x, const void* c, const float* slots, int64_t slot_stride, int64_t n_slots,
+                                    const float* coef, int64_t n, float scale, float dsigma, scail_stream_t stream);
+int scail_unipc_step_cached_forecast(float* x, float* x_last, const void* c, const float* dslots, int64_t dslot_stride,
+                                     int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride, int64_t n_slots,
+                                     int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                                     scail_stream_t stream);
 
 /* First-block residual cache (scail_b200/step_cache.py).  Token tensors are bf16 [B, N, d] (ref || noise || pose rows of
  * each batch element); the noise rows are rows [n_ref, n_ref + n_seq) of each element.  d % 8 == 0, B*N*d/8 < 2^31, and

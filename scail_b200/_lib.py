@@ -67,6 +67,10 @@ SIGNATURES = {
     "scail_cfg_cache_delta": [c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_p],
     "scail_cfg_euler_cached": [c_p, c_p, c_p, c_i64, c_f, c_f, c_p],
     "scail_unipc_step_cached": [c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f, c_f, c_int, c_p, c_p],
+    "scail_cfg_cache_delta_forecast": [c_p, c_p, c_i64, c_i64, c_i64, c_p, c_p, c_i64, c_p, c_i64, c_p],
+    "scail_cfg_euler_cached_forecast": [c_p, c_p, c_p, c_i64, c_i64, c_p, c_i64, c_f, c_f, c_p],
+    "scail_unipc_step_cached_forecast": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f, c_f,
+                                         c_int, c_p, c_p],
     "scail_step_cache_indicator": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_update": [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_apply": [c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],

@@ -2,8 +2,8 @@
 
 Every sampler step runs the DiT on the CFG batch [uncond, cond] (b = 2).  The difference delta = c - u of the two outputs
 changes slowly over late steps, so some steps can run the conditional branch alone (b = 1) and rebuild the unconditional
-output as u = c - delta, with delta from the last full step (a hold: delta is not forecast in sigma).  This module owns the
-policy:
+output as u = c - delta, with delta from the last full step (order 0, a hold) or forecast in sigma from the last full
+steps (order >= 1, below).  This module owns the policy:
 
   full step         the b = 2 forward, then ops.cfg_cache_delta: delta_new = f32(c) - f32(u) (fp32 [1, t, 16, h, w], one
                     subtraction rounded once) and the sums num = sum|delta_new - delta_ref|, den = sum|delta_ref|, where
@@ -25,13 +25,34 @@ which is dropped when the cache is garbage-collected.  torch.cuda.Stream() hands
 objects may still come to share one handle and hence one workspace; for eager forwards that costs a reallocation at most,
 and GraphedStep keeps the workspace tensors its graphs were captured against (see sampler.GraphedStep), so no graph ever
 reads freed memory.  No default threshold is chosen: that needs real weights and a visual check.
+
+Taylor forecast (order >= 1).  Instead of holding delta, the cache keeps delta of the last order + 1 full steps, each with
+the sampler's sigma of its step, in order + 1 fp32 slots shaped like the latent (zero-filled at allocation); the j-th full
+step since reset() writes slot j mod (order + 1).  The forecast at sigma is step_cache.forecast_coefficients(sigma, slot
+sigmas, full steps so far, order): the Lagrange polynomial in sigma through the m + 1 most recent full steps, m = min(order,
+full steps - 1), reduced until their sigmas are pairwise distinct, with its fp64 coefficients rounded once to fp32 (the
+first-block cache's forecast).  On the device delta_hat = c0*S0, then + c1*S1, then + c2*S2, every product and sum rounded
+on its own, and a slot whose coefficient is 0 is not read.
+
+  full step j       ops.cfg_cache_delta_forecast: slot j mod (order + 1) = f32(c) - f32(u), and the sums num = sum|delta_j -
+                    delta_hat|, den = sum|delta_hat| against the forecast at sigma_j from the j earlier full steps, so the
+                    indicator measures how far the forecast was off.  At j = 0 every coefficient is 0 (+inf); at j = 1 the
+                    forecast is the hold, and the sums are cfg_cache_delta's bit for bit.  The slot written may be the oldest
+                    one the forecast reads: the kernel reads all of an element before it writes it.
+  decision          unchanged.
+  conditional-only  u = f32(c) - delta_hat(sigma) from the order + 1 most recent full steps: ops.cfg_euler_cached_forecast_
+                    or UniPC.step(forecast=).
+
+The coefficients are kernel arguments, so nothing here is captured in a graph.  Each step needs its sigma on the host
+(begin_step(x, sigma)); sampler_step and GraphedStep pass it.  Memory: order + 1 fp32 latents instead of 2 (16.5 MB at
+512x512 and 29 MB at 512x896 at order 2).  No default order is chosen either.
 """
 import weakref
 
 import torch
 
 from . import ops
-from .step_cache import check_max_skips, check_threshold, indicator
+from .step_cache import check_max_skips, check_order, check_sigma, check_threshold, forecast_coefficients, indicator
 
 def _drop_workspaces(handles):
     """Free the per-stream DiT workspace of the given stream handles (a CFGCache's streams, once it is collected)."""
@@ -65,13 +86,21 @@ def check_cache(cfg_cache):
 
 class Buffers:
     """The cache's device state for one latent (shape, device): delta_ref and delta_new (fp32, the latent's shape; delta_ref
-    zero-filled), the delta kernel's partial sums and its fp64 result {num, den, ratio, 0}."""
+    zero-filled), the delta kernel's partial sums and its fp64 result {num, den, ratio, 0}.  At order >= 1, d_ref and d_new
+    are None and `slots` (fp32 [order + 1, *shape], zero-filled) takes their place, with slot_sigma (the sigma of the full
+    step each slot holds, None while empty) and n_full (full steps written since allocation)."""
 
-    def __init__(self, key):
+    def __init__(self, key, order=0):
         shape, device = key
         self.key = key
-        self.d_ref = torch.zeros(shape, device=device, dtype=torch.float32)
-        self.d_new = torch.empty(shape, device=device, dtype=torch.float32)
+        self.d_ref = self.d_new = self.slots = None
+        if order == 0:
+            self.d_ref = torch.zeros(shape, device=device, dtype=torch.float32)
+            self.d_new = torch.empty(shape, device=device, dtype=torch.float32)
+        else:
+            self.slots = torch.zeros((order + 1, *shape), device=device, dtype=torch.float32)
+            self.slot_sigma = [None] * (order + 1)
+            self.n_full = 0
         self.partials = torch.empty(ops.STEP_CACHE_PARTIALS, device=device, dtype=torch.float32)
         self.out = torch.zeros(4, device=device, dtype=torch.float64)
 
@@ -81,7 +110,7 @@ class Buffers:
         return indicator(num, den)
 
     def nbytes(self):
-        return sum(t.numel() * t.element_size() for t in (self.d_ref, self.d_new))
+        return sum(t.numel() * t.element_size() for t in (self.d_ref, self.d_new, self.slots) if t is not None)
 
 
 class CFGCache:
@@ -90,11 +119,17 @@ class CFGCache:
     threshold (float >= 0, inf allowed; validated as FirstBlockCache's) may change between steps.  max_skips (None or an
     int >= 0): after that many conditional-only steps in a row the next step is full (0: never skip).  `history` lists
     (indicator, cond_only) for every step since reset(): the indicator the step decided on, i.e. that of the last full
-    step, or None while the cache holds no delta."""
+    step, or None while the cache holds no delta.
 
-    def __init__(self, threshold, max_skips=None):
+    order (0, 1 or 2; validated as FirstBlockCache's): the degree of the forecast of delta in the sampler's sigma.  0 holds
+    delta of the last full step; 1 and 2 extrapolate it from the last 2 or 3 full steps and measure each full step against
+    that forecast (see the module docstring), at the cost of order + 1 fp32 latents instead of 2.  At order >= 1 every
+    step needs its sigma (begin_step(x, sigma)); sampler_step and GraphedStep pass it."""
+
+    def __init__(self, threshold, max_skips=None, order=0):
         self.threshold = threshold
         self.max_skips = max_skips
+        self._order = check_order(order, "cfg_cache")
         self._streams = {}  # device index -> this cache's stream for the conditional-only forward
         self._handles = set()  # every stream handle this cache ran a forward on: their workspaces go with the cache
         weakref.finalize(self, _drop_workspaces, self._handles)
@@ -109,6 +144,10 @@ class CFGCache:
         self._threshold = check_threshold(value, "cfg_cache")
 
     @property
+    def order(self):
+        return self._order
+
+    @property
     def max_skips(self):
         return self._max_skips
 
@@ -117,17 +156,21 @@ class CFGCache:
         self._max_skips = check_max_skips(value, "cfg_cache")
 
     def reset(self):
-        """Drop the held delta and its buffers: the next two steps are full."""
+        """Drop the held delta and its buffers (the forecast slots and their sigmas with them): the next two steps are full."""
         self.buffers = None
         self._ind = None  # indicator of the last full step; None while no delta is held
         self._pending = False  # the last full step's sums are on the device, not yet read
         self._run = 0  # consecutive conditional-only steps
+        self._sigma = None  # sigma of the current step (order >= 1)
         self.history = []
 
     @property
     def delta(self):
-        """delta_ref: c - u of the last full step (fp32, the latent's shape), or None."""
-        return None if self.buffers is None else self.buffers.d_ref
+        """c - u of the last full step (fp32, the latent's shape: delta_ref, or at order >= 1 its slot), or None."""
+        b = self.buffers
+        if b is None or self._order == 0:
+            return None if b is None else b.d_ref
+        return None if b.n_full == 0 else b.slots[(b.n_full - 1) % (self._order + 1)]
 
     def decide(self, ind):
         """The pure rule: ind is the indicator of the last full step, or None when no delta is held.  Conditional-only iff
@@ -138,9 +181,15 @@ class CFGCache:
         self.history.append((ind, cond_only))
         return cond_only
 
-    def begin_step(self, x):
-        """Before a step's forward on the latent x: read the last full step's sums if they are still on the device, then
-        decide.  A latent of another shape or device than the held delta's drops the state first."""
+    def begin_step(self, x, sigma=None):
+        """Before a step's forward on the latent x at the sampler's `sigma`: read the last full step's sums if they are still
+        on the device, then decide.  A latent of another shape or device than the held delta's drops the state first.  At
+        order >= 1 sigma is required: without it, ValueError before anything is read or recorded."""
+        if self._order >= 1:
+            if sigma is None:
+                raise ValueError(f"cfg_cache: a CFGCache of order {self._order} needs the sampler's sigma of every step "
+                                 "(begin_step(x, sigma)); sampler_step and GraphedStep pass it")
+            self._sigma = check_sigma(sigma, "cfg_cache")
         if self.buffers is not None and self.buffers.key != (tuple(x.shape), x.device):
             self.buffers, self._ind, self._pending = None, None, False
         if self._pending:
@@ -148,16 +197,47 @@ class CFGCache:
             self._pending = False
         return self.decide(self._ind)
 
+    def full_control(self):
+        """(slot, coefficients) of the next full step at order >= 1: it writes slot n_full mod (order + 1) and measures
+        against the forecast at this step's sigma from the earlier full steps (all zero before the first)."""
+        b = self.buffers
+        return b.n_full % (self._order + 1), forecast_coefficients(self._sigma, b.slot_sigma, b.n_full, self._order)
+
+    def forecast(self):
+        """The coefficients of delta_hat at this step's sigma from the order + 1 most recent full steps (order >= 1)."""
+        b = self.buffers
+        return forecast_coefficients(self._sigma, b.slot_sigma, b.n_full, self._order)
+
     def full_step(self, v):
         """After a full step's forward, v the bf16 CFG pair [2, t, 16, h, w]: launch the delta kernel and swap delta_ref and
-        delta_new.  The sums are read by the next begin_step."""
+        delta_new (at order >= 1: write the next slot, tag it with this step's sigma).  The sums are read by the next
+        begin_step."""
         key = ((1, *v.shape[1:]), v.device)
         if self.buffers is None:
-            self.buffers = Buffers(key)
+            self.buffers = Buffers(key, self._order)
         b = self.buffers
-        ops.cfg_cache_delta(v, b.d_ref, b.d_new, b.partials, b.out)
-        b.d_ref, b.d_new = b.d_new, b.d_ref
+        if self._order == 0:
+            ops.cfg_cache_delta(v, b.d_ref, b.d_new, b.partials, b.out)
+            b.d_ref, b.d_new = b.d_new, b.d_ref
+        else:
+            slot, coef = self.full_control()
+            ops.cfg_cache_delta_forecast(v, b.slots, slot, coef, b.partials, b.out)
+            b.slot_sigma[slot] = self._sigma
+            b.n_full += 1
         self._pending = True
+
+    def cond_update(self, x, c, scale, sigma, next_sigma, solver=None):
+        """The conditional-only step's latent update in place on x from c, the conditional output alone (bf16 [1, ...]): u =
+        f32(c) - delta (order 0) or f32(c) - delta_hat(sigma) (order >= 1), then the Euler step, or solver.step (a UniPC)
+        when given.  Returns x."""
+        if self._order == 0:
+            if solver is not None:
+                return solver.step(x, c, scale, sigma, next_sigma, delta=self.delta)
+            return ops.cfg_euler_cached_(x, c, self.delta, scale, float(next_sigma) - float(sigma))
+        fc = (self.buffers.slots, self.forecast())
+        if solver is not None:
+            return solver.step(x, c, scale, sigma, next_sigma, forecast=fc)
+        return ops.cfg_euler_cached_forecast_(x, c, *fc, scale, float(next_sigma) - float(sigma))
 
     def stream(self, device):
         """This cache's stream for the conditional-only forward on `device`, created on first use.  Should the caller come

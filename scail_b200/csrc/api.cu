@@ -856,7 +856,7 @@ int scail_unipc_step(float* x, float* x_last, const void* v, float* slots, int64
     scail::unipc_step_kernel<false><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
                                       static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(v), slots, slot_stride,
-        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, nullptr);
+        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, nullptr, 0, scail::DeltaForecast{});
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -873,7 +873,85 @@ int scail_unipc_step_cached(float* x, float* x_last, const void* c, const float*
     scail::unipc_step_kernel<true><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
                                      static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(c), slots, slot_stride,
-        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, reinterpret_cast<const float4*>(delta));
+        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, reinterpret_cast<const float4*>(delta), 0,
+        scail::DeltaForecast{});
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// Checks shared by the forecast entry points of the CFG cache's delta slots; fills k.  Returns 0 or the fail() code.
+static int delta_forecast_coef(const char* what, int64_t slot_stride, int64_t n_slots, int64_t n, const float* coef,
+                               scail::DeltaForecast* k) {
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "%s: need n a positive multiple of 4 (got n=%lld)", what, (long long)n);
+    SCAIL_REQUIRE(n_slots >= 1 && n_slots <= scail::DELTA_MAX_SLOTS, "%s: need 1 <= n_slots <= %d delta slots (got %lld)",
+                  what, scail::DELTA_MAX_SLOTS, (long long)n_slots);
+    SCAIL_REQUIRE(slot_stride >= n && slot_stride % 4 == 0, "%s: delta slot_stride = %lld floats must be >= n = %lld and a "
+                  "multiple of 4 so that every slot is whole and 16-byte aligned", what, (long long)slot_stride, (long long)n);
+    for (int s = 0; s < scail::DELTA_MAX_SLOTS; ++s) {
+        k->c[s] = coef[s];
+        SCAIL_REQUIRE(s < n_slots || k->c[s] == 0.f, "%s: the forecast coefficient of delta slot %d must be 0 with n_slots = %lld",
+                      what, s, (long long)n_slots);
+    }
+    return 0;
+}
+
+int scail_cfg_cache_delta_forecast(const void* v, float* slots, int64_t slot_stride, int64_t n_slots, int64_t write_slot,
+                                   const float* coef, float* partials, int64_t partials_len, double* out, int64_t n,
+                                   scail_stream_t stream) {
+    SCAIL_REQUIRE(v && slots && coef && partials && out, "cfg_cache_delta_forecast: null operand");
+    SCAIL_REQUIRE(aligned16(v) && aligned16(slots), "cfg_cache_delta_forecast: v and slots must be 16-byte aligned");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0,
+                  "cfg_cache_delta_forecast: partials must be 4-byte and out 8-byte aligned");
+    scail::DeltaForecast k;
+    if (int rc = delta_forecast_coef("cfg_cache_delta_forecast", slot_stride, n_slots, n, coef, &k)) return rc;
+    SCAIL_REQUIRE(write_slot >= 0 && write_slot < n_slots,
+                  "cfg_cache_delta_forecast: write_slot = %lld must be in [0, n_slots = %lld)", (long long)write_slot,
+                  (long long)n_slots);
+    const int64_t nvec = n / 4;
+    const int ctas = static_cast<int>(std::min<int64_t>(scail::SC_MAX_CTAS, (nvec + scail::SC_THREADS - 1) / scail::SC_THREADS));
+    SCAIL_REQUIRE(partials_len >= 2 * ctas, "cfg_cache_delta_forecast: partials holds %lld floats, this size needs %d",
+                  (long long)partials_len, 2 * ctas);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    scail::cfg_cache_delta_forecast_kernel<<<ctas, scail::SC_THREADS, 0, st>>>(static_cast<const uint2*>(v), slots, slot_stride,
+                                                                               (int)write_slot, k, partials, nvec);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    scail::step_cache_finish_kernel<<<1, scail::SC_THREADS, 0, st>>>(partials, ctas, out);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_cfg_euler_cached_forecast(float* x, const void* c, const float* slots, int64_t slot_stride, int64_t n_slots,
+                                    const float* coef, int64_t n, float scale, float dsigma, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && c && slots && coef, "cfg_euler_cached_forecast: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(c) && aligned16(slots),
+                  "cfg_euler_cached_forecast: x, c and slots must be 16-byte aligned");
+    scail::DeltaForecast k;
+    if (int rc = delta_forecast_coef("cfg_euler_cached_forecast", slot_stride, n_slots, n, coef, &k)) return rc;
+    const int64_t nvec = n / 4;
+    scail::cfg_euler_cached_forecast_kernel<<<blocks_for(nvec, scail::CFGC_THREADS), scail::CFGC_THREADS, 0,
+                                              static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<float4*>(x), static_cast<const uint2*>(c), slots, slot_stride, k, nvec, scale, dsigma);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_unipc_step_cached_forecast(float* x, float* x_last, const void* c, const float* dslots, int64_t dslot_stride,
+                                     int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride, int64_t n_slots,
+                                     int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                                     scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && c && dslots && dcoef && slots && coef, "unipc_step_cached_forecast: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(c) && aligned16(dslots) && aligned16(slots),
+                  "unipc_step_cached_forecast: x, x_last, c, dslots and slots must be 16-byte aligned");
+    scail::UnipcCoef k;
+    if (int rc = unipc_coef("unipc_step_cached_forecast", slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
+    scail::DeltaForecast dk;
+    if (int rc = delta_forecast_coef("unipc_step_cached_forecast", dslot_stride, n_dslots, n, dcoef, &dk)) return rc;
+    const int64_t nvec = n / 4;
+    scail::unipc_step_kernel<true, true><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
+                                           static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(c), slots, slot_stride,
+        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, reinterpret_cast<const float4*>(dslots),
+        dslot_stride, dk);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

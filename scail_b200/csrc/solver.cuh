@@ -34,20 +34,50 @@ __device__ __forceinline__ void unipc_axpy(float (&acc)[4], float c, const float
     }
 }
 
+// The CFG cache's forecast of delta = c - u (scail_b200/cfg_cache.py, order >= 1): the host's fp32 coefficient of each of
+// up to DELTA_MAX_SLOTS fp32 slots of delta, slot s at `slots + s * slot_stride` floats.
+constexpr int DELTA_MAX_SLOTS = 3;
+struct DeltaForecast {
+    float c[DELTA_MAX_SLOTS];
+};
+
+// t = c0*S0, then t = t + c1*S1, then t = t + c2*S2 at vector i, each product and sum rounded on its own (no FMA).  A slot
+// whose coefficient is exactly 0 is neither read nor added, so stale or NaN slots cannot leak, and c = (1, 0, 0) gives S0
+// bit for bit; with no active slot t = 0.
+__device__ __forceinline__ void delta_forecast4(const float* slots, int64_t slot_stride, const DeltaForecast& k, int64_t i,
+                                                float (&t)[4]) {
+    bool first = true;
+#pragma unroll
+    for (int s = 0; s < DELTA_MAX_SLOTS; ++s) {
+        if (k.c[s] == 0.f) continue;
+        float S[4];
+        unipc_load(reinterpret_cast<const float4*>(slots + s * slot_stride), i, S);
+        unipc_axpy(t, k.c[s], S, first);
+        first = false;
+    }
+    if (first) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) t[j] = 0.f;
+    }
+}
+
 // In fixed order, per element: g = u + s*(c - u); m = x - sigma*g; y = a_x*x_last + a[k]*M_k (slot order) + a_m*m when
 // `correct`, else y = x; z = b_y*y + b[k]*M_k (slot order) + b_m*m.  Writes x = z, x_last = y and slot `write_slot` = m.
 // A slot whose a[k] and b[k] are both exactly 0 is not read, and a term with a zero slot coefficient is not added, so stale
 // or NaN slots cannot leak.  Every thread reads all it needs before it writes, so the write slot may be one it reads.
 // kCached = false: v is the bf16 CFG pair [2, nvec * 4] and `delta` is not read.  kCached = true (the CFG cache's
 // conditional-only step, scail_b200/cfg_cache.py): v is the conditional output alone [nvec * 4] and u = f32(c) - delta;
-// every instruction after that is shared.  `delta` is the last parameter, so the pair instantiation's parameters keep their
-// offsets.
-template <bool kCached>
+// every instruction after that is shared.  kForecast (with kCached; CFGCache(order >= 1)): delta is the forecast
+// delta_forecast4 of the slots at `delta` (stride delta_stride floats) with the coefficients dk, in place of one held
+// delta.  `delta`, delta_stride and dk are the last parameters, so the other parameters keep their offsets.
+template <bool kCached, bool kForecast = false>
 __global__ void __launch_bounds__(UNIPC_THREADS) unipc_step_kernel(float4* __restrict__ x, float4* __restrict__ x_last,
                                                                    const uint2* __restrict__ v, float* __restrict__ slots,
                                                                    int64_t slot_stride, int n_slots, int write_slot,
                                                                    int64_t nvec, float scale, float sigma, int correct,
-                                                                   UnipcCoef k, const float4* __restrict__ delta) {
+                                                                   UnipcCoef k, const float4* __restrict__ delta,
+                                                                   int64_t delta_stride, DeltaForecast dk) {
+    static_assert(kCached || !kForecast, "the forecast form is a cached step");
     const int64_t i = static_cast<int64_t>(blockIdx.x) * UNIPC_THREADS + threadIdx.x;
     if (i >= nvec) return;
     float fx[4], fu[4], fc[4], m[4], y[4], z[4];
@@ -55,7 +85,10 @@ __global__ void __launch_bounds__(UNIPC_THREADS) unipc_step_kernel(float4* __res
     if constexpr (kCached) {
         float fd[4];
         unipc_unpack4(v[i], fc);
-        unipc_load(delta, i, fd);
+        if constexpr (kForecast)
+            delta_forecast4(reinterpret_cast<const float*>(delta), delta_stride, dk, i, fd);
+        else
+            unipc_load(delta, i, fd);
 #pragma unroll
         for (int j = 0; j < 4; ++j) fu[j] = __fsub_rn(fc[j], fd[j]);
     } else {

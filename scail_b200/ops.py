@@ -619,6 +619,61 @@ def unipc_step_cached_(x, x_last, c, delta, slots, write_slot, scale, sigma, coe
     return x
 
 
+def _delta_forecast(slots, coef, n):
+    """The delta slots (fp32 [n_slots, n], contiguous) and their forecast coefficients (n_slots floats, padded with zeros to
+    the kernels' 3) -> (slot stride, n_slots, the ctypes float[3])."""
+    assert slots.dim() >= 2 and slots.is_contiguous() and slots[0].numel() == n, tuple(slots.shape)
+    assert len(coef) == slots.shape[0]
+    return slots.stride(0), slots.shape[0], (ctypes.c_float * 3)(*coef, *[0.0] * (3 - len(coef)))
+
+
+def cfg_cache_delta_forecast(v, slots, write_slot, coef, partials, out):
+    """cfg_cache_delta against a forecast: slots[write_slot] = f32(v[1]) - f32(v[0]) and out = (sum |d_new - t|, sum |t|,
+    their ratio, 0) with t = c0*S0, then t + c1*S1, then t + c2*S2 (each product and sum rounded on its own; a slot whose
+    coefficient is 0 is not read).  slots fp32 [n_slots, ...] with v[0]'s element count per slot, coef n_slots fp32 values.
+    Bit-reproducible.  Returns out."""
+    _req(v), _req(slots, torch.float32), _req(partials, torch.float32), _req(out, torch.float64)
+    n = v.numel() // 2
+    assert v.is_contiguous() and partials.is_contiguous() and out.is_contiguous() and out.numel() >= 4
+    stride, n_slots, k = _delta_forecast(slots, coef, n)
+    _lib.check(_lib.lib().scail_cfg_cache_delta_forecast(_ptr(v), _ptr(slots), stride, n_slots, int(write_slot),
+                                                         ctypes.addressof(k), _ptr(partials), partials.numel(), _ptr(out), n,
+                                                         _stream()), "scail_cfg_cache_delta_forecast")
+    _count(2)
+    return out
+
+
+def cfg_euler_cached_forecast_(x, c, slots, coef, scale, dsigma):
+    """cfg_euler_cached_ with delta = the forecast of the delta slots (as cfg_cache_delta_forecast forms it)."""
+    _req(x, torch.float32), _req(c), _req(slots, torch.float32)
+    assert x.is_contiguous() and c.is_contiguous() and c.numel() == x.numel()
+    stride, n_slots, k = _delta_forecast(slots, coef, x.numel())
+    _lib.check(_lib.lib().scail_cfg_euler_cached_forecast(_ptr(x), _ptr(c), _ptr(slots), stride, n_slots, ctypes.addressof(k),
+                                                          x.numel(), float(scale), float(dsigma), _stream()),
+               "scail_cfg_euler_cached_forecast")
+    _count()
+    return x
+
+
+def unipc_step_cached_forecast_(x, x_last, c, dslots, dcoef, slots, write_slot, scale, sigma, coef, correct):
+    """unipc_step_cached_ with delta = the forecast of the delta slots dslots with the coefficients dcoef (as
+    cfg_cache_delta_forecast forms it); everything else as unipc_step_.  Returns x."""
+    _req(x, torch.float32), _req(x_last, torch.float32), _req(c), _req(dslots, torch.float32), _req(slots, torch.float32)
+    assert x.is_contiguous() and x_last.is_contiguous() and x_last.shape == x.shape
+    assert c.is_contiguous() and c.numel() == x.numel()
+    assert slots.dim() == 2 and slots.is_contiguous() and slots.shape[1] == x.numel(), tuple(slots.shape)
+    assert len(coef) == 10
+    dstride, n_d, dk = _delta_forecast(dslots, dcoef, x.numel())
+    k = (ctypes.c_float * 10)(*coef)
+    _lib.check(_lib.lib().scail_unipc_step_cached_forecast(_ptr(x), _ptr(x_last), _ptr(c), _ptr(dslots), dstride, n_d,
+                                                           ctypes.addressof(dk), _ptr(slots), slots.stride(0), slots.shape[0],
+                                                           int(write_slot), x.numel(), float(scale), float(sigma),
+                                                           int(bool(correct)), ctypes.addressof(k), _stream()),
+               "scail_unipc_step_cached_forecast")
+    _count()
+    return x
+
+
 # ---------------------------------------------------------------- first-block residual cache (scail_b200.step_cache)
 STEP_CACHE_PARTIALS = 2048  # fp32 partial sums of step_cache_indicator: 2 per CTA, at most 1024 CTAs
 

@@ -54,14 +54,14 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     solver: an optional scail_b200.unipc.UniPC with a bound schedule; its step replaces the Euler update.  (sigma, next_sigma)
     must be the solver's next pair and x its latent, else ValueError before anything runs.
     cfg_cache: an optional scail_b200.cfg_cache.CFGCache (single GPU only).  It decides before the forward whether this step
-    runs the conditional branch alone (b = 1, on the cache's stream) and rebuilds u = c - delta for the update; the
-    first-block cache then sits the step out."""
+    runs the conditional branch alone (b = 1, on the cache's stream) and rebuilds u = c - delta for the update (delta
+    forecast at this step's sigma when the cache's order is >= 1); the first-block cache then sits the step out."""
     _check_cfg_cache(model, cfg_cache, plan, model_kwargs)
     if solver is not None:
         solver.check_step(x, sigma, next_sigma)
     if step_cache is not None:
         check_supported(plan=plan)
-    cond_only = cfg_cache is not None and cfg_cache.begin_step(x)
+    cond_only = cfg_cache is not None and cfg_cache.begin_step(x, sigma if _sigma_override is None else _sigma_override)
     if step_cache is not None and not cond_only:
         step_cache.set_sigma(sigma if _sigma_override is None else _sigma_override)
         model_kwargs["_step_cache"] = step_cache
@@ -73,9 +73,7 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     if cond_only:
         ts = torch.full((1,), c_noise, device=x.device, dtype=torch.float32)
         c = cfg_cache.cond_forward(model, x_in, ts, ctx[1:2], kw)
-        if solver is not None:
-            return solver.step(x, c, scale, sigma, next_sigma, delta=cfg_cache.delta)
-        return ops.cfg_euler_cached_(x, c, cfg_cache.delta, scale, float(next_sigma) - float(sigma))
+        return cfg_cache.cond_update(x, c, scale, sigma, next_sigma, solver)
     if plan is None:
         x2 = torch.cat([x_in, x_in], 0)
         ts = torch.full((2,), c_noise, device=x.device, dtype=torch.float32)
@@ -208,7 +206,8 @@ class GraphedStep:
     cfg_cache (a scail_b200.cfg_cache.CFGCache, reset at construction): the conditional-only forward (b = 1 on the cond
     row) is one more graph, captured on a stream of this object's own so that it has its own workspace; the host decides
     before each step which graphs replay.  Every graph's workspace tensors are held here (_workspace_of).  The delta kernel and the updates run eagerly after the replay (delta_ref and delta_new
-    alternate between two buffers, which a graph would fix)."""
+    alternate between two buffers, which a graph would fix; at order >= 1 the forecast coefficients are kernel arguments
+    computed from each step's sigma, so no graph depends on them either)."""
 
     def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None, solver=None, cfg_cache=None):
         _check_cfg_cache(model, cfg_cache)
@@ -308,11 +307,9 @@ class GraphedStep:
         self.kernels_in_graph = ops.LAUNCHES - n0
         self._ws = _workspace_of(side)
 
-    def _update(self, v, sigma, next_sigma, delta=None):
+    def _update(self, v, sigma, next_sigma):
         if self.solver is not None:
-            return self.solver.step(self.x, v, self.scale, sigma, next_sigma, delta=delta)
-        if delta is not None:
-            return ops.cfg_euler_cached_(self.x, v, delta, self.scale, float(next_sigma) - float(sigma))
+            return self.solver.step(self.x, v, self.scale, sigma, next_sigma)
         return ops.cfg_euler_(self.x, v, self.scale, float(next_sigma) - float(sigma))
 
     def __call__(self, sigma, next_sigma):
@@ -321,10 +318,10 @@ class GraphedStep:
         if self.fp8:
             self.adaln.prepare_fp8_weights()
         cc = self.cfg_cache
-        if cc is not None and cc.begin_step(self.x):
+        if cc is not None and cc.begin_step(self.x, sigma):
             self.ts1.fill_(float(sigma) * 1000.0)
             self.graph1.replay()
-            return self._update(self.v1, sigma, next_sigma, cc.delta)
+            return cc.cond_update(self.x, self.v1, self.scale, sigma, next_sigma, self.solver)
         v = self._full(sigma)
         if cc is not None:
             cc.full_step(v)

@@ -45,13 +45,13 @@ def check_threshold(threshold, what="step cache"):
     return t
 
 
-def check_order(order):
+def check_order(order, what="step cache"):
     """The degree of the forecast polynomial: an int in {0, 1, 2}.  Raises TypeError for bools and non-ints, ValueError for
-    other ints."""
+    other ints; the messages name `what`."""
     if isinstance(order, bool) or not isinstance(order, numbers.Integral):
-        raise TypeError(f"step cache order must be an int in {{0, 1, 2}}, got {order!r}")
+        raise TypeError(f"{what} order must be an int in {{0, 1, 2}}, got {order!r}")
     if not 0 <= int(order) <= 2:
-        raise ValueError(f"step cache order must be 0, 1 or 2, got {order!r}")
+        raise ValueError(f"{what} order must be 0, 1 or 2, got {order!r}")
     return int(order)
 
 
@@ -67,13 +67,14 @@ def check_max_skips(max_skips, what="step cache"):
     return int(max_skips)
 
 
-def check_sigma(sigma):
-    """The sampler's sigma of a step as a finite float (a Python number or a one-element tensor, as sampler_step takes it)."""
+def check_sigma(sigma, what="step cache"):
+    """The sampler's sigma of a step as a finite float (a Python number or a one-element tensor, as sampler_step takes it);
+    the messages name `what`."""
     if isinstance(sigma, bool):
-        raise TypeError(f"step cache sigma must be a real number, got {sigma!r}")
+        raise TypeError(f"{what} sigma must be a real number, got {sigma!r}")
     s = float(sigma)
     if not math.isfinite(s):
-        raise ValueError(f"step cache sigma must be finite, got {sigma!r}")
+        raise ValueError(f"{what} sigma must be finite, got {sigma!r}")
     return s
 
 
