@@ -261,6 +261,44 @@ int scail_unipc_step_cached_forecast(float* x, float* x_last, const void* c, con
                                      int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride, int64_t n_slots,
                                      int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
                                      scail_stream_t stream);
+/* CFG-Zero* guidance (scail_b200/guidance.py).  n fp32 elements (n % 4 == 0); every tensor pointer is 16-byte aligned
+ * except partials (4), out (8) and u_scale (4), a single fp32 value in device memory.
+ * scail_cfg_zero_scale: s* = <c, u> / (|u|^2 + 1e-8) over all n elements, with u and c by `form`:
+ *   0: v is the bf16 CFG pair [2, n]; delta, delta_stride, n_dslots and dcoef are not read;
+ *   1: v is c alone, bf16 [n], and u = f32(c) - delta, delta fp32 [n]; delta_stride, n_dslots and dcoef are not read;
+ *   2: v is c alone and u = f32(c) - t, t the forecast of the delta slots (delta, delta_stride, n_dslots, dcoef) as in
+ *      scail_cfg_euler_cached_forecast.
+ * u is formed as the update of the same form forms it.  fp32 partial sums of c*u and u*u per CTA over a fixed partition
+ * (each product and sum rounded on its own; partials: at least 2 * 1024 floats), then one CTA adds them in fp64 in a fixed
+ * order: out = {dot, norm, 0, 0} (fp64) and *u_scale = dot / (norm + 1e-8) in fp64, rounded once to fp32.
+ * Bit-reproducible; two launches.
+ * The scaled twins take one more argument, u_scale, and form u' = (*u_scale) * u (one rounded product) where their
+ * unscaled form uses u:
+ *   scail_cfg_euler_scaled: per element, each product and sum rounded on its own, u' = s*u; g = u' + scale*(c - u');
+ *     x = x + dsigma*g (v the pair [2, n]; x and v 16-byte aligned).  Not bit-equal to scail_cfg_euler at s = 1, whose
+ *     arithmetic the compiler may contract.
+ *   scail_cfg_euler_cached_scaled, scail_cfg_euler_cached_forecast_scaled, scail_unipc_step_scaled,
+ *   scail_unipc_step_cached_scaled, scail_unipc_step_cached_forecast_scaled: every other instruction and check as in the
+ *     unscaled entry point, so *u_scale == 1 gives its result bit for bit. */
+int scail_cfg_zero_scale(int form, const void* v, const float* delta, int64_t delta_stride, int64_t n_dslots, const float* dcoef,
+                         float* partials, int64_t partials_len, double* out, float* u_scale, int64_t n, scail_stream_t stream);
+int scail_cfg_euler_scaled(float* x, const void* v, int64_t n, float scale, float dsigma, const float* u_scale,
+                           scail_stream_t stream);
+int scail_cfg_euler_cached_scaled(float* x, const void* c, const float* delta, int64_t n, float scale, float dsigma,
+                                  const float* u_scale, scail_stream_t stream);
+int scail_cfg_euler_cached_forecast_scaled(float* x, const void* c, const float* slots, int64_t slot_stride, int64_t n_slots,
+                                           const float* coef, int64_t n, float scale, float dsigma, const float* u_scale,
+                                           scail_stream_t stream);
+int scail_unipc_step_scaled(float* x, float* x_last, const void* v, float* slots, int64_t slot_stride, int64_t n_slots,
+                            int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                            const float* u_scale, scail_stream_t stream);
+int scail_unipc_step_cached_scaled(float* x, float* x_last, const void* c, const float* delta, float* slots,
+                                   int64_t slot_stride, int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma,
+                                   int correct, const float* coef, const float* u_scale, scail_stream_t stream);
+int scail_unipc_step_cached_forecast_scaled(float* x, float* x_last, const void* c, const float* dslots, int64_t dslot_stride,
+                                            int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride,
+                                            int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma,
+                                            int correct, const float* coef, const float* u_scale, scail_stream_t stream);
 
 /* First-block residual cache (scail_b200/step_cache.py).  Token tensors are bf16 [B, N, d] (ref || noise || pose rows of
  * each batch element); the noise rows are rows [n_ref, n_ref + n_seq) of each element.  d % 8 == 0, B*N*d/8 < 2^31, and

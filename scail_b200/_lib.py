@@ -71,6 +71,14 @@ SIGNATURES = {
     "scail_cfg_euler_cached_forecast": [c_p, c_p, c_p, c_i64, c_i64, c_p, c_i64, c_f, c_f, c_p],
     "scail_unipc_step_cached_forecast": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f, c_f,
                                          c_int, c_p, c_p],
+    "scail_cfg_zero_scale": [c_int, c_p, c_p, c_i64, c_i64, c_p, c_p, c_i64, c_p, c_p, c_i64, c_p],
+    "scail_cfg_euler_scaled": [c_p, c_p, c_i64, c_f, c_f, c_p, c_p],
+    "scail_cfg_euler_cached_scaled": [c_p, c_p, c_p, c_i64, c_f, c_f, c_p, c_p],
+    "scail_cfg_euler_cached_forecast_scaled": [c_p, c_p, c_p, c_i64, c_i64, c_p, c_i64, c_f, c_f, c_p, c_p],
+    "scail_unipc_step_scaled": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f, c_f, c_int, c_p, c_p, c_p],
+    "scail_unipc_step_cached_scaled": [c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f, c_f, c_int, c_p, c_p, c_p],
+    "scail_unipc_step_cached_forecast_scaled": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f,
+                                                c_f, c_int, c_p, c_p, c_p],
     "scail_step_cache_indicator": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_update": [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_apply": [c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],

@@ -226,18 +226,22 @@ class CFGCache:
             b.n_full += 1
         self._pending = True
 
-    def cond_update(self, x, c, scale, sigma, next_sigma, solver=None):
+    def cond_update(self, x, c, scale, sigma, next_sigma, solver=None, guidance=None):
         """The conditional-only step's latent update in place on x from c, the conditional output alone (bf16 [1, ...]): u =
         f32(c) - delta (order 0) or f32(c) - delta_hat(sigma) (order >= 1), then the Euler step, or solver.step (a UniPC)
-        when given.  Returns x."""
+        when given.  With guidance (a scail_b200.guidance.CFGZeroStar), s* is reduced from that same u first and the
+        update is the scaled one.  Returns x."""
+        ds = float(next_sigma) - float(sigma)
         if self._order == 0:
+            kw = {} if guidance is None else dict(u_scale=guidance.scale(c, delta=self.delta))
             if solver is not None:
-                return solver.step(x, c, scale, sigma, next_sigma, delta=self.delta)
-            return ops.cfg_euler_cached_(x, c, self.delta, scale, float(next_sigma) - float(sigma))
+                return solver.step(x, c, scale, sigma, next_sigma, delta=self.delta, **kw)
+            return ops.cfg_euler_cached_(x, c, self.delta, scale, ds, **kw)
         fc = (self.buffers.slots, self.forecast())
+        kw = {} if guidance is None else dict(u_scale=guidance.scale(c, forecast=fc))
         if solver is not None:
-            return solver.step(x, c, scale, sigma, next_sigma, forecast=fc)
-        return ops.cfg_euler_cached_forecast_(x, c, *fc, scale, float(next_sigma) - float(sigma))
+            return solver.step(x, c, scale, sigma, next_sigma, forecast=fc, **kw)
+        return ops.cfg_euler_cached_forecast_(x, c, *fc, scale, ds, **kw)
 
     def stream(self, device):
         """This cache's stream for the conditional-only forward on `device`, created on first use.  Should the caller come

@@ -17,6 +17,7 @@
 #include "adaptive.cuh"
 #include "attention.cuh"
 #include "cfg_cache.cuh"
+#include "cfg_zero.cuh"
 #include "conv.cuh"
 #include "gemm.cuh"
 #include "rowops.cuh"
@@ -844,41 +845,6 @@ static int unipc_coef(const char* what, int64_t slot_stride, int64_t n_slots, in
     return 0;
 }
 
-int scail_unipc_step(float* x, float* x_last, const void* v, float* slots, int64_t slot_stride, int64_t n_slots,
-                     int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
-                     scail_stream_t stream) {
-    SCAIL_REQUIRE(x && x_last && v && slots && coef, "unipc_step: null operand");
-    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(v) && aligned16(slots),
-                  "unipc_step: x, x_last, v and slots must be 16-byte aligned");
-    scail::UnipcCoef k;
-    if (int rc = unipc_coef("unipc_step", slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
-    const int64_t nvec = n / 4;
-    scail::unipc_step_kernel<false><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
-                                      static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(v), slots, slot_stride,
-        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, nullptr, 0, scail::DeltaForecast{});
-    SCAIL_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-int scail_unipc_step_cached(float* x, float* x_last, const void* c, const float* delta, float* slots, int64_t slot_stride,
-                            int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma, int correct,
-                            const float* coef, scail_stream_t stream) {
-    SCAIL_REQUIRE(x && x_last && c && delta && slots && coef, "unipc_step_cached: null operand");
-    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(c) && aligned16(delta) && aligned16(slots),
-                  "unipc_step_cached: x, x_last, c, delta and slots must be 16-byte aligned");
-    scail::UnipcCoef k;
-    if (int rc = unipc_coef("unipc_step_cached", slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
-    const int64_t nvec = n / 4;
-    scail::unipc_step_kernel<true><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
-                                     static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(c), slots, slot_stride,
-        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, reinterpret_cast<const float4*>(delta), 0,
-        scail::DeltaForecast{});
-    SCAIL_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
 // Checks shared by the forecast entry points of the CFG cache's delta slots; fills k.  Returns 0 or the fail() code.
 static int delta_forecast_coef(const char* what, int64_t slot_stride, int64_t n_slots, int64_t n, const float* coef,
                                scail::DeltaForecast* k) {
@@ -893,6 +859,93 @@ static int delta_forecast_coef(const char* what, int64_t slot_stride, int64_t n_
                       what, s, (long long)n_slots);
     }
     return 0;
+}
+
+// The u_scale check of every scaled entry point (CFG-Zero*): a non-null, 4-byte aligned device scalar.
+static int check_u_scale(const char* what, const float* u_scale) {
+    SCAIL_REQUIRE(u_scale, "%s: null u_scale", what);
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(u_scale) & 3) == 0, "%s: u_scale must be 4-byte aligned", what);
+    return 0;
+}
+
+// The three UniPC step forms, unscaled (u_scale == nullptr) or scaled.  cached: c alone with delta (one fp32 tensor, or
+// with dcoef the forecast of n_dslots slots at stride dslot_stride); else v is the pair and delta is not read.
+static int unipc_launch(const char* what, float* x, float* x_last, const void* v, bool cached, const float* delta,
+                        int64_t dslot_stride, int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride,
+                        int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                        const float* u_scale, cudaStream_t st) {
+    scail::UnipcCoef k;
+    if (int rc = unipc_coef(what, slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
+    scail::DeltaForecast dk{};
+    if (dcoef)
+        if (int rc = delta_forecast_coef(what, dslot_stride, n_dslots, n, dcoef, &dk)) return rc;
+    const int64_t nvec = n / 4;
+    const int grid = static_cast<int>(blocks_for(nvec, scail::UNIPC_THREADS));
+    float4* x4 = reinterpret_cast<float4*>(x);
+    float4* xl4 = reinterpret_cast<float4*>(x_last);
+    const uint2* v2 = static_cast<const uint2*>(v);
+    const float4* d4 = reinterpret_cast<const float4*>(delta);
+    const int64_t ds = dcoef ? dslot_stride : 0;
+    const int corr = correct ? 1 : 0;
+#define SCAIL_UNIPC_LAUNCH(...)                                                                                          \
+    scail::unipc_step_kernel<__VA_ARGS__><<<grid, scail::UNIPC_THREADS, 0, st>>>(x4, xl4, v2, slots, slot_stride,      \
+                                                                                 (int)n_slots, (int)write_slot, nvec,  \
+                                                                                 scale, sigma, corr, k, d4, ds, dk, u_scale)
+    if (!cached)
+        u_scale ? SCAIL_UNIPC_LAUNCH(false, false, true) : SCAIL_UNIPC_LAUNCH(false);
+    else if (!dcoef)
+        u_scale ? SCAIL_UNIPC_LAUNCH(true, false, true) : SCAIL_UNIPC_LAUNCH(true);
+    else
+        u_scale ? SCAIL_UNIPC_LAUNCH(true, true, true) : SCAIL_UNIPC_LAUNCH(true, true);
+#undef SCAIL_UNIPC_LAUNCH
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_unipc_step(float* x, float* x_last, const void* v, float* slots, int64_t slot_stride, int64_t n_slots,
+                     int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                     scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && v && slots && coef, "unipc_step: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(v) && aligned16(slots),
+                  "unipc_step: x, x_last, v and slots must be 16-byte aligned");
+    return unipc_launch("unipc_step", x, x_last, v, false, nullptr, 0, 0, nullptr, slots, slot_stride, n_slots, write_slot, n,
+                        scale, sigma, correct, coef, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int scail_unipc_step_scaled(float* x, float* x_last, const void* v, float* slots, int64_t slot_stride, int64_t n_slots,
+                            int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
+                            const float* u_scale, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && v && slots && coef, "unipc_step_scaled: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(v) && aligned16(slots),
+                  "unipc_step_scaled: x, x_last, v and slots must be 16-byte aligned");
+    if (int rc = check_u_scale("unipc_step_scaled", u_scale)) return rc;
+    return unipc_launch("unipc_step_scaled", x, x_last, v, false, nullptr, 0, 0, nullptr, slots, slot_stride, n_slots,
+                        write_slot, n, scale, sigma, correct, coef, u_scale, static_cast<cudaStream_t>(stream));
+}
+
+static int unipc_cached(const char* what, float* x, float* x_last, const void* c, const float* delta, float* slots,
+                        int64_t slot_stride, int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma,
+                        int correct, const float* coef, const float* u_scale, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && c && delta && slots && coef, "%s: null operand", what);
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(c) && aligned16(delta) && aligned16(slots),
+                  "%s: x, x_last, c, delta and slots must be 16-byte aligned", what);
+    return unipc_launch(what, x, x_last, c, true, delta, 0, 0, nullptr, slots, slot_stride, n_slots, write_slot, n, scale,
+                        sigma, correct, coef, u_scale, static_cast<cudaStream_t>(stream));
+}
+
+int scail_unipc_step_cached(float* x, float* x_last, const void* c, const float* delta, float* slots, int64_t slot_stride,
+                            int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma, int correct,
+                            const float* coef, scail_stream_t stream) {
+    return unipc_cached("unipc_step_cached", x, x_last, c, delta, slots, slot_stride, n_slots, write_slot, n, scale, sigma,
+                        correct, coef, nullptr, stream);
+}
+
+int scail_unipc_step_cached_scaled(float* x, float* x_last, const void* c, const float* delta, float* slots,
+                                   int64_t slot_stride, int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma,
+                                   int correct, const float* coef, const float* u_scale, scail_stream_t stream) {
+    if (int rc = check_u_scale("unipc_step_cached_scaled", u_scale)) return rc;
+    return unipc_cached("unipc_step_cached_scaled", x, x_last, c, delta, slots, slot_stride, n_slots, write_slot, n, scale,
+                        sigma, correct, coef, u_scale, stream);
 }
 
 int scail_cfg_cache_delta_forecast(const void* v, float* slots, int64_t slot_stride, int64_t n_slots, int64_t write_slot,
@@ -920,40 +973,68 @@ int scail_cfg_cache_delta_forecast(const void* v, float* slots, int64_t slot_str
     return 0;
 }
 
-int scail_cfg_euler_cached_forecast(float* x, const void* c, const float* slots, int64_t slot_stride, int64_t n_slots,
-                                    const float* coef, int64_t n, float scale, float dsigma, scail_stream_t stream) {
-    SCAIL_REQUIRE(x && c && slots && coef, "cfg_euler_cached_forecast: null operand");
-    SCAIL_REQUIRE(aligned16(x) && aligned16(c) && aligned16(slots),
-                  "cfg_euler_cached_forecast: x, c and slots must be 16-byte aligned");
+static int cfg_euler_cached_forecast(const char* what, float* x, const void* c, const float* slots, int64_t slot_stride,
+                                     int64_t n_slots, const float* coef, int64_t n, float scale, float dsigma,
+                                     const float* u_scale, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && c && slots && coef, "%s: null operand", what);
+    SCAIL_REQUIRE(aligned16(x) && aligned16(c) && aligned16(slots), "%s: x, c and slots must be 16-byte aligned", what);
     scail::DeltaForecast k;
-    if (int rc = delta_forecast_coef("cfg_euler_cached_forecast", slot_stride, n_slots, n, coef, &k)) return rc;
+    if (int rc = delta_forecast_coef(what, slot_stride, n_slots, n, coef, &k)) return rc;
     const int64_t nvec = n / 4;
-    scail::cfg_euler_cached_forecast_kernel<<<blocks_for(nvec, scail::CFGC_THREADS), scail::CFGC_THREADS, 0,
-                                              static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(x), static_cast<const uint2*>(c), slots, slot_stride, k, nvec, scale, dsigma);
+    const int grid = static_cast<int>(blocks_for(nvec, scail::CFGC_THREADS));
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float4* x4 = reinterpret_cast<float4*>(x);
+    const uint2* c2 = static_cast<const uint2*>(c);
+    if (u_scale)
+        scail::cfg_euler_cached_forecast_kernel<true><<<grid, scail::CFGC_THREADS, 0, st>>>(x4, c2, slots, slot_stride, k, nvec,
+                                                                                           scale, dsigma, u_scale);
+    else
+        scail::cfg_euler_cached_forecast_kernel<false><<<grid, scail::CFGC_THREADS, 0, st>>>(x4, c2, slots, slot_stride, k, nvec,
+                                                                                            scale, dsigma, nullptr);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int scail_cfg_euler_cached_forecast(float* x, const void* c, const float* slots, int64_t slot_stride, int64_t n_slots,
+                                    const float* coef, int64_t n, float scale, float dsigma, scail_stream_t stream) {
+    return cfg_euler_cached_forecast("cfg_euler_cached_forecast", x, c, slots, slot_stride, n_slots, coef, n, scale, dsigma,
+                                     nullptr, stream);
+}
+
+int scail_cfg_euler_cached_forecast_scaled(float* x, const void* c, const float* slots, int64_t slot_stride, int64_t n_slots,
+                                           const float* coef, int64_t n, float scale, float dsigma, const float* u_scale,
+                                           scail_stream_t stream) {
+    if (int rc = check_u_scale("cfg_euler_cached_forecast_scaled", u_scale)) return rc;
+    return cfg_euler_cached_forecast("cfg_euler_cached_forecast_scaled", x, c, slots, slot_stride, n_slots, coef, n, scale,
+                                     dsigma, u_scale, stream);
+}
+
+static int unipc_cached_forecast(const char* what, float* x, float* x_last, const void* c, const float* dslots,
+                                 int64_t dslot_stride, int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride,
+                                 int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma, int correct,
+                                 const float* coef, const float* u_scale, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && c && dslots && dcoef && slots && coef, "%s: null operand", what);
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(c) && aligned16(dslots) && aligned16(slots),
+                  "%s: x, x_last, c, dslots and slots must be 16-byte aligned", what);
+    return unipc_launch(what, x, x_last, c, true, dslots, dslot_stride, n_dslots, dcoef, slots, slot_stride, n_slots, write_slot,
+                        n, scale, sigma, correct, coef, u_scale, static_cast<cudaStream_t>(stream));
 }
 
 int scail_unipc_step_cached_forecast(float* x, float* x_last, const void* c, const float* dslots, int64_t dslot_stride,
                                      int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride, int64_t n_slots,
                                      int64_t write_slot, int64_t n, float scale, float sigma, int correct, const float* coef,
                                      scail_stream_t stream) {
-    SCAIL_REQUIRE(x && x_last && c && dslots && dcoef && slots && coef, "unipc_step_cached_forecast: null operand");
-    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(c) && aligned16(dslots) && aligned16(slots),
-                  "unipc_step_cached_forecast: x, x_last, c, dslots and slots must be 16-byte aligned");
-    scail::UnipcCoef k;
-    if (int rc = unipc_coef("unipc_step_cached_forecast", slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
-    scail::DeltaForecast dk;
-    if (int rc = delta_forecast_coef("unipc_step_cached_forecast", dslot_stride, n_dslots, n, dcoef, &dk)) return rc;
-    const int64_t nvec = n / 4;
-    scail::unipc_step_kernel<true, true><<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0,
-                                           static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), static_cast<const uint2*>(c), slots, slot_stride,
-        (int)n_slots, (int)write_slot, nvec, scale, sigma, correct ? 1 : 0, k, reinterpret_cast<const float4*>(dslots),
-        dslot_stride, dk);
-    SCAIL_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return unipc_cached_forecast("unipc_step_cached_forecast", x, x_last, c, dslots, dslot_stride, n_dslots, dcoef, slots,
+                                 slot_stride, n_slots, write_slot, n, scale, sigma, correct, coef, nullptr, stream);
+}
+
+int scail_unipc_step_cached_forecast_scaled(float* x, float* x_last, const void* c, const float* dslots, int64_t dslot_stride,
+                                            int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride,
+                                            int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma,
+                                            int correct, const float* coef, const float* u_scale, scail_stream_t stream) {
+    if (int rc = check_u_scale("unipc_step_cached_forecast_scaled", u_scale)) return rc;
+    return unipc_cached_forecast("unipc_step_cached_forecast_scaled", x, x_last, c, dslots, dslot_stride, n_dslots, dcoef,
+                                 slots, slot_stride, n_slots, write_slot, n, scale, sigma, correct, coef, u_scale, stream);
 }
 
 int scail_cfg_cache_delta(const void* v, const float* d_ref, float* d_new, float* partials, int64_t partials_len, double* out,
@@ -977,15 +1058,82 @@ int scail_cfg_cache_delta(const void* v, const float* d_ref, float* d_new, float
     return 0;
 }
 
+static int cfg_euler_cached(const char* what, float* x, const void* c, const float* delta, int64_t n, float scale,
+                            float dsigma, const float* u_scale, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && c && delta, "%s: null operand", what);
+    SCAIL_REQUIRE(aligned16(x) && aligned16(c) && aligned16(delta), "%s: x, c and delta must be 16-byte aligned", what);
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "%s: need n a positive multiple of 4 (got n=%lld)", what, (long long)n);
+    const int64_t nvec = n / 4;
+    const int grid = static_cast<int>(blocks_for(nvec, scail::CFGC_THREADS));
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float4* x4 = reinterpret_cast<float4*>(x);
+    const uint2* c2 = static_cast<const uint2*>(c);
+    const float4* d4 = reinterpret_cast<const float4*>(delta);
+    if (u_scale)
+        scail::cfg_euler_cached_kernel<true><<<grid, scail::CFGC_THREADS, 0, st>>>(x4, c2, d4, nvec, scale, dsigma, u_scale);
+    else
+        scail::cfg_euler_cached_kernel<false><<<grid, scail::CFGC_THREADS, 0, st>>>(x4, c2, d4, nvec, scale, dsigma, nullptr);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 int scail_cfg_euler_cached(float* x, const void* c, const float* delta, int64_t n, float scale, float dsigma,
                            scail_stream_t stream) {
-    SCAIL_REQUIRE(x && c && delta, "cfg_euler_cached: null operand");
-    SCAIL_REQUIRE(aligned16(x) && aligned16(c) && aligned16(delta), "cfg_euler_cached: x, c and delta must be 16-byte aligned");
-    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "cfg_euler_cached: need n a positive multiple of 4 (got n=%lld)", (long long)n);
+    return cfg_euler_cached("cfg_euler_cached", x, c, delta, n, scale, dsigma, nullptr, stream);
+}
+
+int scail_cfg_euler_cached_scaled(float* x, const void* c, const float* delta, int64_t n, float scale, float dsigma,
+                                  const float* u_scale, scail_stream_t stream) {
+    if (int rc = check_u_scale("cfg_euler_cached_scaled", u_scale)) return rc;
+    return cfg_euler_cached("cfg_euler_cached_scaled", x, c, delta, n, scale, dsigma, u_scale, stream);
+}
+
+int scail_cfg_euler_scaled(float* x, const void* v, int64_t n, float scale, float dsigma, const float* u_scale,
+                           scail_stream_t stream) {
+    SCAIL_REQUIRE(x && v, "cfg_euler_scaled: null operand");
+    if (int rc = check_u_scale("cfg_euler_scaled", u_scale)) return rc;
+    SCAIL_REQUIRE(aligned16(x) && aligned16(v), "cfg_euler_scaled: x and v must be 16-byte aligned");
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "cfg_euler_scaled: need n a positive multiple of 4 (got n=%lld)", (long long)n);
     const int64_t nvec = n / 4;
-    scail::cfg_euler_cached_kernel<<<blocks_for(nvec, scail::CFGC_THREADS), scail::CFGC_THREADS, 0,
-                                     static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(x), static_cast<const uint2*>(c), reinterpret_cast<const float4*>(delta), nvec, scale, dsigma);
+    scail::cfg_euler_scaled_kernel<<<blocks_for(nvec, scail::CFGC_THREADS), scail::CFGC_THREADS, 0,
+                                     static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<float4*>(x),
+                                                                          static_cast<const uint2*>(v), nvec, scale, dsigma,
+                                                                          u_scale);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_cfg_zero_scale(int form, const void* v, const float* delta, int64_t delta_stride, int64_t n_dslots, const float* dcoef,
+                         float* partials, int64_t partials_len, double* out, float* u_scale, int64_t n, scail_stream_t stream) {
+    SCAIL_REQUIRE(form >= scail::CFGZ_PAIR && form <= scail::CFGZ_FORECAST,
+                  "cfg_zero_scale: form = %d must be 0 (pair), 1 (cached) or 2 (forecast)", form);
+    SCAIL_REQUIRE(v && partials && out && u_scale, "cfg_zero_scale: null operand");
+    SCAIL_REQUIRE(form == scail::CFGZ_PAIR || delta, "cfg_zero_scale: null delta with form %d", form);
+    SCAIL_REQUIRE(form != scail::CFGZ_FORECAST || dcoef, "cfg_zero_scale: null dcoef with form 2");
+    SCAIL_REQUIRE(aligned16(v) && (form == scail::CFGZ_PAIR || aligned16(delta)),
+                  "cfg_zero_scale: v and delta must be 16-byte aligned");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0 &&
+                      (reinterpret_cast<uintptr_t>(u_scale) & 3) == 0,
+                  "cfg_zero_scale: partials and u_scale must be 4-byte and out 8-byte aligned");
+    SCAIL_REQUIRE(n >= 4 && n % 4 == 0, "cfg_zero_scale: need n a positive multiple of 4 (got n=%lld)", (long long)n);
+    scail::DeltaForecast dk{};
+    if (form == scail::CFGZ_FORECAST)
+        if (int rc = delta_forecast_coef("cfg_zero_scale", delta_stride, n_dslots, n, dcoef, &dk)) return rc;
+    const int64_t nvec = n / 4;
+    const int ctas = static_cast<int>(std::min<int64_t>(scail::SC_MAX_CTAS, (nvec + scail::SC_THREADS - 1) / scail::SC_THREADS));
+    SCAIL_REQUIRE(partials_len >= 2 * ctas, "cfg_zero_scale: partials holds %lld floats, this size needs %d",
+                  (long long)partials_len, 2 * ctas);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const uint2* v2 = static_cast<const uint2*>(v);
+    const int64_t ds = form == scail::CFGZ_FORECAST ? delta_stride : 0;
+    if (form == scail::CFGZ_PAIR)
+        scail::cfg_zero_dot_kernel<scail::CFGZ_PAIR><<<ctas, scail::SC_THREADS, 0, st>>>(v2, nullptr, 0, dk, partials, nvec);
+    else if (form == scail::CFGZ_CACHED)
+        scail::cfg_zero_dot_kernel<scail::CFGZ_CACHED><<<ctas, scail::SC_THREADS, 0, st>>>(v2, delta, 0, dk, partials, nvec);
+    else
+        scail::cfg_zero_dot_kernel<scail::CFGZ_FORECAST><<<ctas, scail::SC_THREADS, 0, st>>>(v2, delta, ds, dk, partials, nvec);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    scail::cfg_zero_finish_kernel<<<1, scail::SC_THREADS, 0, st>>>(partials, ctas, out, u_scale);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

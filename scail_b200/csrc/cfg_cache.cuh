@@ -6,7 +6,7 @@
 #include <cuda_bf16.h>
 
 #include "solver.cuh"      // unipc_unpack4, unipc_load, DeltaForecast, delta_forecast4
-#include "step_cache.cuh"  // SC_THREADS, SC_MAX_CTAS, step_cache_finish_kernel, warp_sum
+#include "step_cache.cuh"  // SC_THREADS, SC_MAX_CTAS, sc_write_partials, step_cache_finish_kernel
 
 namespace scail {
 
@@ -34,40 +34,29 @@ __global__ void __launch_bounds__(SC_THREADS) cfg_cache_delta_kernel(const uint2
         }
         d_new[i] = make_float4(fd[0], fd[1], fd[2], fd[3]);
     }
-    __shared__ float red[2][SC_THREADS / 32];
-    s_diff = warp_sum(s_diff);
-    s_ref = warp_sum(s_ref);
-    if ((threadIdx.x & 31) == 0) {
-        red[0][threadIdx.x >> 5] = s_diff;
-        red[1][threadIdx.x >> 5] = s_ref;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float a = 0.f, b = 0.f;
-#pragma unroll
-        for (int w = 0; w < SC_THREADS / 32; ++w) {
-            a += red[0][w];
-            b += red[1][w];
-        }
-        partials[blockIdx.x] = a;
-        partials[gridDim.x + blockIdx.x] = b;
-    }
+    sc_write_partials(s_diff, s_ref, partials);
 }
 
 // The conditional-only Euler step, per element in this order, each product and sum rounded on its own (no FMA):
 // u = c - delta; g = u + scale*(c - u); x = x + dsigma*g.  c is the conditional output alone (bf16 [nvec * 4]).
+// kScaled (CFG-Zero*, scail_b200/guidance.py): u = (*u_scale) * u, one rounded product, right after u is formed; with
+// *u_scale == 1 the step is the unscaled one bit for bit.  u_scale is not read otherwise.
+template <bool kScaled = false>
 __global__ void __launch_bounds__(CFGC_THREADS) cfg_euler_cached_kernel(float4* __restrict__ x, const uint2* __restrict__ c,
                                                                         const float4* __restrict__ delta, int64_t nvec,
-                                                                        float scale, float dsigma) {
+                                                                        float scale, float dsigma,
+                                                                        const float* __restrict__ u_scale) {
     const int64_t i = static_cast<int64_t>(blockIdx.x) * CFGC_THREADS + threadIdx.x;
     if (i >= nvec) return;
     float fx[4], fc[4], fd[4];
     unipc_load(x, i, fx);
     unipc_unpack4(c[i], fc);
     unipc_load(delta, i, fd);
+    const float su = kScaled ? *u_scale : 1.f;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-        const float u = __fsub_rn(fc[j], fd[j]);
+        float u = __fsub_rn(fc[j], fd[j]);
+        if constexpr (kScaled) u = __fmul_rn(su, u);
         const float g = __fadd_rn(u, __fmul_rn(scale, __fsub_rn(fc[j], u)));
         fx[j] = __fadd_rn(fx[j], __fmul_rn(dsigma, g));
     }
@@ -101,41 +90,28 @@ __global__ void __launch_bounds__(SC_THREADS) cfg_cache_delta_forecast_kernel(co
         }
         d_new[i] = make_float4(fd[0], fd[1], fd[2], fd[3]);
     }
-    __shared__ float red[2][SC_THREADS / 32];
-    s_diff = warp_sum(s_diff);
-    s_ref = warp_sum(s_ref);
-    if ((threadIdx.x & 31) == 0) {
-        red[0][threadIdx.x >> 5] = s_diff;
-        red[1][threadIdx.x >> 5] = s_ref;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float a = 0.f, b = 0.f;
-#pragma unroll
-        for (int w = 0; w < SC_THREADS / 32; ++w) {
-            a += red[0][w];
-            b += red[1][w];
-        }
-        partials[blockIdx.x] = a;
-        partials[gridDim.x + blockIdx.x] = b;
-    }
+    sc_write_partials(s_diff, s_ref, partials);
 }
 
 // cfg_euler_cached_kernel with delta = delta_forecast4(k): with c = (1, 0, 0) it is cfg_euler_cached_kernel bit for bit.
+template <bool kScaled = false>
 __global__ void __launch_bounds__(CFGC_THREADS) cfg_euler_cached_forecast_kernel(float4* __restrict__ x,
                                                                                  const uint2* __restrict__ c,
                                                                                  const float* __restrict__ slots,
                                                                                  int64_t slot_stride, DeltaForecast k,
-                                                                                 int64_t nvec, float scale, float dsigma) {
+                                                                                 int64_t nvec, float scale, float dsigma,
+                                                                                 const float* __restrict__ u_scale) {
     const int64_t i = static_cast<int64_t>(blockIdx.x) * CFGC_THREADS + threadIdx.x;
     if (i >= nvec) return;
     float fx[4], fc[4], fd[4];
     unipc_load(x, i, fx);
     unipc_unpack4(c[i], fc);
     delta_forecast4(slots, slot_stride, k, i, fd);
+    const float su = kScaled ? *u_scale : 1.f;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-        const float u = __fsub_rn(fc[j], fd[j]);
+        float u = __fsub_rn(fc[j], fd[j]);
+        if constexpr (kScaled) u = __fmul_rn(su, u);
         const float g = __fadd_rn(u, __fmul_rn(scale, __fsub_rn(fc[j], u)));
         fx[j] = __fadd_rn(fx[j], __fmul_rn(dsigma, g));
     }

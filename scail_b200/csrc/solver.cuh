@@ -70,13 +70,16 @@ __device__ __forceinline__ void delta_forecast4(const float* slots, int64_t slot
 // every instruction after that is shared.  kForecast (with kCached; CFGCache(order >= 1)): delta is the forecast
 // delta_forecast4 of the slots at `delta` (stride delta_stride floats) with the coefficients dk, in place of one held
 // delta.  `delta`, delta_stride and dk are the last parameters, so the other parameters keep their offsets.
-template <bool kCached, bool kForecast = false>
+// kScaled (CFG-Zero*, scail_b200/guidance.py): u = (*u_scale) * u, one rounded product, once u is formed; the rest is
+// unchanged, so *u_scale == 1 gives the unscaled step bit for bit.  u_scale is the last parameter and is not read otherwise.
+template <bool kCached, bool kForecast = false, bool kScaled = false>
 __global__ void __launch_bounds__(UNIPC_THREADS) unipc_step_kernel(float4* __restrict__ x, float4* __restrict__ x_last,
                                                                    const uint2* __restrict__ v, float* __restrict__ slots,
                                                                    int64_t slot_stride, int n_slots, int write_slot,
                                                                    int64_t nvec, float scale, float sigma, int correct,
                                                                    UnipcCoef k, const float4* __restrict__ delta,
-                                                                   int64_t delta_stride, DeltaForecast dk) {
+                                                                   int64_t delta_stride, DeltaForecast dk,
+                                                                   const float* __restrict__ u_scale) {
     static_assert(kCached || !kForecast, "the forecast form is a cached step");
     const int64_t i = static_cast<int64_t>(blockIdx.x) * UNIPC_THREADS + threadIdx.x;
     if (i >= nvec) return;
@@ -94,6 +97,11 @@ __global__ void __launch_bounds__(UNIPC_THREADS) unipc_step_kernel(float4* __res
     } else {
         unipc_unpack4(v[i], fu);
         unipc_unpack4(v[nvec + i], fc);
+    }
+    if constexpr (kScaled) {
+        const float su = *u_scale;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) fu[j] = __fmul_rn(su, fu[j]);
     }
     float M[UNIPC_MAX_SLOTS][4];
 #pragma unroll

@@ -37,6 +37,29 @@ __device__ __forceinline__ int64_t sc_noise_to_full(unsigned v, unsigned vpr, un
     return (static_cast<int64_t>(b) * N + n_ref + n) * vpr + c;
 }
 
+// Pass 1's CTA epilogue: this thread's fp32 sums a and b, summed over the CTA in a fixed order (warp shuffle tree, then
+// the warps in index order) -> partials[blockIdx.x] and partials[gridDim.x + blockIdx.x].  Every thread of the CTA calls it.
+__device__ __forceinline__ void sc_write_partials(float s_a, float s_b, float* __restrict__ partials) {
+    __shared__ float red[2][SC_THREADS / 32];
+    s_a = warp_sum(s_a);
+    s_b = warp_sum(s_b);
+    if ((threadIdx.x & 31) == 0) {
+        red[0][threadIdx.x >> 5] = s_a;
+        red[1][threadIdx.x >> 5] = s_b;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float a = 0.f, b = 0.f;
+#pragma unroll
+        for (int w = 0; w < SC_THREADS / 32; ++w) {
+            a += red[0][w];
+            b += red[1][w];
+        }
+        partials[blockIdx.x] = a;
+        partials[gridDim.x + blockIdx.x] = b;
+    }
+}
+
 // Pass 1 of the indicator.  r = bf16_rn(f32(h1) - f32(h0)) -> r_new; h1's noise rows -> h1c; this CTA's fp32 partial sums
 // of |r - r_ref| and |r_ref| -> partials[blockIdx.x] and partials[gridDim.x + blockIdx.x].  The grid is a function of the
 // shape only and every thread walks the same grid-stride vectors in the same order, so the partials do not depend on the
@@ -67,31 +90,12 @@ __global__ void __launch_bounds__(SC_THREADS) step_cache_indicator_kernel(
         if (n >= 0 && n < n_seq)
             h1c[(static_cast<int64_t>(bb) * n_seq + n) * vpr + (static_cast<unsigned>(v) - row * vpr)] = b;
     }
-    __shared__ float red[2][SC_THREADS / 32];
-    s_diff = warp_sum(s_diff);
-    s_ref = warp_sum(s_ref);
-    if ((threadIdx.x & 31) == 0) {
-        red[0][threadIdx.x >> 5] = s_diff;
-        red[1][threadIdx.x >> 5] = s_ref;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float a = 0.f, b = 0.f;
-#pragma unroll
-        for (int w = 0; w < SC_THREADS / 32; ++w) {
-            a += red[0][w];
-            b += red[1][w];
-        }
-        partials[blockIdx.x] = a;
-        partials[gridDim.x + blockIdx.x] = b;
-    }
+    sc_write_partials(s_diff, s_ref, partials);
 }
 
-// Pass 2: one CTA sums the n_parts partials in fp64 in a fixed order -> out = {sum|r - r_ref|, sum|r_ref|, ratio, 0}; the
-// ratio is +inf when the denominator is zero (and NaN propagates).
-__global__ void __launch_bounds__(SC_THREADS) step_cache_finish_kernel(const float* __restrict__ partials, int n_parts,
-                                                                       double* __restrict__ out) {
-    __shared__ double red[2][SC_THREADS];
+// The two fp64 sums of n_parts partial pairs (partials[i] and partials[n_parts + i]) by one CTA of SC_THREADS threads, in a
+// fixed order; thread 0 gets them in red[0][0] and red[1][0].  Shared by every pass 2 of a two-pass reduction.
+__device__ __forceinline__ void sc_sum_partials(const float* __restrict__ partials, int n_parts, double (&red)[2][SC_THREADS]) {
     double a = 0.0, b = 0.0;
     for (int i = threadIdx.x; i < n_parts; i += SC_THREADS) {
         a += static_cast<double>(partials[i]);
@@ -107,6 +111,14 @@ __global__ void __launch_bounds__(SC_THREADS) step_cache_finish_kernel(const flo
         }
         __syncthreads();
     }
+}
+
+// Pass 2: one CTA sums the n_parts partials in fp64 in a fixed order -> out = {sum|r - r_ref|, sum|r_ref|, ratio, 0}; the
+// ratio is +inf when the denominator is zero (and NaN propagates).
+__global__ void __launch_bounds__(SC_THREADS) step_cache_finish_kernel(const float* __restrict__ partials, int n_parts,
+                                                                       double* __restrict__ out) {
+    __shared__ double red[2][SC_THREADS];
+    sc_sum_partials(partials, n_parts, red);
     if (threadIdx.x == 0) {
         const double num = red[0][0], den = red[1][0];
         out[0] = num;

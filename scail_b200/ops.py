@@ -547,30 +547,49 @@ def unpatchify(lin, B, T, Hp, Wp):
     return out
 
 
-def cfg_euler_(x, v, scale, dsigma):
-    """x (fp32, [1,...]) += dsigma * (v[0] + scale * (v[1] - v[0])); v bf16 [2, ...]."""
+def _u_scale(u_scale):
+    """The CFG-Zero* scale operand of a scaled update: a one-element fp32 device tensor (scail_b200.guidance)."""
+    _req(u_scale, torch.float32)
+    assert u_scale.numel() == 1, tuple(u_scale.shape)
+    return _ptr(u_scale)
+
+
+def cfg_euler_(x, v, scale, dsigma, u_scale=None):
+    """x (fp32, [1,...]) += dsigma * (v[0] + scale * (v[1] - v[0])); v bf16 [2, ...].
+    With u_scale (fp32 [1] on the device, CFG-Zero*'s s), another kernel, per element in this order with each product and
+    sum rounded on its own: u' = s*v[0]; g = u' + scale*(v[1] - u'); x = x + dsigma*g (x.numel() % 4 == 0).  Returns x."""
     _req(x, torch.float32), _req(v)
     assert x.is_contiguous() and v.is_contiguous() and v.numel() == 2 * x.numel()
-    _lib.check(_lib.lib().scail_cfg_euler(_ptr(x), _ptr(v), x.numel(), float(scale), float(dsigma), _stream()), "scail_cfg_euler")
+    if u_scale is None:
+        _lib.check(_lib.lib().scail_cfg_euler(_ptr(x), _ptr(v), x.numel(), float(scale), float(dsigma), _stream()),
+                   "scail_cfg_euler")
+    else:
+        _lib.check(_lib.lib().scail_cfg_euler_scaled(_ptr(x), _ptr(v), x.numel(), float(scale), float(dsigma),
+                                                     _u_scale(u_scale), _stream()), "scail_cfg_euler_scaled")
     _count()
     return x
 
 
-def unipc_step_(x, x_last, v, slots, write_slot, scale, sigma, coef, correct):
+def unipc_step_(x, x_last, v, slots, write_slot, scale, sigma, coef, correct, u_scale=None):
     """One fused UniPC step (scail_b200.unipc), in place: g = v[0] + scale*(v[1] - v[0]); m = x - sigma*g; y = a_x*x_last +
     a_k*slots[k] (slot order) + a_m*m if `correct`, else y = x; x = b_y*y + b_k*slots[k] + b_m*m; x_last = y;
     slots[write_slot] = m.  Each product and sum rounded on its own; slots with zero coefficients are not read.
     x, x_last fp32 (same shape, contiguous), v bf16 [2, ...], slots fp32 [n_slots, x.numel()]; coef: 10 floats
-    (a_x, a_0, a_1, a_2, a_m, b_y, b_0, b_1, b_2, b_m), passed by value.  Returns x."""
+    (a_x, a_0, a_1, a_2, a_m, b_y, b_0, b_1, b_2, b_m), passed by value.  With u_scale (fp32 [1] on the device, CFG-Zero*'s
+    s), u = s*v[0] (one rounded product) comes first and every later instruction is the same: s = 1 gives the unscaled
+    step bit for bit.  Returns x."""
     _req(x, torch.float32), _req(x_last, torch.float32), _req(v), _req(slots, torch.float32)
     assert x.is_contiguous() and x_last.is_contiguous() and x_last.shape == x.shape
     assert v.is_contiguous() and v.numel() == 2 * x.numel()
     assert slots.dim() == 2 and slots.is_contiguous() and slots.shape[1] == x.numel(), tuple(slots.shape)
     assert len(coef) == 10
     c = (ctypes.c_float * 10)(*coef)
-    _lib.check(_lib.lib().scail_unipc_step(_ptr(x), _ptr(x_last), _ptr(v), _ptr(slots), slots.stride(0), slots.shape[0],
-                                           int(write_slot), x.numel(), float(scale), float(sigma), int(bool(correct)),
-                                           ctypes.addressof(c), _stream()), "scail_unipc_step")
+    args = (_ptr(x), _ptr(x_last), _ptr(v), _ptr(slots), slots.stride(0), slots.shape[0], int(write_slot), x.numel(),
+            float(scale), float(sigma), int(bool(correct)), ctypes.addressof(c))
+    if u_scale is None:
+        _lib.check(_lib.lib().scail_unipc_step(*args, _stream()), "scail_unipc_step")
+    else:
+        _lib.check(_lib.lib().scail_unipc_step_scaled(*args, _u_scale(u_scale), _stream()), "scail_unipc_step_scaled")
     _count()
     return x
 
@@ -591,30 +610,39 @@ def cfg_cache_delta(v, d_ref, d_new, partials, out):
     return out
 
 
-def cfg_euler_cached_(x, c, delta, scale, dsigma):
+def cfg_euler_cached_(x, c, delta, scale, dsigma, u_scale=None):
     """The conditional-only Euler step, in place on x (fp32): u = c - delta; g = u + scale*(c - u); x = x + dsigma*g, each
-    product and sum rounded on its own.  c bf16 (the conditional output alone), delta fp32, both with x's element count."""
+    product and sum rounded on its own.  c bf16 (the conditional output alone), delta fp32, both with x's element count.
+    With u_scale (fp32 [1] on the device, CFG-Zero*'s s), u = s*u (one rounded product) right after u is formed; s = 1
+    gives the unscaled step bit for bit."""
     _req(x, torch.float32), _req(c), _req(delta, torch.float32)
     assert x.is_contiguous() and c.is_contiguous() and delta.is_contiguous() and c.numel() == x.numel() == delta.numel()
-    _lib.check(_lib.lib().scail_cfg_euler_cached(_ptr(x), _ptr(c), _ptr(delta), x.numel(), float(scale), float(dsigma),
-                                                 _stream()), "scail_cfg_euler_cached")
+    args = (_ptr(x), _ptr(c), _ptr(delta), x.numel(), float(scale), float(dsigma))
+    if u_scale is None:
+        _lib.check(_lib.lib().scail_cfg_euler_cached(*args, _stream()), "scail_cfg_euler_cached")
+    else:
+        _lib.check(_lib.lib().scail_cfg_euler_cached_scaled(*args, _u_scale(u_scale), _stream()),
+                   "scail_cfg_euler_cached_scaled")
     _count()
     return x
 
 
-def unipc_step_cached_(x, x_last, c, delta, slots, write_slot, scale, sigma, coef, correct):
+def unipc_step_cached_(x, x_last, c, delta, slots, write_slot, scale, sigma, coef, correct, u_scale=None):
     """unipc_step_ with u = f32(c) - delta in place of the pair's u: c bf16 (the conditional output alone), delta fp32, both
-    with x's element count; everything else as unipc_step_.  Returns x."""
+    with x's element count; everything else (u_scale included) as unipc_step_.  Returns x."""
     _req(x, torch.float32), _req(x_last, torch.float32), _req(c), _req(delta, torch.float32), _req(slots, torch.float32)
     assert x.is_contiguous() and x_last.is_contiguous() and x_last.shape == x.shape
     assert c.is_contiguous() and delta.is_contiguous() and c.numel() == x.numel() == delta.numel()
     assert slots.dim() == 2 and slots.is_contiguous() and slots.shape[1] == x.numel(), tuple(slots.shape)
     assert len(coef) == 10
     k = (ctypes.c_float * 10)(*coef)
-    _lib.check(_lib.lib().scail_unipc_step_cached(_ptr(x), _ptr(x_last), _ptr(c), _ptr(delta), _ptr(slots), slots.stride(0),
-                                                  slots.shape[0], int(write_slot), x.numel(), float(scale), float(sigma),
-                                                  int(bool(correct)), ctypes.addressof(k), _stream()),
-               "scail_unipc_step_cached")
+    args = (_ptr(x), _ptr(x_last), _ptr(c), _ptr(delta), _ptr(slots), slots.stride(0), slots.shape[0], int(write_slot),
+            x.numel(), float(scale), float(sigma), int(bool(correct)), ctypes.addressof(k))
+    if u_scale is None:
+        _lib.check(_lib.lib().scail_unipc_step_cached(*args, _stream()), "scail_unipc_step_cached")
+    else:
+        _lib.check(_lib.lib().scail_unipc_step_cached_scaled(*args, _u_scale(u_scale), _stream()),
+                   "scail_unipc_step_cached_scaled")
     _count()
     return x
 
@@ -643,21 +671,25 @@ def cfg_cache_delta_forecast(v, slots, write_slot, coef, partials, out):
     return out
 
 
-def cfg_euler_cached_forecast_(x, c, slots, coef, scale, dsigma):
-    """cfg_euler_cached_ with delta = the forecast of the delta slots (as cfg_cache_delta_forecast forms it)."""
+def cfg_euler_cached_forecast_(x, c, slots, coef, scale, dsigma, u_scale=None):
+    """cfg_euler_cached_ (u_scale included) with delta = the forecast of the delta slots (as cfg_cache_delta_forecast forms
+    it)."""
     _req(x, torch.float32), _req(c), _req(slots, torch.float32)
     assert x.is_contiguous() and c.is_contiguous() and c.numel() == x.numel()
     stride, n_slots, k = _delta_forecast(slots, coef, x.numel())
-    _lib.check(_lib.lib().scail_cfg_euler_cached_forecast(_ptr(x), _ptr(c), _ptr(slots), stride, n_slots, ctypes.addressof(k),
-                                                          x.numel(), float(scale), float(dsigma), _stream()),
-               "scail_cfg_euler_cached_forecast")
+    args = (_ptr(x), _ptr(c), _ptr(slots), stride, n_slots, ctypes.addressof(k), x.numel(), float(scale), float(dsigma))
+    if u_scale is None:
+        _lib.check(_lib.lib().scail_cfg_euler_cached_forecast(*args, _stream()), "scail_cfg_euler_cached_forecast")
+    else:
+        _lib.check(_lib.lib().scail_cfg_euler_cached_forecast_scaled(*args, _u_scale(u_scale), _stream()),
+                   "scail_cfg_euler_cached_forecast_scaled")
     _count()
     return x
 
 
-def unipc_step_cached_forecast_(x, x_last, c, dslots, dcoef, slots, write_slot, scale, sigma, coef, correct):
+def unipc_step_cached_forecast_(x, x_last, c, dslots, dcoef, slots, write_slot, scale, sigma, coef, correct, u_scale=None):
     """unipc_step_cached_ with delta = the forecast of the delta slots dslots with the coefficients dcoef (as
-    cfg_cache_delta_forecast forms it); everything else as unipc_step_.  Returns x."""
+    cfg_cache_delta_forecast forms it); everything else (u_scale included) as unipc_step_.  Returns x."""
     _req(x, torch.float32), _req(x_last, torch.float32), _req(c), _req(dslots, torch.float32), _req(slots, torch.float32)
     assert x.is_contiguous() and x_last.is_contiguous() and x_last.shape == x.shape
     assert c.is_contiguous() and c.numel() == x.numel()
@@ -665,13 +697,52 @@ def unipc_step_cached_forecast_(x, x_last, c, dslots, dcoef, slots, write_slot, 
     assert len(coef) == 10
     dstride, n_d, dk = _delta_forecast(dslots, dcoef, x.numel())
     k = (ctypes.c_float * 10)(*coef)
-    _lib.check(_lib.lib().scail_unipc_step_cached_forecast(_ptr(x), _ptr(x_last), _ptr(c), _ptr(dslots), dstride, n_d,
-                                                           ctypes.addressof(dk), _ptr(slots), slots.stride(0), slots.shape[0],
-                                                           int(write_slot), x.numel(), float(scale), float(sigma),
-                                                           int(bool(correct)), ctypes.addressof(k), _stream()),
-               "scail_unipc_step_cached_forecast")
+    args = (_ptr(x), _ptr(x_last), _ptr(c), _ptr(dslots), dstride, n_d, ctypes.addressof(dk), _ptr(slots), slots.stride(0),
+            slots.shape[0], int(write_slot), x.numel(), float(scale), float(sigma), int(bool(correct)), ctypes.addressof(k))
+    if u_scale is None:
+        _lib.check(_lib.lib().scail_unipc_step_cached_forecast(*args, _stream()), "scail_unipc_step_cached_forecast")
+    else:
+        _lib.check(_lib.lib().scail_unipc_step_cached_forecast_scaled(*args, _u_scale(u_scale), _stream()),
+                   "scail_unipc_step_cached_forecast_scaled")
     _count()
     return x
+
+
+# ---------------------------------------------------------------- CFG-Zero* guidance (scail_b200.guidance)
+def cfg_zero_scale(v, partials, out, u_scale, delta=None, forecast=None):
+    """CFG-Zero*'s optimised scale s = <c, u> / (|u|^2 + 1e-8) over all elements, on the device: u_scale (fp32 [1]) = s,
+    computed in fp64 and rounded once, and out (fp64 [4]) = (<c, u>, |u|^2, 0, 0).  u and c come from
+      v alone:        v bf16 [2, ...], the CFG pair (u, c) as cfg_euler_ reads it;
+      delta:          v = c alone (bf16 [1, ...]) and u = f32(c) - delta (fp32), as cfg_euler_cached_ forms it;
+      forecast:       v = c alone and u = f32(c) - delta_hat with forecast = (slots, coefficients), as
+                      cfg_euler_cached_forecast_ forms it.
+    Pass 1 adds f32(c)*u and u*u per CTA in fp32 (each product and sum rounded on its own) over a partition fixed by the
+    size; pass 2 adds the CTA sums in fp64 in a fixed order.  Bit-reproducible; partials fp32 [>= STEP_CACHE_PARTIALS]
+    scratch.  Returns u_scale."""
+    if delta is not None and forecast is not None:
+        raise ValueError("cfg_zero_scale: pass delta or forecast, not both")
+    _req(v), _req(partials, torch.float32), _req(out, torch.float64)
+    assert v.is_contiguous() and partials.is_contiguous() and out.is_contiguous() and out.numel() >= 4
+    up = _u_scale(u_scale)
+    dptr, dstride, n_d, dk = None, 0, 0, None
+    if forecast is not None:
+        n = v.numel()
+        _req(forecast[0], torch.float32)
+        dstride, n_d, dk = _delta_forecast(forecast[0], forecast[1], n)
+        form, dptr = 2, _ptr(forecast[0])
+    elif delta is not None:
+        n = v.numel()
+        _req(delta, torch.float32)
+        assert delta.is_contiguous() and delta.numel() == n
+        form, dptr = 1, _ptr(delta)
+    else:
+        n = v.numel() // 2
+        form = 0
+    _lib.check(_lib.lib().scail_cfg_zero_scale(form, _ptr(v), dptr, dstride, n_d, None if dk is None else ctypes.addressof(dk),
+                                               _ptr(partials), partials.numel(), _ptr(out), up, n, _stream()),
+               "scail_cfg_zero_scale")
+    _count(2)
+    return u_scale
 
 
 # ---------------------------------------------------------------- first-block residual cache (scail_b200.step_cache)

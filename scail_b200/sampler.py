@@ -12,6 +12,7 @@ import torch
 
 from . import cfg_cache as cfgc
 from . import dit, ops
+from . import guidance as gd
 from .step_cache import check_supported
 
 
@@ -42,8 +43,14 @@ def _check_cfg_cache(model, cfg_cache, plan=None, model_kwargs=None):
         cfgc.check_supported(getattr(_adaln(model), "cp", None), mk.get("chunk_dim"), mk.get("_num_layers"), plan)
 
 
+def _check_guidance(model, guidance, model_kwargs=None):
+    """Validate a guidance argument and refuse what it does not cover (scail_b200.guidance.check_supported)."""
+    if gd.check_guidance(guidance) is not None:
+        gd.check_supported(getattr(_adaln(model), "cp", None), (model_kwargs or {}).get("chunk_dim"))
+
+
 def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, plan=None, _x_override=None, _sigma_override=None,
-                 step_cache=None, solver=None, cfg_cache=None, **model_kwargs):
+                 step_cache=None, solver=None, cfg_cache=None, guidance=None, **model_kwargs):
     """One reference sampler step: x [1,t,16,h,w] fp32 (updated in place and returned).
     cond/uc: dicts with 'crossattn' [1,L,text_dim]; cond also carries ref_concat, concat_smpl_render,
     image_clip_features, concat_images (shared by both CFG branches, guiders.py:50-56).
@@ -55,12 +62,19 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     must be the solver's next pair and x its latent, else ValueError before anything runs.
     cfg_cache: an optional scail_b200.cfg_cache.CFGCache (single GPU only).  It decides before the forward whether this step
     runs the conditional branch alone (b = 1, on the cache's stream) and rebuilds u = c - delta for the update (delta
-    forecast at this step's sigma when the cache's order is >= 1); the first-block cache then sits the step out."""
+    forecast at this step's sigma when the cache's order is >= 1); the first-block cache then sits the step out.
+    guidance: an optional scail_b200.guidance.CFGZeroStar (not under context parallelism or chunk_dim).  It counts this
+    step first: a zero-initialised step runs no forward and tells neither cache about it, leaves x as it is with Euler and
+    runs the solver on a zero CFG pair; any other step scales u by s*, reduced on the device from the pair (or from the CFG
+    cache's rebuilt u), before the combine.  (guided_velocity does not count steps: it applies s* only.)"""
     _check_cfg_cache(model, cfg_cache, plan, model_kwargs)
+    _check_guidance(model, guidance, model_kwargs)
     if solver is not None:
         solver.check_step(x, sigma, next_sigma)
     if step_cache is not None:
         check_supported(plan=plan)
+    if guidance is not None and _x_override is None and guidance.begin_step():
+        return guidance.zero_step(x, scale, sigma, next_sigma, solver)
     cond_only = cfg_cache is not None and cfg_cache.begin_step(x, sigma if _sigma_override is None else _sigma_override)
     if step_cache is not None and not cond_only:
         step_cache.set_sigma(sigma if _sigma_override is None else _sigma_override)
@@ -73,7 +87,7 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     if cond_only:
         ts = torch.full((1,), c_noise, device=x.device, dtype=torch.float32)
         c = cfg_cache.cond_forward(model, x_in, ts, ctx[1:2], kw)
-        return cfg_cache.cond_update(x, c, scale, sigma, next_sigma, solver)
+        return cfg_cache.cond_update(x, c, scale, sigma, next_sigma, solver, guidance)
     if plan is None:
         x2 = torch.cat([x_in, x_in], 0)
         ts = torch.full((2,), c_noise, device=x.device, dtype=torch.float32)
@@ -84,19 +98,26 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
         v = plan.gather_branches(model(x_in, timesteps=ts, context=ctx[b:b + 1], **kw))
     if cfg_cache is not None:
         cfg_cache.full_step(v.contiguous())
+    if guidance is not None:
+        return guidance.update(x, v.contiguous(), scale, sigma, next_sigma, solver)
     if solver is not None:
         return solver.step(x, v.contiguous(), scale, sigma, next_sigma)
     return ops.cfg_euler_(x, v.contiguous(), scale, float(next_sigma) - float(sigma))
 
 
-def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None, step_cache=None, solver=None, cfg_cache=None):
+def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=None, step_cache=None, solver=None, cfg_cache=None,
+           guidance=None):
     """RFSampler.__call__ (sampling.py:965-982): the full Euler loop.  With `adaln_layer.cache_cross_kv` the step-invariant
     conditioning (text / CLIP embeddings and all layers' cross-attention K,V) is computed once for this call.  step_cache (a
     scail_b200.step_cache.FirstBlockCache) is reset here and then decides on every step whether blocks 1..L-1 run.
     solver (a scail_b200.unipc.UniPC) is bound to this call's schedule here and replaces the Euler update on every step.
     cfg_cache (a scail_b200.cfg_cache.CFGCache) is reset here and then decides on every step whether only the conditional
-    branch runs; with cache_cross_kv that forward reads the cond row of this call's conditioning."""
+    branch runs; with cache_cross_kv that forward reads the cond row of this call's conditioning.  guidance (a
+    scail_b200.guidance.CFGZeroStar) is reset here; its first zero_init_steps steps run no forward."""
     _check_cfg_cache(model, cfg_cache, plan)
+    _check_guidance(model, guidance)
+    if guidance is not None:
+        guidance.reset()
     if cfg_cache is not None:
         cfg_cache.reset()
     if step_cache is not None:
@@ -113,17 +134,19 @@ def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=No
     try:
         for i in range(num_steps):
             x = sampler_step(model, x, sig[i], sig[i + 1], cond, uc, scale, _ctx=ctx, plan=plan, step_cache=step_cache,
-                             solver=solver, cfg_cache=cfg_cache)
+                             solver=solver, cfg_cache=cfg_cache, guidance=guidance)
     finally:
         if cache:
             model.clear_conditioning()
     return x
 
 
-def guided_velocity(model, x, sigma, cond, uc, scale=4.0, ctx=None, plan=None):
+def guided_velocity(model, x, sigma, cond, uc, scale=4.0, ctx=None, plan=None, guidance=None):
     """RFSampler.denoise (sampling.py:945-953): CFG batch-2 forward + `u + s (c - u)` -> fp32 guided velocity [1,t,16,h,w]
-    (the fused CFG+Euler kernel applied to a zero latent with d_sigma = 1)."""
-    return sampler_step(model, torch.zeros_like(x), 0.0, 1.0, cond, uc, scale, _ctx=ctx, plan=plan, _x_override=x, _sigma_override=sigma)
+    (the fused CFG+Euler kernel applied to a zero latent with d_sigma = 1).  With guidance (a CFGZeroStar), u is scaled by
+    this call's own s* (the scaled kernel); zero-init is the caller's decision (sample_long), so no step is counted."""
+    return sampler_step(model, torch.zeros_like(x), 0.0, 1.0, cond, uc, scale, _ctx=ctx, plan=plan, _x_override=x, _sigma_override=sigma,
+                        guidance=guidance)
 
 
 def make_tile_indices(num_frames, segment, stride):
@@ -166,10 +189,16 @@ def sampler_step_long(denoise, x, sigma, next_sigma, tile_indices, smpl_tiled, c
     return x + (next_sigma - sigma) * denoised
 
 
-def sample_long(model, x, cond, uc, tile_indices, num_steps=50, shift_scale=5.0, scale=4.0, denoise=None, plan=None):
+def sample_long(model, x, cond, uc, tile_indices, num_steps=50, shift_scale=5.0, scale=4.0, denoise=None, plan=None,
+                guidance=None):
     """RFSamplerLong.__call__ (sampling.py:1070-1085): tiled long-video sampling.  x [1,T,16,h,w] fp32 over ALL latent frames;
     cond['smpl_tiled'] [1, n_tiles, segment, 16, h/2, w/2] holds the pose render of every window; `tile_indices` lists the
-    latent-frame indices of every window (equal lengths).  `denoise` overrides the network call (tests)."""
+    latent-frame indices of every window (equal lengths).  `denoise` overrides the network call (tests).
+    guidance (a scail_b200.guidance.CFGZeroStar) is reset here.  On a zero-initialised step every window's velocity is zero,
+    so the whole step is skipped and x is unchanged; on every other step each window's guided_velocity uses its own s*."""
+    _check_guidance(model, guidance)
+    if guidance is not None:
+        guidance.reset()
     sig = make_flow_timesteps(num_steps, shift_scale).to(x.device)
     smpl_tiled = cond["smpl_tiled"]
     uc = dict(uc if uc is not None else cond)
@@ -178,8 +207,11 @@ def sample_long(model, x, cond, uc, tile_indices, num_steps=50, shift_scale=5.0,
         ctx = prepare_context(cond, uc)
 
         def denoise(x_tile, sigma, c_k, u_k):
-            return guided_velocity(model, x_tile.contiguous(), float(sigma), c_k, u_k, scale, ctx=ctx, plan=plan)
+            return guided_velocity(model, x_tile.contiguous(), float(sigma), c_k, u_k, scale, ctx=ctx, plan=plan,
+                                   guidance=guidance)
     for i in range(num_steps):
+        if guidance is not None and guidance.begin_step():
+            continue
         x = sampler_step_long(denoise, x, sig[i], sig[i + 1], tile_indices, smpl_tiled, cond, uc)
     return x
 
@@ -207,10 +239,14 @@ class GraphedStep:
     row) is one more graph, captured on a stream of this object's own so that it has its own workspace; the host decides
     before each step which graphs replay.  Every graph's workspace tensors are held here (_workspace_of).  The delta kernel and the updates run eagerly after the replay (delta_ref and delta_new
     alternate between two buffers, which a graph would fix; at order >= 1 the forecast coefficients are kernel arguments
-    computed from each step's sigma, so no graph depends on them either)."""
+    computed from each step's sigma, so no graph depends on them either).
+    guidance (a scail_b200.guidance.CFGZeroStar, reset at construction): a zero-initialised step replays nothing and runs
+    only the solver's step on a zero pair, if there is a solver; on any other step the reduction of s* and the scaled
+    update run eagerly after the replay, and s* stays on the device, so no graph depends on it."""
 
-    def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None, solver=None, cfg_cache=None):
+    def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None, solver=None, cfg_cache=None, guidance=None):
         _check_cfg_cache(model, cfg_cache)
+        _check_guidance(model, guidance)
         if step_cache is not None:
             check_supported(getattr(model.mixins["adaln_layer"], "cp", None))
         if getattr(model.mixins["adaln_layer"], "cp", None) is not None:
@@ -227,7 +263,9 @@ class GraphedStep:
         self.fp8 = getattr(self.adaln, "fp8_linear", False)
         # the e4m3 weights are derived on this stream and held here: the graph replays against these very buffers
         self._fp8_weights = self.adaln.prepare_fp8_weights() if self.fp8 else []
-        self.step_cache, self.cfg_cache = step_cache, cfg_cache
+        self.step_cache, self.cfg_cache, self.guidance = step_cache, cfg_cache, guidance
+        if guidance is not None:
+            guidance.reset()
         if cfg_cache is not None:
             cfg_cache.reset()
             self._capture_cond()
@@ -308,6 +346,8 @@ class GraphedStep:
         self._ws = _workspace_of(side)
 
     def _update(self, v, sigma, next_sigma):
+        if self.guidance is not None:
+            return self.guidance.update(self.x, v, self.scale, sigma, next_sigma, self.solver)
         if self.solver is not None:
             return self.solver.step(self.x, v, self.scale, sigma, next_sigma)
         return ops.cfg_euler_(self.x, v, self.scale, float(next_sigma) - float(sigma))
@@ -315,13 +355,16 @@ class GraphedStep:
     def __call__(self, sigma, next_sigma):
         if self.solver is not None:
             self.solver.check_step(self.x, sigma, next_sigma)
+        g = self.guidance
+        if g is not None and g.begin_step():
+            return g.zero_step(self.x, self.scale, sigma, next_sigma, self.solver)
         if self.fp8:
             self.adaln.prepare_fp8_weights()
         cc = self.cfg_cache
         if cc is not None and cc.begin_step(self.x, sigma):
             self.ts1.fill_(float(sigma) * 1000.0)
             self.graph1.replay()
-            return cc.cond_update(self.x, self.v1, self.scale, sigma, next_sigma, self.solver)
+            return cc.cond_update(self.x, self.v1, self.scale, sigma, next_sigma, self.solver, g)
         v = self._full(sigma)
         if cc is not None:
             cc.full_step(v)

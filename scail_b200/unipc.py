@@ -226,12 +226,13 @@ class UniPC:
             raise ValueError(f"solver: the latent {tuple(x.shape)} {x.dtype} on {x.device} is not the latent "
                              f"{self._key[0]} {self._key[1]} on {self._key[2]} the solver's state was built for")
 
-    def step(self, x, v, scale, sigma, next_sigma, delta=None, forecast=None):
+    def step(self, x, v, scale, sigma, next_sigma, delta=None, forecast=None, u_scale=None):
         """One solver step in place on x (fp32), from the CFG pair v (bf16 [2, ...], as cfg_euler_ reads it).  With `delta`
         (fp32, x's element count: a scail_b200.cfg_cache.CFGCache's held c - u), v is the conditional output alone (bf16
         [1, ...]) and u = f32(c) - delta; the coefficients and the state are those of the pair step.  `forecast` takes the
         place of delta for a CFGCache of order >= 1: (slots, coefficients), delta_hat = c0*S0 + c1*S1 + c2*S2 as
-        ops.cfg_cache_delta_forecast forms it, and u = f32(c) - delta_hat.  Returns x."""
+        ops.cfg_cache_delta_forecast forms it, and u = f32(c) - delta_hat.  u_scale (fp32 [1] on the device, from
+        scail_b200.guidance.CFGZeroStar) scales u by s* before the guided combine.  Returns x."""
         if delta is not None and forecast is not None:
             raise ValueError("solver: pass delta or forecast, not both")
         self.check_step(x, sigma, next_sigma)
@@ -248,12 +249,13 @@ class UniPC:
         pad = [0.0] * (3 - self._order)
         coef = [k.x_last_c, *k.slot_c, *pad, k.m_c, k.y_c, *k.slot_p, *pad, k.m_p]
         coef = [_f32(c) for c in coef]
+        kw = {} if u_scale is None else dict(u_scale=u_scale)
         if forecast is not None:
             ops.unipc_step_cached_forecast_(x, self.x_last, v, *forecast, self.slots, k.write, scale, self._sigmas[i], coef,
-                                            k.correct)
+                                            k.correct, **kw)
         elif delta is None:
-            ops.unipc_step_(x, self.x_last, v, self.slots, k.write, scale, self._sigmas[i], coef, k.correct)
+            ops.unipc_step_(x, self.x_last, v, self.slots, k.write, scale, self._sigmas[i], coef, k.correct, **kw)
         else:
-            ops.unipc_step_cached_(x, self.x_last, v, delta, self.slots, k.write, scale, self._sigmas[i], coef, k.correct)
+            ops.unipc_step_cached_(x, self.x_last, v, delta, self.slots, k.write, scale, self._sigmas[i], coef, k.correct, **kw)
         self._i = i + 1
         return x
