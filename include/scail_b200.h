@@ -299,6 +299,33 @@ int scail_unipc_step_cached_forecast_scaled(float* x, float* x_last, const void*
                                             int64_t n_dslots, const float* dcoef, float* slots, int64_t slot_stride,
                                             int64_t n_slots, int64_t write_slot, int64_t n, float scale, float sigma,
                                             int correct, const float* coef, const float* u_scale, scail_stream_t stream);
+/* APG, adaptive projected guidance (scail_b200/guidance.py).  The fp32 latent x holds n elements in `frames` frames of
+ * n / frames elements (n % (4 * frames) == 0, 1 <= frames <= 65535); u and c come by `form` as in scail_cfg_zero_scale
+ * (0: the pair [2, n]; 1: c alone with u = f32(c) - delta; 2: c alone with u = f32(c) - the forecast of the delta slots).
+ * x, v, delta, avg and m are 16-byte aligned, partials 4-byte, sums and factors 8-byte.  Per element, each product and sum
+ * rounded on its own: D_c = x - sigma*c, diff = D_c - (x - sigma*u).
+ * scail_apg_reduce (pass 1): with avg (fp32 [n], may be null) avg = diff + momentum*avg, read and written once, and diff =
+ *   avg.  fp32 partial sums of diff*diff, diff*D_c and D_c*D_c per (frame, CTA) over a partition fixed by the shape
+ *   (partials: at least 3 * frames * 32 floats).  Bit-reproducible.
+ * scail_apg_finish (pass 2): per frame, the partials added in fp64 in a fixed order -> sums [frames, 4] fp64 = {|diff|^2,
+ *   <diff, D_c>, |D_c|^2, 0} and factors [frames, 2] = {f, p}, each computed in fp64 and rounded once to fp32: f =
+ *   norm_threshold / |diff| if norm_threshold > 0 and |diff| > norm_threshold, else 1; p = f <diff, D_c> / |D_c|^2, 0 when
+ *   |D_c|^2 = 0.
+ * scail_apg_update: diff as pass 1 left it (avg when given, which then must be the average pass 1 wrote; else formed again
+ *   by the same instructions); par = p*D_c; orth = f*diff - par; D_g = D_c + wm1*(orth + eta*par).  With m (fp32 [n]) D_g
+ *   -> m and x is only read; with m null, x = x + k_euler*(x - D_g) in place.
+ * scail_unipc_step_dpred: scail_unipc_step with the data prediction m read from `m` (fp32 [n]) in place of x - sigma*g;
+ *   every other instruction and check as there. */
+int scail_apg_reduce(int form, const float* x, const void* v, const float* delta, int64_t delta_stride, int64_t n_dslots,
+                     const float* dcoef, float* avg, float sigma, float momentum, float* partials, int64_t partials_len,
+                     int64_t frames, int64_t n, scail_stream_t stream);
+int scail_apg_finish(const float* partials, int64_t partials_len, double* sums, float* factors, double norm_threshold,
+                     int64_t frames, int64_t n, scail_stream_t stream);
+int scail_apg_update(int form, float* x, const void* v, const float* delta, int64_t delta_stride, int64_t n_dslots,
+                     const float* dcoef, const float* avg, const float* factors, float* m, float sigma, float wm1, float eta,
+                     float k_euler, int64_t frames, int64_t n, scail_stream_t stream);
+int scail_unipc_step_dpred(float* x, float* x_last, const float* m, float* slots, int64_t slot_stride, int64_t n_slots,
+                           int64_t write_slot, int64_t n, int correct, const float* coef, scail_stream_t stream);
 
 /* First-block residual cache (scail_b200/step_cache.py).  Token tensors are bf16 [B, N, d] (ref || noise || pose rows of
  * each batch element); the noise rows are rows [n_ref, n_ref + n_seq) of each element.  d % 8 == 0, B*N*d/8 < 2^31, and

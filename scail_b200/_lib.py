@@ -79,6 +79,10 @@ SIGNATURES = {
     "scail_unipc_step_cached_scaled": [c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f, c_f, c_int, c_p, c_p, c_p],
     "scail_unipc_step_cached_forecast_scaled": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_f,
                                                 c_f, c_int, c_p, c_p, c_p],
+    "scail_apg_reduce": [c_int, c_p, c_p, c_p, c_i64, c_i64, c_p, c_p, c_f, c_f, c_p, c_i64, c_i64, c_i64, c_p],
+    "scail_apg_finish": [c_p, c_i64, c_p, c_p, ctypes.c_double, c_i64, c_i64, c_p],
+    "scail_apg_update": [c_int, c_p, c_p, c_p, c_i64, c_i64, c_p, c_p, c_p, c_p, c_f, c_f, c_f, c_f, c_i64, c_i64, c_p],
+    "scail_unipc_step_dpred": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_p, c_p],
     "scail_step_cache_indicator": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_update": [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
     "scail_step_cache_apply": [c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],

@@ -52,6 +52,7 @@ import weakref
 import torch
 
 from . import ops
+from .guidance import APG
 from .step_cache import check_max_skips, check_order, check_sigma, check_threshold, forecast_coefficients, indicator
 
 def _drop_workspaces(handles):
@@ -230,7 +231,10 @@ class CFGCache:
         """The conditional-only step's latent update in place on x from c, the conditional output alone (bf16 [1, ...]): u =
         f32(c) - delta (order 0) or f32(c) - delta_hat(sigma) (order >= 1), then the Euler step, or solver.step (a UniPC)
         when given.  With guidance (a scail_b200.guidance.CFGZeroStar), s* is reduced from that same u first and the
-        update is the scaled one.  Returns x."""
+        update is the scaled one; with a scail_b200.guidance.APG, its step runs on that same u.  Returns x."""
+        if isinstance(guidance, APG):
+            kw = dict(delta=self.delta) if self._order == 0 else dict(forecast=(self.buffers.slots, self.forecast()))
+            return guidance.update(x, c, scale, sigma, next_sigma, solver, **kw)
         ds = float(next_sigma) - float(sigma)
         if self._order == 0:
             kw = {} if guidance is None else dict(u_scale=guidance.scale(c, delta=self.delta))

@@ -15,6 +15,7 @@
 
 #include "../../include/scail_b200.h"
 #include "adaptive.cuh"
+#include "apg.cuh"
 #include "attention.cuh"
 #include "cfg_cache.cuh"
 #include "cfg_zero.cuh"
@@ -890,7 +891,8 @@ static int unipc_launch(const char* what, float* x, float* x_last, const void* v
 #define SCAIL_UNIPC_LAUNCH(...)                                                                                          \
     scail::unipc_step_kernel<__VA_ARGS__><<<grid, scail::UNIPC_THREADS, 0, st>>>(x4, xl4, v2, slots, slot_stride,      \
                                                                                  (int)n_slots, (int)write_slot, nvec,  \
-                                                                                 scale, sigma, corr, k, d4, ds, dk, u_scale)
+                                                                                 scale, sigma, corr, k, d4, ds, dk, u_scale,  \
+                                                                                 nullptr)
     if (!cached)
         u_scale ? SCAIL_UNIPC_LAUNCH(false, false, true) : SCAIL_UNIPC_LAUNCH(false);
     else if (!dcoef)
@@ -1134,6 +1136,136 @@ int scail_cfg_zero_scale(int form, const void* v, const float* delta, int64_t de
         scail::cfg_zero_dot_kernel<scail::CFGZ_FORECAST><<<ctas, scail::SC_THREADS, 0, st>>>(v2, delta, ds, dk, partials, nvec);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     scail::cfg_zero_finish_kernel<<<1, scail::SC_THREADS, 0, st>>>(partials, ctas, out, u_scale);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ---- APG (scail_b200/guidance.py, csrc/apg.cuh)
+
+// Checks shared by the APG entry points: the form and its operands, and the latent's frames; fills dk and the frame's
+// vector count.  Returns 0 or the fail() code.
+static int apg_operands(const char* what, int form, const float* x, const void* v, const float* delta, int64_t delta_stride,
+                        int64_t n_dslots, const float* dcoef, int64_t frames, int64_t n, scail::DeltaForecast* dk,
+                        int64_t* fvec) {
+    SCAIL_REQUIRE(form >= scail::CFGZ_PAIR && form <= scail::CFGZ_FORECAST,
+                  "%s: form = %d must be 0 (pair), 1 (cached) or 2 (forecast)", what, form);
+    SCAIL_REQUIRE(x && v, "%s: null operand", what);
+    SCAIL_REQUIRE(form == scail::CFGZ_PAIR || delta, "%s: null delta with form %d", what, form);
+    SCAIL_REQUIRE(form != scail::CFGZ_FORECAST || dcoef, "%s: null dcoef with form 2", what);
+    SCAIL_REQUIRE(aligned16(x) && aligned16(v) && (form == scail::CFGZ_PAIR || aligned16(delta)),
+                  "%s: x, v and delta must be 16-byte aligned", what);
+    SCAIL_REQUIRE(frames >= 1 && frames <= 65535, "%s: need 1 <= frames <= 65535 (got %lld)", what, (long long)frames);
+    SCAIL_REQUIRE(n >= 4 && n % (4 * frames) == 0 && n / 4 <= 0xffffffffll,
+                  "%s: need n a positive multiple of 4 * frames below 2^34 (got n=%lld, frames=%lld)", what, (long long)n,
+                  (long long)frames);
+    *dk = scail::DeltaForecast{};
+    if (form == scail::CFGZ_FORECAST)
+        if (int rc = delta_forecast_coef(what, delta_stride, n_dslots, n, dcoef, dk)) return rc;
+    *fvec = n / 4 / frames;
+    return 0;
+}
+
+int scail_apg_reduce(int form, const float* x, const void* v, const float* delta, int64_t delta_stride, int64_t n_dslots,
+                     const float* dcoef, float* avg, float sigma, float momentum, float* partials, int64_t partials_len,
+                     int64_t frames, int64_t n, scail_stream_t stream) {
+    scail::DeltaForecast dk;
+    int64_t fvec;
+    if (int rc = apg_operands("apg_reduce", form, x, v, delta, delta_stride, n_dslots, dcoef, frames, n, &dk, &fvec)) return rc;
+    SCAIL_REQUIRE(partials, "apg_reduce: null partials");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 3) == 0 && (!avg || aligned16(avg)),
+                  "apg_reduce: partials must be 4-byte and avg 16-byte aligned");
+    const int parts = scail::apg_ctas_per_frame(fvec);
+    SCAIL_REQUIRE(partials_len >= 3 * frames * parts, "apg_reduce: partials holds %lld floats, this size needs %lld",
+                  (long long)partials_len, (long long)(3 * frames * parts));
+    const dim3 grid(parts, static_cast<unsigned>(frames));
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const float4* x4 = reinterpret_cast<const float4*>(x);
+    const uint2* v2 = static_cast<const uint2*>(v);
+    const int64_t ds = form == scail::CFGZ_FORECAST ? delta_stride : 0;
+    float4* a4 = reinterpret_cast<float4*>(avg);
+#define SCAIL_APG_REDUCE(F, M) \
+    scail::apg_reduce_kernel<F, M><<<grid, scail::APG_THREADS, 0, st>>>(x4, v2, delta, ds, dk, a4, sigma, momentum, partials, fvec)
+    if (form == scail::CFGZ_PAIR)
+        avg ? SCAIL_APG_REDUCE(scail::CFGZ_PAIR, true) : SCAIL_APG_REDUCE(scail::CFGZ_PAIR, false);
+    else if (form == scail::CFGZ_CACHED)
+        avg ? SCAIL_APG_REDUCE(scail::CFGZ_CACHED, true) : SCAIL_APG_REDUCE(scail::CFGZ_CACHED, false);
+    else
+        avg ? SCAIL_APG_REDUCE(scail::CFGZ_FORECAST, true) : SCAIL_APG_REDUCE(scail::CFGZ_FORECAST, false);
+#undef SCAIL_APG_REDUCE
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_apg_finish(const float* partials, int64_t partials_len, double* sums, float* factors, double norm_threshold,
+                     int64_t frames, int64_t n, scail_stream_t stream) {
+    SCAIL_REQUIRE(partials && sums && factors, "apg_finish: null operand");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 3) == 0 && (reinterpret_cast<uintptr_t>(sums) & 7) == 0 &&
+                      (reinterpret_cast<uintptr_t>(factors) & 7) == 0,
+                  "apg_finish: partials must be 4-byte and sums and factors 8-byte aligned");
+    SCAIL_REQUIRE(frames >= 1 && frames <= 65535 && n >= 4 && n % (4 * frames) == 0,
+                  "apg_finish: need 1 <= frames <= 65535 and n a positive multiple of 4 * frames (got n=%lld, frames=%lld)",
+                  (long long)n, (long long)frames);
+    SCAIL_REQUIRE(std::isfinite(norm_threshold) && norm_threshold >= 0.0,
+                  "apg_finish: norm_threshold must be finite and >= 0 (got %g)", norm_threshold);
+    const int parts = scail::apg_ctas_per_frame(n / 4 / frames);
+    SCAIL_REQUIRE(partials_len >= 3 * frames * parts, "apg_finish: partials holds %lld floats, this size needs %lld",
+                  (long long)partials_len, (long long)(3 * frames * parts));
+    scail::apg_finish_kernel<<<static_cast<unsigned>(frames), 32, 0, static_cast<cudaStream_t>(stream)>>>(
+        partials, parts, norm_threshold, sums, factors);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_apg_update(int form, float* x, const void* v, const float* delta, int64_t delta_stride, int64_t n_dslots,
+                     const float* dcoef, const float* avg, const float* factors, float* m, float sigma, float wm1, float eta,
+                     float k_euler, int64_t frames, int64_t n, scail_stream_t stream) {
+    scail::DeltaForecast dk;
+    int64_t fvec;
+    if (int rc = apg_operands("apg_update", form, x, v, delta, delta_stride, n_dslots, dcoef, frames, n, &dk, &fvec)) return rc;
+    SCAIL_REQUIRE(factors, "apg_update: null factors");
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(factors) & 7) == 0 && (!avg || aligned16(avg)) && (!m || aligned16(m)),
+                  "apg_update: factors must be 8-byte and avg and m 16-byte aligned");
+    const int64_t nvec = n / 4;
+    const int grid = blocks_for(nvec, scail::APG_THREADS);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float4* x4 = reinterpret_cast<float4*>(x);
+    const uint2* v2 = static_cast<const uint2*>(v);
+    const int64_t ds = form == scail::CFGZ_FORECAST ? delta_stride : 0;
+    const float4* a4 = reinterpret_cast<const float4*>(avg);
+    const float2* f2 = reinterpret_cast<const float2*>(factors);
+    float4* m4 = reinterpret_cast<float4*>(m);
+    const unsigned fv = static_cast<unsigned>(fvec);
+#define SCAIL_APG_UPDATE(F, M, D)                                                                                           \
+    scail::apg_update_kernel<F, M, D><<<grid, scail::APG_THREADS, 0, st>>>(x4, v2, delta, ds, dk, a4, f2, m4, sigma, wm1, eta, \
+                                                                          k_euler, nvec, fv)
+#define SCAIL_APG_UPDATE_OUT(F, M) m ? SCAIL_APG_UPDATE(F, M, true) : SCAIL_APG_UPDATE(F, M, false)
+    if (avg)  // the diff is the average pass 1 wrote: the form only says where c is
+        form == scail::CFGZ_PAIR ? SCAIL_APG_UPDATE_OUT(scail::CFGZ_PAIR, true) : SCAIL_APG_UPDATE_OUT(scail::CFGZ_CACHED, true);
+    else if (form == scail::CFGZ_PAIR)
+        SCAIL_APG_UPDATE_OUT(scail::CFGZ_PAIR, false);
+    else if (form == scail::CFGZ_CACHED)
+        SCAIL_APG_UPDATE_OUT(scail::CFGZ_CACHED, false);
+    else
+        SCAIL_APG_UPDATE_OUT(scail::CFGZ_FORECAST, false);
+#undef SCAIL_APG_UPDATE_OUT
+#undef SCAIL_APG_UPDATE
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_unipc_step_dpred(float* x, float* x_last, const float* m, float* slots, int64_t slot_stride, int64_t n_slots,
+                           int64_t write_slot, int64_t n, int correct, const float* coef, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && x_last && m && slots && coef, "unipc_step_dpred: null operand");
+    SCAIL_REQUIRE(aligned16(x) && aligned16(x_last) && aligned16(m) && aligned16(slots),
+                  "unipc_step_dpred: x, x_last, m and slots must be 16-byte aligned");
+    scail::UnipcCoef k;
+    if (int rc = unipc_coef("unipc_step_dpred", slot_stride, n_slots, write_slot, n, coef, &k)) return rc;
+    const int64_t nvec = n / 4;
+    scail::unipc_step_kernel<false, false, false, true>
+        <<<blocks_for(nvec, scail::UNIPC_THREADS), scail::UNIPC_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+            reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(x_last), nullptr, slots, slot_stride, (int)n_slots,
+            (int)write_slot, nvec, 0.f, 0.f, correct ? 1 : 0, k, nullptr, 0, scail::DeltaForecast{}, nullptr,
+            reinterpret_cast<const float4*>(m));
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

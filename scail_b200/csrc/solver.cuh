@@ -71,21 +71,28 @@ __device__ __forceinline__ void delta_forecast4(const float* slots, int64_t slot
 // delta_forecast4 of the slots at `delta` (stride delta_stride floats) with the coefficients dk, in place of one held
 // delta.  `delta`, delta_stride and dk are the last parameters, so the other parameters keep their offsets.
 // kScaled (CFG-Zero*, scail_b200/guidance.py): u = (*u_scale) * u, one rounded product, once u is formed; the rest is
-// unchanged, so *u_scale == 1 gives the unscaled step bit for bit.  u_scale is the last parameter and is not read otherwise.
-template <bool kCached, bool kForecast = false, bool kScaled = false>
+// unchanged, so *u_scale == 1 gives the unscaled step bit for bit.  u_scale is not read otherwise.
+// kDataPred (APG, scail_b200/guidance.py): m is read from `mpred` (fp32, the guidance's data prediction) in place of
+// x - sigma*g, and v, delta, u_scale, scale and sigma are not read; every instruction after m is shared.  mpred is the last
+// parameter and is not read otherwise.
+template <bool kCached, bool kForecast = false, bool kScaled = false, bool kDataPred = false>
 __global__ void __launch_bounds__(UNIPC_THREADS) unipc_step_kernel(float4* __restrict__ x, float4* __restrict__ x_last,
                                                                    const uint2* __restrict__ v, float* __restrict__ slots,
                                                                    int64_t slot_stride, int n_slots, int write_slot,
                                                                    int64_t nvec, float scale, float sigma, int correct,
                                                                    UnipcCoef k, const float4* __restrict__ delta,
                                                                    int64_t delta_stride, DeltaForecast dk,
-                                                                   const float* __restrict__ u_scale) {
+                                                                   const float* __restrict__ u_scale,
+                                                                   const float4* __restrict__ mpred) {
     static_assert(kCached || !kForecast, "the forecast form is a cached step");
+    static_assert(!kDataPred || (!kCached && !kScaled), "the data-prediction form reads m alone");
     const int64_t i = static_cast<int64_t>(blockIdx.x) * UNIPC_THREADS + threadIdx.x;
     if (i >= nvec) return;
     float fx[4], fu[4], fc[4], m[4], y[4], z[4];
     unipc_load(x, i, fx);
-    if constexpr (kCached) {
+    if constexpr (kDataPred) {
+        unipc_load(mpred, i, m);
+    } else if constexpr (kCached) {
         float fd[4];
         unipc_unpack4(v[i], fc);
         if constexpr (kForecast)
@@ -108,10 +115,12 @@ __global__ void __launch_bounds__(UNIPC_THREADS) unipc_step_kernel(float4* __res
     for (int s = 0; s < UNIPC_MAX_SLOTS; ++s)
         if (s < n_slots && (k.a[s] != 0.f || k.b[s] != 0.f))
             unipc_load(reinterpret_cast<const float4*>(slots + s * slot_stride), i, M[s]);
+    if constexpr (!kDataPred) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const float g = __fadd_rn(fu[j], __fmul_rn(scale, __fsub_rn(fc[j], fu[j])));
-        m[j] = __fsub_rn(fx[j], __fmul_rn(sigma, g));
+        for (int j = 0; j < 4; ++j) {
+            const float g = __fadd_rn(fu[j], __fmul_rn(scale, __fsub_rn(fc[j], fu[j])));
+            m[j] = __fsub_rn(fx[j], __fmul_rn(sigma, g));
+        }
     }
     if (correct) {
         float xl[4];

@@ -1,7 +1,7 @@
-"""CFG-Zero* guidance (Fan et al., 2025, "CFG-Zero*: Improved Classifier-Free Guidance for Flow Matching Models"): an
-opt-in replacement for the sampler's vanilla guidance g = u + s (c - u).
+"""Opt-in replacements for the sampler's vanilla guidance g = u + s (c - u): CFG-Zero* and APG.  This module is the only one
+that knows their rules.
 
-This module is the only one that knows the rule.  It makes two changes:
+CFG-Zero* (Fan et al., 2025, "CFG-Zero*: Improved Classifier-Free Guidance for Flow Matching Models") makes two changes:
 
   optimised scale   the unconditional output is scaled by s* = <c, u> / (|u|^2 + 1e-8), one scalar over all latent
                     elements of the sample, before the usual combine: g = s* u + s (c - s* u).  When u is all zero s* = 0
@@ -21,7 +21,37 @@ Each update then forms u' = s* u (one rounded product) and runs its usual instru
 Memory per (latent shape, device): the reduction's fp32 partials (8 KiB), an fp64 {dot, norm, 0, 0} and one fp32 s*;
 with a UniPC solver and k >= 1, also a zero bf16 CFG pair (4 bytes per latent element).  No default k is chosen: what
 real weights want is not measured here.
+
+APG, adaptive projected guidance (Sadat, Hilliges, Weber, "Eliminating Oversaturation and Artifacts of High Guidance
+Scales in Diffusion Models", ICLR 2025), guides in data-prediction space.  For a step from sigma to sigma' with guidance
+scale w (the sampler's scale), on the latent x [1, T, 16, h, w]:
+
+  D_c = x - sigma c,  D_u = x - sigma u,  diff = D_c - D_u
+  momentum beta       avg <- diff + beta avg;  diff <- avg            (avg: one fp32 latent, zero after reset(); 0 = off)
+  norm threshold r    per frame t: diff_t <- diff_t min(1, r / |diff_t|)   (0 = off; factor 1 when |diff_t| = 0)
+  projection          per frame t: par_t = (<diff_t, D_c,t> / |D_c,t|^2) D_c,t (0 when |D_c,t| = 0), orth_t = diff_t - par_t
+  D_g = D_c + (w - 1) (orth + eta par)
+  Euler: x' = x + (sigma' - sigma) (x - D_g) / sigma;   UniPC: D_g is the step's data prediction m.
+
+A frame is one latent frame x[0, t], 16 h w contiguous elements: the paper's per-image rule applied to each frame of the
+video.  With eta = 1, beta = 0 and r = 0 the step is vanilla CFG in exact arithmetic.  NaN propagates.
+
+On the device (ops.apg_reduce, ops.apg_finish, then ops.apg_update_): pass 1 forms D_c and diff per element, applies the
+momentum (reading and writing avg once: this pass owns the write, and the update reads the new avg as diff) and adds
+diff*diff, diff*D_c and D_c*D_c per (frame, CTA) in fp32 over a partition fixed by the shape; pass 2 adds each frame's
+partials in fp64 in a fixed order and writes the threshold factor f_t and the projection coefficient p_t = f_t <diff_t,
+D_c,t> / |D_c,t|^2, each rounded once to fp32, to a [T, 2] device buffer; the update applies the rule, then the Euler step
+in place or D_g into an fp32 buffer that the solver's data-prediction step reads.  The factors never go to the host, so no
+step adds a host synchronisation and no captured graph depends on them.  u is formed as the update forms it: from the CFG
+pair on a full step, as f32(c) - delta (or its forecast) on a CFG cache's conditional-only step, and the momentum advances
+on every guided step, full or conditional-only.
+
+Memory per (latent shape, device): with momentum one fp32 latent (16.5 MB at 512x512 and 28.9 MB at 512x896, as every
+latent copy here); with a UniPC solver one fp32 latent for D_g; 3 T 32 fp32 partials, T x 4 fp64 sums and T x 2 fp32
+factors.  APG is not available in sample_long (momentum would need state per window) or guided_velocity.  No default
+eta, r or beta is chosen: what real weights want is not measured here.
 """
+import math
 import numbers
 
 import torch
@@ -30,21 +60,23 @@ from . import ops
 
 
 def check_guidance(guidance):
-    """None or a CFGZeroStar; anything else is a TypeError naming guidance."""
-    if guidance is not None and not isinstance(guidance, CFGZeroStar):
-        raise TypeError(f"guidance must be a scail_b200.guidance.CFGZeroStar or None, got {type(guidance).__name__}")
+    """None, a CFGZeroStar or an APG; anything else is a TypeError naming guidance."""
+    if guidance is not None and not isinstance(guidance, (CFGZeroStar, APG)):
+        raise TypeError("guidance must be a scail_b200.guidance.CFGZeroStar, a scail_b200.guidance.APG or None, got "
+                        f"{type(guidance).__name__}")
     return guidance
 
 
 def check_supported(cp=None, chunk_dim=None):
-    """Refuse what the rule does not cover: under context parallelism (size > 1) or with chunk_dim a rank may hold only part
-    of the velocity, so its s* would be a partial sum."""
+    """Refuse what the rules do not cover: under context parallelism (size > 1) or with chunk_dim a rank may hold only part
+    of the velocity, so CFG-Zero*'s s* and APG's per-frame sums would be partial sums."""
     if cp is not None and getattr(cp, "size", 1) > 1:
         raise NotImplementedError(f"guidance is not implemented under context parallelism (a ContextParallel of size "
-                                  f"{cp.size}): s* would be a partial sum; run without guidance or on one GPU")
+                                  f"{cp.size}): s* or APG's per-frame sums would be partial sums; run without guidance or "
+                                  "on one GPU")
     if chunk_dim is not None:
-        raise NotImplementedError("guidance is not implemented with chunk_dim (pre-chunked sequence parallelism): s* would "
-                                  "be a partial sum")
+        raise NotImplementedError("guidance is not implemented with chunk_dim (pre-chunked sequence parallelism): s* or "
+                                  "APG's per-frame sums would be partial sums")
 
 
 class _Buffers:
@@ -134,3 +166,113 @@ class CFGZeroStar:
         if solver is not None:
             return solver.step(x, v, scale, sigma, next_sigma, u_scale=s)
         return ops.cfg_euler_(x, v, scale, float(next_sigma) - float(sigma), u_scale=s)
+
+
+def _check_real(name, value, nonneg=False):
+    """A finite real number (not a bool) -> float; else ValueError naming the argument."""
+    ok = isinstance(value, numbers.Real) and not isinstance(value, bool) and math.isfinite(value)
+    if not ok or (nonneg and value < 0):
+        raise ValueError(f"APG: {name} must be a finite {'real >= 0' if nonneg else 'real'}, got {value!r}")
+    return float(value)
+
+
+class _APGBuffers:
+    """The device state for one latent (shape, device): pass 1's partials, pass 2's fp64 sums [T, 4] and fp32 factors [T, 2],
+    the momentum average (fp32, the latent's shape; with momentum only) and, on first use with a solver, D_g."""
+
+    def __init__(self, key, momentum):
+        shape, device = key
+        T = shape[1]
+        self.key = key
+        self.partials = torch.empty(ops.apg_partials_len(T), device=device, dtype=torch.float32)
+        self.sums = torch.zeros(T, 4, device=device, dtype=torch.float64)
+        self.factors = torch.zeros(T, 2, device=device, dtype=torch.float32)
+        self.avg = torch.zeros(shape, device=device, dtype=torch.float32) if momentum else None
+        self.stale = False  # the average holds a run before reset(): zero it before the next read
+        self.m = None
+
+
+class APG:
+    """APG state of one sampling run, for sampler.sample / sampler_step / GraphedStep(guidance=); see the module docstring.
+
+    eta (finite real): the weight of the component of diff parallel to D_c; eta = 1 with r = 0 and momentum = 0 is vanilla
+    CFG.  norm_threshold r (finite real >= 0; 0 = off): each frame's diff is scaled down to norm r, in data-prediction units
+    per frame, so its meaning depends on the frame's size 16 h w: the same r bounds the per-element difference more tightly
+    on a larger latent.  momentum beta (finite real; 0 = off, the paper uses beta < 0): avg <- diff + beta avg, over the
+    guided steps since reset().  Bools, non-finite values and a negative r raise ValueError naming the argument.  sample()
+    and GraphedStep() call reset()."""
+
+    def __init__(self, eta, norm_threshold=0.0, momentum=0.0):
+        self._eta = _check_real("eta", eta)
+        self._r = _check_real("norm_threshold", norm_threshold, nonneg=True)
+        self._beta = _check_real("momentum", momentum)
+        self._bufs = {}
+        self.reset()
+
+    @property
+    def eta(self):
+        return self._eta
+
+    @property
+    def norm_threshold(self):
+        return self._r
+
+    @property
+    def momentum(self):
+        return self._beta
+
+    def reset(self):
+        """Zero the momentum average (before its next read) and the step count.  The other buffers are kept: every step
+        writes them before it reads them."""
+        self._i = 0
+        self._last = None
+        for b in self._bufs.values():
+            b.stale = True
+
+    @property
+    def step_index(self):
+        """Guided steps counted since reset()."""
+        return self._i
+
+    def begin_step(self):
+        """Count one sampler step; always False: APG has no zero-initialised step (the sampler's CFG-Zero* hook)."""
+        self._i += 1
+        return False
+
+    @property
+    def last_factors(self):
+        """The fp32 [T, 2] device tensor of the last per-frame (threshold factor, projection coefficient), None before the
+        first, for tests; it is overwritten by the next step on a latent of the same shape and device."""
+        return self._last
+
+    def _buffers(self, x):
+        key = (tuple(x.shape), torch.device(x.device))
+        b = self._bufs.get(key)
+        if b is None:
+            b = self._bufs[key] = _APGBuffers(key, self._beta != 0.0)
+        if b.stale:
+            if b.avg is not None:
+                b.avg.zero_()
+            b.stale = False
+        return b
+
+    def update(self, x, v, scale, sigma, next_sigma, solver=None, delta=None, forecast=None):
+        """A guided step in place on x (fp32 [1, T, 16, h, w]) at sigma > 0: the two reductions, then the Euler step, or D_g
+        into this object's buffer and solver.step(m=D_g) with a UniPC.  u and c come from the CFG pair v, or from c = v
+        alone with delta or forecast (a CFGCache's conditional-only step), as ops.apg_reduce takes them.  Returns x."""
+        sigma = float(sigma)
+        if not sigma > 0.0:
+            raise ValueError(f"APG: a guided step needs sigma > 0 (data predictions divide by it), got {sigma!r}")
+        if solver is not None:
+            solver.check_step(x, sigma, next_sigma)
+        b = self._buffers(x)
+        ops.apg_reduce(x, v, sigma, b.partials, b.avg, self._beta, delta=delta, forecast=forecast)
+        ops.apg_finish(b.partials, b.sums, b.factors, self._r, x.shape[1], x.numel())
+        self._last = b.factors
+        if solver is None:
+            return ops.apg_update_(x, v, b.factors, scale, self._eta, sigma, next_sigma, avg=b.avg, delta=delta,
+                                   forecast=forecast)
+        if b.m is None:
+            b.m = torch.empty_like(x)
+        ops.apg_update_(x, v, b.factors, scale, self._eta, sigma, out=b.m, avg=b.avg, delta=delta, forecast=forecast)
+        return solver.step(x, None, scale, sigma, next_sigma, m=b.m)

@@ -745,6 +745,111 @@ def cfg_zero_scale(v, partials, out, u_scale, delta=None, forecast=None):
     return u_scale
 
 
+# ---------------------------------------------------------------- APG guidance (scail_b200.guidance)
+APG_MAX_CTAS_PER_FRAME = 32  # pass 1 of apg_reduce runs at most this many CTAs per latent frame
+
+
+def apg_partials_len(frames):
+    """fp32 partials apg_reduce needs for a latent of `frames` frames: 3 sums per CTA."""
+    return 3 * frames * APG_MAX_CTAS_PER_FRAME
+
+
+def _apg_operands(x, v, delta, forecast):
+    """(form, delta pointer, delta stride, n_dslots, ctypes coefficients or None, frames) of an APG launch on x [1, T, ...]
+    fp32 with u and c as cfg_zero_scale takes them: v the pair, or c alone with delta or forecast = (slots, coefficients)."""
+    if delta is not None and forecast is not None:
+        raise ValueError("apg: pass delta or forecast, not both")
+    _req(x, torch.float32), _req(v)
+    assert x.is_contiguous() and v.is_contiguous() and x.dim() >= 2 and x.shape[0] == 1, tuple(x.shape)
+    n = x.numel()
+    if forecast is not None:
+        _req(forecast[0], torch.float32)
+        assert v.numel() == n
+        stride, n_d, dk = _delta_forecast(forecast[0], forecast[1], n)
+        return 2, _ptr(forecast[0]), stride, n_d, dk, x.shape[1]
+    if delta is not None:
+        _req(delta, torch.float32)
+        assert v.numel() == n and delta.is_contiguous() and delta.numel() == n
+        return 1, _ptr(delta), 0, 0, None, x.shape[1]
+    assert v.numel() == 2 * n
+    return 0, None, 0, 0, None, x.shape[1]
+
+
+def apg_reduce(x, v, sigma, partials, avg=None, momentum=0.0, delta=None, forecast=None):
+    """APG pass 1 on the latent x (fp32 [1, T, ...], one frame per x[0, t]) at the step's sigma: D_c = x - sigma*c,
+    diff = D_c - (x - sigma*u), each product and sum rounded on its own; u and c from the pair v, or from c = v alone with
+    delta or forecast, as cfg_zero_scale forms them.  With avg (fp32, x's shape) avg = diff + momentum*avg in place, and
+    diff = avg.  fp32 partial sums of diff*diff, diff*D_c and D_c*D_c per (frame, CTA) over a partition fixed by the shape
+    -> partials (fp32, at least apg_partials_len(T)).  Bit-reproducible.  Returns partials."""
+    form, dptr, dstride, n_d, dk, frames = _apg_operands(x, v, delta, forecast)
+    _req(partials, torch.float32)
+    assert partials.is_contiguous()
+    if avg is not None:
+        _req(avg, torch.float32)
+        assert avg.is_contiguous() and avg.numel() == x.numel()
+    _lib.check(_lib.lib().scail_apg_reduce(form, _ptr(x), _ptr(v), dptr, dstride, n_d,
+                                           None if dk is None else ctypes.addressof(dk), _ptr(avg), float(sigma),
+                                           float(momentum), _ptr(partials), partials.numel(), frames, x.numel(), _stream()),
+               "scail_apg_reduce")
+    _count()
+    return partials
+
+
+def apg_finish(partials, sums, factors, norm_threshold, frames, n):
+    """APG pass 2: per frame, the partials of apg_reduce on a latent of n elements in `frames` frames added in fp64 in a fixed
+    order -> sums (fp64 [frames, 4]) = (|diff|^2, <diff, D_c>, |D_c|^2, 0) and factors (fp32 [frames, 2]) = (f, p), computed
+    in fp64 and rounded once: f = r / |diff| if r = norm_threshold > 0 and |diff| > r, else 1; p = f <diff, D_c> / |D_c|^2,
+    0 for |D_c| = 0.  Returns factors."""
+    _req(partials, torch.float32), _req(sums, torch.float64), _req(factors, torch.float32)
+    assert sums.is_contiguous() and sums.numel() >= 4 * frames and factors.is_contiguous() and factors.numel() >= 2 * frames
+    _lib.check(_lib.lib().scail_apg_finish(_ptr(partials), partials.numel(), _ptr(sums), _ptr(factors), float(norm_threshold),
+                                           int(frames), int(n), _stream()), "scail_apg_finish")
+    _count()
+    return factors
+
+
+def apg_update_(x, v, factors, scale, eta, sigma, next_sigma=None, out=None, avg=None, delta=None, forecast=None):
+    """The APG update of x (fp32 [1, T, ...]) with the per-frame factors (f, p) of apg_finish: D_c and diff as apg_reduce
+    forms them (diff = avg, the average apg_reduce wrote, when avg is given); par = p*D_c; orth = f*diff - par; D_g = D_c +
+    (scale - 1)*(orth + eta*par), each product and sum rounded on its own.  With out (fp32, x's shape) D_g -> out and x is
+    left as it is; else the Euler step x = x + k*(x - D_g) in place, k = (next_sigma - sigma) / sigma (fp64, rounded once).
+    scale - 1 is likewise formed in fp64 and rounded once.  Returns out, or x."""
+    form, dptr, dstride, n_d, dk, frames = _apg_operands(x, v, delta, forecast)
+    _req(factors, torch.float32)
+    assert factors.is_contiguous() and factors.numel() >= 2 * frames
+    if avg is not None:
+        _req(avg, torch.float32)
+        assert avg.is_contiguous() and avg.numel() == x.numel()
+    if out is not None:
+        _req(out, torch.float32)
+        assert out.is_contiguous() and out.numel() == x.numel()
+        k = 0.0
+    else:
+        k = (float(next_sigma) - float(sigma)) / float(sigma)
+    _lib.check(_lib.lib().scail_apg_update(form, _ptr(x), _ptr(v), dptr, dstride, n_d,
+                                           None if dk is None else ctypes.addressof(dk), _ptr(avg), _ptr(factors), _ptr(out),
+                                           float(sigma), float(scale) - 1.0, float(eta), k, frames, x.numel(), _stream()),
+               "scail_apg_update")
+    _count()
+    return x if out is None else out
+
+
+def unipc_step_dpred_(x, x_last, m, slots, write_slot, coef, correct):
+    """unipc_step_ with the data prediction m (fp32, x's shape: APG's D_g) read in place of x - sigma*g; every later
+    instruction is the same.  Returns x."""
+    _req(x, torch.float32), _req(x_last, torch.float32), _req(m, torch.float32), _req(slots, torch.float32)
+    assert x.is_contiguous() and x_last.is_contiguous() and x_last.shape == x.shape
+    assert m.is_contiguous() and m.numel() == x.numel()
+    assert slots.dim() == 2 and slots.is_contiguous() and slots.shape[1] == x.numel(), tuple(slots.shape)
+    assert len(coef) == 10
+    c = (ctypes.c_float * 10)(*coef)
+    _lib.check(_lib.lib().scail_unipc_step_dpred(_ptr(x), _ptr(x_last), _ptr(m), _ptr(slots), slots.stride(0), slots.shape[0],
+                                                 int(write_slot), x.numel(), int(bool(correct)), ctypes.addressof(c),
+                                                 _stream()), "scail_unipc_step_dpred")
+    _count()
+    return x
+
+
 # ---------------------------------------------------------------- first-block residual cache (scail_b200.step_cache)
 STEP_CACHE_PARTIALS = 2048  # fp32 partial sums of step_cache_indicator: 2 per CTA, at most 1024 CTAs
 

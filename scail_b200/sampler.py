@@ -63,10 +63,12 @@ def sampler_step(model, x, sigma, next_sigma, cond, uc, scale=4.0, _ctx=None, pl
     cfg_cache: an optional scail_b200.cfg_cache.CFGCache (single GPU only).  It decides before the forward whether this step
     runs the conditional branch alone (b = 1, on the cache's stream) and rebuilds u = c - delta for the update (delta
     forecast at this step's sigma when the cache's order is >= 1); the first-block cache then sits the step out.
-    guidance: an optional scail_b200.guidance.CFGZeroStar (not under context parallelism or chunk_dim).  It counts this
-    step first: a zero-initialised step runs no forward and tells neither cache about it, leaves x as it is with Euler and
-    runs the solver on a zero CFG pair; any other step scales u by s*, reduced on the device from the pair (or from the CFG
-    cache's rebuilt u), before the combine.  (guided_velocity does not count steps: it applies s* only.)"""
+    guidance: an optional scail_b200.guidance.CFGZeroStar or APG (not under context parallelism or chunk_dim).  It counts
+    this step first: a zero-initialised step runs no forward and tells neither cache about it, leaves x as it is with Euler
+    and runs the solver on a zero CFG pair; any other step scales u by s*, reduced on the device from the pair (or from the
+    CFG cache's rebuilt u), before the combine.  (guided_velocity does not count steps: it applies s* only.)  An APG step
+    reduces its per-frame factors on the device from the same u and c and replaces the combine by its data-prediction rule:
+    the Euler step, or the solver's step on D_g."""
     _check_cfg_cache(model, cfg_cache, plan, model_kwargs)
     _check_guidance(model, guidance, model_kwargs)
     if solver is not None:
@@ -113,7 +115,8 @@ def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=No
     solver (a scail_b200.unipc.UniPC) is bound to this call's schedule here and replaces the Euler update on every step.
     cfg_cache (a scail_b200.cfg_cache.CFGCache) is reset here and then decides on every step whether only the conditional
     branch runs; with cache_cross_kv that forward reads the cond row of this call's conditioning.  guidance (a
-    scail_b200.guidance.CFGZeroStar) is reset here; its first zero_init_steps steps run no forward."""
+    scail_b200.guidance.CFGZeroStar or APG) is reset here; a CFGZeroStar's first zero_init_steps steps run no forward, and
+    an APG's momentum starts from zero."""
     _check_cfg_cache(model, cfg_cache, plan)
     _check_guidance(model, guidance)
     if guidance is not None:
@@ -144,7 +147,12 @@ def sample(model, x, cond, uc, num_steps=50, shift_scale=5.0, scale=4.0, plan=No
 def guided_velocity(model, x, sigma, cond, uc, scale=4.0, ctx=None, plan=None, guidance=None):
     """RFSampler.denoise (sampling.py:945-953): CFG batch-2 forward + `u + s (c - u)` -> fp32 guided velocity [1,t,16,h,w]
     (the fused CFG+Euler kernel applied to a zero latent with d_sigma = 1).  With guidance (a CFGZeroStar), u is scaled by
-    this call's own s* (the scaled kernel); zero-init is the caller's decision (sample_long), so no step is counted."""
+    this call's own s* (the scaled kernel); zero-init is the caller's decision (sample_long), so no step is counted.  An
+    APG is refused (NotImplementedError): its rule needs the step's latent and sigma, and this call runs on a zero latent."""
+    _check_guidance(model, guidance)
+    if isinstance(guidance, gd.APG):
+        raise NotImplementedError("guided_velocity does not take an APG guidance: its data predictions need the step's "
+                                  "latent, and guided_velocity accumulates into a zero latent; use sampler_step")
     return sampler_step(model, torch.zeros_like(x), 0.0, 1.0, cond, uc, scale, _ctx=ctx, plan=plan, _x_override=x, _sigma_override=sigma,
                         guidance=guidance)
 
@@ -195,8 +203,12 @@ def sample_long(model, x, cond, uc, tile_indices, num_steps=50, shift_scale=5.0,
     cond['smpl_tiled'] [1, n_tiles, segment, 16, h/2, w/2] holds the pose render of every window; `tile_indices` lists the
     latent-frame indices of every window (equal lengths).  `denoise` overrides the network call (tests).
     guidance (a scail_b200.guidance.CFGZeroStar) is reset here.  On a zero-initialised step every window's velocity is zero,
-    so the whole step is skipped and x is unchanged; on every other step each window's guided_velocity uses its own s*."""
+    so the whole step is skipped and x is unchanged; on every other step each window's guided_velocity uses its own s*.
+    An APG is refused (NotImplementedError): its momentum would need state per window."""
     _check_guidance(model, guidance)
+    if isinstance(guidance, gd.APG):
+        raise NotImplementedError("sample_long does not take an APG guidance: its momentum average would need state per "
+                                  "window, and each window would need its own per-frame sums; use CFGZeroStar or None")
     if guidance is not None:
         guidance.reset()
     sig = make_flow_timesteps(num_steps, shift_scale).to(x.device)
@@ -240,9 +252,10 @@ class GraphedStep:
     before each step which graphs replay.  Every graph's workspace tensors are held here (_workspace_of).  The delta kernel and the updates run eagerly after the replay (delta_ref and delta_new
     alternate between two buffers, which a graph would fix; at order >= 1 the forecast coefficients are kernel arguments
     computed from each step's sigma, so no graph depends on them either).
-    guidance (a scail_b200.guidance.CFGZeroStar, reset at construction): a zero-initialised step replays nothing and runs
-    only the solver's step on a zero pair, if there is a solver; on any other step the reduction of s* and the scaled
-    update run eagerly after the replay, and s* stays on the device, so no graph depends on it."""
+    guidance (a scail_b200.guidance.CFGZeroStar or APG, reset at construction): a zero-initialised step replays nothing and
+    runs only the solver's step on a zero pair, if there is a solver; on any other step the reduction of s* and the scaled
+    update run eagerly after the replay, and s* stays on the device, so no graph depends on it.  An APG's reductions and
+    update run eagerly after the replay in the same way, with sigma and its coefficients as kernel arguments."""
 
     def __init__(self, model, x, cond, uc, scale=4.0, step_cache=None, solver=None, cfg_cache=None, guidance=None):
         _check_cfg_cache(model, cfg_cache)

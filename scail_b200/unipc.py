@@ -226,15 +226,19 @@ class UniPC:
             raise ValueError(f"solver: the latent {tuple(x.shape)} {x.dtype} on {x.device} is not the latent "
                              f"{self._key[0]} {self._key[1]} on {self._key[2]} the solver's state was built for")
 
-    def step(self, x, v, scale, sigma, next_sigma, delta=None, forecast=None, u_scale=None):
+    def step(self, x, v, scale, sigma, next_sigma, delta=None, forecast=None, u_scale=None, m=None):
         """One solver step in place on x (fp32), from the CFG pair v (bf16 [2, ...], as cfg_euler_ reads it).  With `delta`
         (fp32, x's element count: a scail_b200.cfg_cache.CFGCache's held c - u), v is the conditional output alone (bf16
         [1, ...]) and u = f32(c) - delta; the coefficients and the state are those of the pair step.  `forecast` takes the
         place of delta for a CFGCache of order >= 1: (slots, coefficients), delta_hat = c0*S0 + c1*S1 + c2*S2 as
         ops.cfg_cache_delta_forecast forms it, and u = f32(c) - delta_hat.  u_scale (fp32 [1] on the device, from
-        scail_b200.guidance.CFGZeroStar) scales u by s* before the guided combine.  Returns x."""
+        scail_b200.guidance.CFGZeroStar) scales u by s* before the guided combine.  With m (fp32, x's element count: the data
+        prediction of scail_b200.guidance.APG), v and scale are not used and m takes the place of x - sigma*g; the coefficients,
+        the slots and everything after m are the same.  Returns x."""
         if delta is not None and forecast is not None:
             raise ValueError("solver: pass delta or forecast, not both")
+        if m is not None and (delta is not None or forecast is not None or u_scale is not None):
+            raise ValueError("solver: a data prediction m takes no delta, forecast or u_scale")
         self.check_step(x, sigma, next_sigma)
         i = self._i
         if i == 0:
@@ -250,7 +254,9 @@ class UniPC:
         coef = [k.x_last_c, *k.slot_c, *pad, k.m_c, k.y_c, *k.slot_p, *pad, k.m_p]
         coef = [_f32(c) for c in coef]
         kw = {} if u_scale is None else dict(u_scale=u_scale)
-        if forecast is not None:
+        if m is not None:
+            ops.unipc_step_dpred_(x, self.x_last, m, self.slots, k.write, coef, k.correct)
+        elif forecast is not None:
             ops.unipc_step_cached_forecast_(x, self.x_last, v, *forecast, self.slots, k.write, scale, self._sigmas[i], coef,
                                             k.correct, **kw)
         elif delta is None:
