@@ -149,12 +149,43 @@ int scail_attention_fp8_sparse_bh(const void* Q, int64_t ldq, const float* q_sca
                                   const float* k_scale, const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B,
                                   int64_t H, int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
                                   int64_t ptr_stride, const int32_t* kv_tile_idx, int64_t idx_stride, scail_stream_t stream);
+/* fp8_attention="int8_qk": the INT8 row format is s = amax / 127 (IEEE division), q = round-half-even(x / s) saturated to
+ * [-127, 127], s = 1 for an all-zero row; one row = one 128-wide head of one token.
+ * RMSNorm(+RoPE) as scail_rmsnorm_rope over two slabs (nslabs must be 2): slab 0 (Q) goes to INT8 rows q8 [rows, ld8] with
+ * scales q_scale head-major [B, D/128, L_pad] (zeros past rows_per_batch), equal bit for bit to quantising what
+ * scail_rmsnorm_rope writes; slab 1 (K) is written back into buf in bf16 exactly as scail_rmsnorm_rope writes it.
+ * D % 128 == 0, ld8 % 16 == 0, rows_per_batch <= L_pad, L_pad % 128 == 0. */
+int scail_rmsnorm_rope_int8q(void* buf, int64_t ld, int64_t rows, int64_t rows_per_batch, int64_t D, int nslabs,
+                             int64_t col_offset0, const void* weight0, int64_t col_offset1, const void* weight1,
+                             const float* cos, const float* sin, float eps, void* q8, float* q_scale, int64_t ld8, int64_t L_pad,
+                             scail_stream_t stream);
+/* Smoothed INT8 K: K bf16 [B*L, H*128] (column slab, leading dim ldk) -> kbar float32 [B, H*128], the mean over the L keys
+ * of each batch element (summed in fp64 over fixed 256-key chunks, chunks added in ascending order, divided by L in fp64,
+ * rounded once to fp32), and K' = f32(k) - kbar (one fp32 rounding) in the INT8 row format: k8 [B*L, ld8], k_scale
+ * [B, H, L_pad] with zeros past L.  partial: fp64 workspace of partial_len >= B*ceil(L/256)*H*128 entries.
+ * Three launches, no atomics and no host reads: bit-reproducible and capturable in a CUDA graph.  L <= L_pad, L_pad % 128 == 0,
+ * H*128 <= 5120. */
+int scail_quant_k_int8(const void* k, int64_t ldk, void* k8, int64_t ld8, float* k_scale, float* kbar, double* partial,
+                       int64_t partial_len, int64_t B, int64_t H, int64_t L, int64_t L_pad, scail_stream_t stream);
+/* Self-attention with INT8 Q and K (scail_rmsnorm_rope_int8q, scail_quant_k_int8) and the e4m3 V^T of scail_quant_vt_fp8:
+ * S = Q K^T in exact s32, then as scail_attention_fp8.  kv_tile_ptr NULL: dense.  Otherwise a block-sparse map as
+ * scail_attention_sparse_bh with ptr_stride / idx_stride per (batch, head), or both 0 for one map shared by every (batch,
+ * head); its contents are trusted (the host checks pointers, alignment and strides). */
+int scail_attention_int8qk(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                           const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H, int64_t head_dim,
+                           int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr, int64_t ptr_stride,
+                           const int32_t* kv_tile_idx, int64_t idx_stride, scail_stream_t stream);
 /* Tile pooling for adaptive tile selection: out fp32 [B, H, ceil(L/128), 128] = the mean over each 128-row tile's valid rows
  * of one self-attention operand, x [B*L, ldx] with head h at columns [h*128, h*128+128).  fp8 == 0: x is bf16 and x_scale
  * NULL.  fp8 == 1: x is e4m3 and the value is x * x_scale[b, h, row] with x_scale fp32 [B, H, L_pad]
  * (scail_rmsnorm_rope_fp8).  Summed in ascending row order in fp64: bit-reproducible. */
 int scail_attention_tile_pool(const void* x, int64_t ldx, const float* x_scale, int fp8, float* out, int64_t B, int64_t H,
                               int64_t L, int64_t L_pad, scail_stream_t stream);
+/* scail_attention_tile_pool of an INT8 operand (fp8_attention="int8_qk": scail_rmsnorm_rope_int8q, scail_quant_k_int8): the
+ * value is x * x_scale[b, h, row], x int8 [B*L, ldx], x_scale fp32 [B, H, L_pad].  Pooling the smoothed K' instead of K
+ * shifts every s_k of one query tile by the same amount, so the selection does not change. */
+int scail_attention_tile_pool_int8(const void* x, int64_t ldx, const float* x_scale, float* out, int64_t B, int64_t H, int64_t L,
+                                   int64_t L_pad, scail_stream_t stream);
 /* Adaptive tile selection on the device.  qbar, kbar fp32 [B, H, n, 128] (scail_attention_tile_pool), n = ceil(L/128).
  * Query tile q of (b, h) lists the key tiles with e_k = n_k exp(s_k - max s), s_k = qbar_q . kbar_k / sqrt(128), n_k the
  * valid keys of tile k: always k == q and every k < ceil(n_ref/128) (reference tokens), then the others by e_k descending

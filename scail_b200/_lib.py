@@ -46,6 +46,12 @@ SIGNATURES = {
     "scail_attention_fp8_sparse_bh": [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64,
                                       c_i64, c_f, c_p, c_i64, c_p, c_i64, c_p],
     "scail_attention_tile_pool": [c_p, c_i64, c_p, c_int, c_p, c_i64, c_i64, c_i64, c_i64, c_p],
+    "scail_rmsnorm_rope_int8q": [c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_f, c_p, c_p, c_i64,
+                                 c_i64, c_p],
+    "scail_quant_k_int8": [c_p, c_i64, c_p, c_i64, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_p],
+    "scail_attention_tile_pool_int8": [c_p, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_p],
+    "scail_attention_int8qk": [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f,
+                               c_p, c_i64, c_p, c_i64, c_p],
     "scail_attention_select_tiles": [c_p, c_p, c_i64, c_i64, c_i64, c_i64, ctypes.c_double, c_i64, c_p, c_i64, c_p, c_i64,
                                      c_p, c_i64, c_p],
     "scail_attention_partial": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,

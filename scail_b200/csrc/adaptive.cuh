@@ -1,7 +1,7 @@
 // Content-adaptive block-sparse self-attention (scail_b200/sparse.py, AdaptiveTiles): the per-(batch, head) tile maps are
 // chosen on the device, per forward, from tile-pooled Q and K, so the whole selection can be captured in a CUDA graph.
 //   tile_pool_kernel      : Qbar or Kbar [B, H, n_t, 128] fp32 = the mean of each 128-row tile's valid rows (bf16 slab, or
-//                           e4m3 slab times its [B, H, L_pad] per-token scales).
+//                           e4m3 or INT8 slab times its [B, H, L_pad] per-token scales).
 //   select_tiles_kernel   : per (b, h, query tile q): s_k = Qbar_q . Kbar_k / sqrt(128), e_k = n_k exp(s_k - max s), keep the
 //                           forced tiles (k == q and the tiles holding reference tokens) plus the largest e_k (ties: lower k)
 //                           until the kept mass reaches `mass` of the total or `max_tiles` were taken; the row goes to a
@@ -20,9 +20,10 @@ constexpr int ADA_SELECT_THREADS = 256;  // 8 warps
 constexpr int ADA_MAX_TILES = 2048;      // select_tiles_kernel keeps 20 bytes per key tile in shared memory: L <= 262144
 
 // One CTA per (tile, head, batch), one thread per channel.  x: [B*L, ld] (head h at columns h*128); scale: null for bf16,
-// else the e4m3 operand's per-token scales [B, H, L_pad].  Rows are summed in ascending order in fp64 (exact products for
-// e4m3 x fp32) and the mean rounded once to fp32.
-template <bool kFp8>
+// else the e4m3 (kInt8: INT8) operand's per-token scales [B, H, L_pad].  Rows are summed in ascending order in fp64 (exact
+// products for e4m3 or int8 x fp32) and the mean rounded once to fp32.  fp8_attention="int8_qk" pools the smoothed K', whose
+// s_k of one query tile all shift by the same -Qbar . k-bar: e_k = n_k exp(s_k - max s) and hence the selection do not change.
+template <bool kFp8, bool kInt8 = false>
 __global__ void __launch_bounds__(ATT_D) tile_pool_kernel(const void* __restrict__ x, int64_t ld, const float* __restrict__ scale,
                                                           float* __restrict__ out, int L, int L_pad, int heads) {
     const int t = blockIdx.x, h = blockIdx.y, b = blockIdx.z, c = threadIdx.x;
@@ -38,7 +39,10 @@ __global__ void __launch_bounds__(ATT_D) tile_pool_kernel(const void* __restrict
             v[i] = 0.0;
             if (i0 + i < n) {
                 const int64_t off = base + static_cast<int64_t>(i0 + i) * ld;
-                if (kFp8) {
+                if (kInt8) {
+                    const int8_t q = static_cast<const int8_t*>(x)[off];
+                    v[i] = static_cast<double>(q) * static_cast<double>(scale[bh * L_pad + r0 + i0 + i]);
+                } else if (kFp8) {
                     __nv_fp8_e4m3 q;
                     q.__x = static_cast<const __nv_fp8_storage_t*>(x)[off];
                     v[i] = static_cast<double>(static_cast<float>(q)) * static_cast<double>(scale[bh * L_pad + r0 + i0 + i]);

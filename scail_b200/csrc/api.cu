@@ -496,6 +496,67 @@ int scail_rmsnorm_rope_fp8(const void* buf, int64_t ld, int64_t rows, int64_t ro
     return 0;
 }
 
+int scail_rmsnorm_rope_int8q(void* buf, int64_t ld, int64_t rows, int64_t rows_per_batch, int64_t D, int nslabs,
+                             int64_t col_offset0, const void* weight0, int64_t col_offset1, const void* weight1,
+                             const float* cos, const float* sin, float eps, void* q8, float* q_scale, int64_t ld8, int64_t L_pad,
+                             scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(nslabs == 2, "rmsnorm_rope_int8q: nslabs=%d must be 2 (slab 0 = Q, slab 1 = K)", nslabs);
+    SCAIL_REQUIRE(buf && weight0 && weight1 && q8 && q_scale, "rmsnorm_rope_int8q: null operand");
+    SCAIL_REQUIRE(D % 128 == 0 && D <= ROW_MAXV * ROW_THREADS * 8, "rmsnorm_rope_int8q: D=%lld must be a multiple of the 128-wide head and <= %d",
+                  (long long)D, ROW_MAXV * ROW_THREADS * 8);
+    SCAIL_REQUIRE(ld % 8 == 0 && col_offset0 % 8 == 0 && col_offset1 % 8 == 0 && aligned16(buf), "rmsnorm_rope_int8q: bad ld/offset");
+    SCAIL_REQUIRE(ld8 % 16 == 0 && ld8 >= D && aligned16(q8) && aligned4(q_scale),
+                  "rmsnorm_rope_int8q: ld8 must be a multiple of 16 and >= D, q8 16-byte and q_scale 4-byte aligned");
+    SCAIL_REQUIRE(rows > 0 && rows_per_batch > 0 && rows % rows_per_batch == 0, "rmsnorm_rope_int8q: bad row counts");
+    SCAIL_REQUIRE(L_pad % 128 == 0 && rows_per_batch <= L_pad, "rmsnorm_rope_int8q: L_pad=%lld must be a multiple of 128 and >= L=%lld",
+                  (long long)L_pad, (long long)rows_per_batch);
+    SCAIL_REQUIRE((cos == nullptr) == (sin == nullptr), "rmsnorm_rope_int8q: cos/sin come in pairs");
+    RmsRopeParams p;
+    p.buf = static_cast<__nv_bfloat16*>(buf); p.ld = ld;
+    p.col_offset[0] = (int)col_offset0; p.col_offset[1] = (int)col_offset1;
+    p.weight[0] = static_cast<const __nv_bfloat16*>(weight0); p.weight[1] = static_cast<const __nv_bfloat16*>(weight1);
+    p.nslabs = 2; p.D = (int)D; p.rows = (int)rows; p.rows_per_batch = (int)rows_per_batch;
+    p.cos = cos; p.sin = sin; p.eps = eps;
+    p.q8[0] = static_cast<uint8_t*>(q8); p.q8[1] = nullptr;
+    p.s8[0] = q_scale; p.s8[1] = nullptr; p.ld8 = ld8; p.L_pad = (int)L_pad;
+    dim3 grid((unsigned)rows, 2);
+    rmsnorm_rope_kernel<false, true><<<grid, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_quant_k_int8(const void* k, int64_t ldk, void* k8, int64_t ld8, float* k_scale, float* kbar, double* partial,
+                       int64_t partial_len, int64_t B, int64_t H, int64_t L, int64_t L_pad, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(k && k8 && k_scale && kbar && partial, "quant_k_int8: null operand");
+    const int64_t need = B * ((L + KMEAN_ROWS - 1) / KMEAN_ROWS) * H * ATT_D;
+    SCAIL_REQUIRE(partial_len >= need, "quant_k_int8: partial_len=%lld must be >= B*ceil(L/256)*H*128 = %lld", (long long)partial_len,
+                  (long long)need);
+    SCAIL_REQUIRE(B > 0 && H > 0 && L > 0 && L_pad % 128 == 0 && L <= L_pad && B <= 65535,
+                  "quant_k_int8: bad shape B=%lld H=%lld L=%lld L_pad=%lld (L <= L_pad, L_pad %% 128 == 0)", (long long)B,
+                  (long long)H, (long long)L, (long long)L_pad);
+    SCAIL_REQUIRE(H * ATT_D <= ROW_MAXV * ROW_THREADS * 8, "quant_k_int8: H*128=%lld must be <= %d", (long long)(H * ATT_D),
+                  ROW_MAXV * ROW_THREADS * 8);
+    SCAIL_REQUIRE(ldk % 8 == 0 && ldk >= H * ATT_D && ld8 % 16 == 0 && ld8 >= H * ATT_D,
+                  "quant_k_int8: ldk must be a multiple of 8 and ld8 of 16, both >= H*128");
+    SCAIL_REQUIRE(aligned16(k) && aligned16(k8) && aligned16(kbar) && aligned4(k_scale) && (reinterpret_cast<uintptr_t>(partial) & 7) == 0,
+                  "quant_k_int8: k, k8 and kbar must be 16-byte aligned, k_scale 4-byte, partial 8-byte");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int D = (int)(H * ATT_D);
+    const unsigned n_chunks = blocks_for(L, KMEAN_ROWS);
+    dim3 gp(n_chunks, (unsigned)B, blocks_for(D, 128 * 8));
+    k_mean_partial_kernel<<<gp, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(k), ldk, partial, (int)L, D);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    dim3 gf(blocks_for(D, 128), (unsigned)B);
+    k_mean_finish_kernel<<<gf, 128, 0, st>>>(partial, kbar, (int)n_chunks, (int)L, D);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    quant_k_int8_kernel<<<(unsigned)(B * L), ROW_THREADS, 0, st>>>(static_cast<const __nv_bfloat16*>(k), ldk, kbar,
+                                                                    static_cast<int8_t*>(k8), ld8, k_scale, (int)L, (int)L_pad, D);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 int scail_quant_vt_fp8(const void* v, int64_t ldv, void* vt, float* v_scale, void* amax_work, int64_t B, int64_t H,
                        int64_t head_dim, int64_t L, int64_t L_pad, scail_stream_t stream) {
     using namespace scail;
@@ -533,21 +594,36 @@ static int check_tile_map(const char* what, const int32_t* kv_tile_ptr, const in
     return 0;
 }
 
+// attention_fp8_kernel<sparse, int8qk>, one of its four instantiations
+static int launch_attention_fp8(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const scail::Attn8Params& p,
+                                dim3 grid, bool sparse, bool int8qk, cudaStream_t st) {
+    using namespace scail;
+    int rc;
+    auto kernel = sparse ? (int8qk ? attention_fp8_kernel<true, true> : attention_fp8_kernel<true, false>)
+                         : (int8qk ? attention_fp8_kernel<false, true> : attention_fp8_kernel<false, false>);
+    if ((rc = set_smem(kernel, ATT8_SMEM_BYTES))) return rc;
+    kernel<<<grid, ATT_THREADS, ATT8_SMEM_BYTES, st>>>(tq, tk, tv, p);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// int8qk: Q and K are INT8 (attention_fp8_kernel<., true>); `what` names the entry point in the messages
 static int attention_fp8_impl(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
                               const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H,
                               int64_t head_dim, int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr,
-                              const int32_t* kv_tile_idx, scail_stream_t stream, int64_t ptr_stride = 0, int64_t idx_stride = 0) {
+                              const int32_t* kv_tile_idx, scail_stream_t stream, int64_t ptr_stride = 0, int64_t idx_stride = 0,
+                              bool int8qk = false, const char* what = "attention_fp8") {
     using namespace scail;
-    SCAIL_REQUIRE(Q && q_scale && K && k_scale && vt && v_scale && out, "attention_fp8: null operand");
-    SCAIL_REQUIRE(head_dim == ATT_D, "attention_fp8: head_dim=%lld, only 128 is supported", (long long)head_dim);
+    SCAIL_REQUIRE(Q && q_scale && K && k_scale && vt && v_scale && out, "%s: null operand", what);
+    SCAIL_REQUIRE(head_dim == ATT_D, "%s: head_dim=%lld, only 128 is supported", what, (long long)head_dim);
     SCAIL_REQUIRE(B > 0 && H > 0 && L > 0 && L_pad % 128 == 0 && L <= L_pad,
-                  "attention_fp8: bad shape B=%lld H=%lld L=%lld L_pad=%lld (L <= L_pad, L_pad %% 128 == 0)", (long long)B,
+                  "%s: bad shape B=%lld H=%lld L=%lld L_pad=%lld (L <= L_pad, L_pad %% 128 == 0)", what, (long long)B,
                   (long long)H, (long long)L, (long long)L_pad);
     SCAIL_REQUIRE(ldq % 16 == 0 && ldk % 16 == 0 && ldq >= H * ATT_D && ldk >= H * ATT_D && ldo % 8 == 0 && ldo >= H * ATT_D,
-                  "attention_fp8: ldq and ldk must be multiples of 16, ldo of 8, all >= H*128");
+                  "%s: ldq and ldk must be multiples of 16, ldo of 8, all >= H*128", what);
     SCAIL_REQUIRE(aligned16(Q) && aligned16(K) && aligned16(vt) && aligned16(out) && aligned16(k_scale) && aligned4(q_scale) &&
                       (reinterpret_cast<uintptr_t>(v_scale) & 7) == 0,
-                  "attention_fp8: Q, K, vt, out and k_scale must be 16-byte aligned, v_scale 8-byte, q_scale 4-byte");
+                  "%s: Q, K, vt, out and k_scale must be 16-byte aligned, v_scale 8-byte, q_scale 4-byte", what);
     CUtensorMap tq, tk, tv;
     int rc;
     const uint64_t cols = (uint64_t)H * ATT_D;
@@ -563,15 +639,7 @@ static int attention_fp8_impl(const void* Q, int64_t ldq, const float* q_scale, 
     p.ptr_stride = ptr_stride; p.idx_stride = idx_stride;
     dim3 grid((unsigned)(L_pad / ATT_BQ), (unsigned)H, (unsigned)B);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (kv_tile_ptr) {
-        if ((rc = set_smem(attention_fp8_kernel<true>, ATT8_SMEM_BYTES))) return rc;
-        attention_fp8_kernel<true><<<grid, ATT_THREADS, ATT8_SMEM_BYTES, st>>>(tq, tk, tv, p);
-    } else {
-        if ((rc = set_smem(attention_fp8_kernel<false>, ATT8_SMEM_BYTES))) return rc;
-        attention_fp8_kernel<false><<<grid, ATT_THREADS, ATT8_SMEM_BYTES, st>>>(tq, tk, tv, p);
-    }
-    SCAIL_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return launch_attention_fp8(tq, tk, tv, p, grid, kv_tile_ptr != nullptr, int8qk, st);
 }
 
 int scail_attention_fp8(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
@@ -690,6 +758,24 @@ int scail_attention_fp8_sparse_bh(const void* Q, int64_t ldq, const float* q_sca
                               kv_tile_ptr, kv_tile_idx, stream, ptr_stride, idx_stride);
 }
 
+int scail_attention_int8qk(const void* Q, int64_t ldq, const float* q_scale, const void* K, int64_t ldk, const float* k_scale,
+                           const void* vt, const float* v_scale, void* out, int64_t ldo, int64_t B, int64_t H, int64_t head_dim,
+                           int64_t L, int64_t L_pad, float scale, const int32_t* kv_tile_ptr, int64_t ptr_stride,
+                           const int32_t* kv_tile_idx, int64_t idx_stride, scail_stream_t stream) {
+    int rc;
+    if (kv_tile_ptr || kv_tile_idx) {
+        SCAIL_REQUIRE(kv_tile_ptr && kv_tile_idx, "attention_int8qk: kv_tile_ptr and kv_tile_idx come together (both null: dense)");
+        SCAIL_REQUIRE((ptr_stride == 0) == (idx_stride == 0), "attention_int8qk: ptr_stride and idx_stride are both 0 (one shared map) or both set");
+        if (ptr_stride != 0) {
+            if ((rc = check_bh_maps("attention_int8qk", kv_tile_ptr, ptr_stride, kv_tile_idx, idx_stride, L))) return rc;
+        } else {
+            SCAIL_REQUIRE(aligned4(kv_tile_ptr) && aligned4(kv_tile_idx), "attention_int8qk: kv_tile_ptr and kv_tile_idx must be 4-byte aligned int32");
+        }
+    }
+    return attention_fp8_impl(Q, ldq, q_scale, K, ldk, k_scale, vt, v_scale, out, ldo, B, H, head_dim, L, L_pad, scale,
+                              kv_tile_ptr, kv_tile_idx, stream, ptr_stride, idx_stride, true, "attention_int8qk");
+}
+
 int scail_attention_tile_pool(const void* x, int64_t ldx, const float* x_scale, int fp8, float* out, int64_t B, int64_t H,
                               int64_t L, int64_t L_pad, scail_stream_t stream) {
     using namespace scail;
@@ -707,6 +793,23 @@ int scail_attention_tile_pool(const void* x, int64_t ldx, const float* x_scale, 
     dim3 grid(blocks_for(L, ATT_BKV), (unsigned)H, (unsigned)B);
     if (fp8) tile_pool_kernel<true><<<grid, ATT_D, 0, st>>>(x, ldx, x_scale, out, (int)L, (int)L_pad, (int)H);
     else tile_pool_kernel<false><<<grid, ATT_D, 0, st>>>(x, ldx, nullptr, out, (int)L, 0, (int)H);
+    SCAIL_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int scail_attention_tile_pool_int8(const void* x, int64_t ldx, const float* x_scale, float* out, int64_t B, int64_t H, int64_t L,
+                                   int64_t L_pad, scail_stream_t stream) {
+    using namespace scail;
+    SCAIL_REQUIRE(x && x_scale && out, "attention_tile_pool_int8: null operand");
+    SCAIL_REQUIRE(B > 0 && H > 0 && L > 0 && B <= 65535 && H <= 65535,
+                  "attention_tile_pool_int8: bad shape B=%lld H=%lld L=%lld", (long long)B, (long long)H, (long long)L);
+    SCAIL_REQUIRE(ldx >= H * ATT_D, "attention_tile_pool_int8: ldx=%lld must be >= H*128 = %lld", (long long)ldx, (long long)(H * ATT_D));
+    SCAIL_REQUIRE(L_pad % 128 == 0 && L <= L_pad, "attention_tile_pool_int8: L_pad=%lld must be a multiple of 128 and >= L=%lld",
+                  (long long)L_pad, (long long)L);
+    SCAIL_REQUIRE(aligned4(out) && aligned4(x_scale), "attention_tile_pool_int8: out and x_scale must be 4-byte aligned");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    dim3 grid(blocks_for(L, ATT_BKV), (unsigned)H, (unsigned)B);
+    tile_pool_kernel<false, true><<<grid, ATT_D, 0, st>>>(x, ldx, x_scale, out, (int)L, (int)L_pad, (int)H);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -327,7 +327,12 @@ struct Attn8Params {
 
 // kSparse: the block-sparse map selects the CTA's key tiles, as in attention_fwd_kernel<true>; tile j's K rows, K scales
 // and V^T columns start at key 128 kv_tile_idx[j].
-template <bool kSparse>
+// kInt8QK (fp8_attention="int8_qk"): Q and K are INT8 codes in [-127, 127] with the same per-(token, head) scales (the INT8
+// row format of rowops.cuh; K smoothed by its per-(batch, channel) mean first, quant_k_int8), and S = Q K^T runs as
+// wgmma m64n128k32 s8 x 4 into s32.  V^, P^ and everything after S are unchanged.  Subtracting k-bar from every key shifts
+// each logit of a query row by the same q . k-bar, which the softmax cancels, so the listed tiles of a sparse map need no
+// correction either.
+template <bool kSparse, bool kInt8QK = false>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                      const __grid_constant__ CUtensorMap tmap_vt, const Attn8Params p) {
@@ -424,12 +429,28 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
             float sc[ATT_BKV / 2];
             mbar_wait(bar(B_KFULL + s), par, 21);
             const uint64_t k_desc = wgmma_desc_kmajor_sw128(k_smem + s * ATT8_TILE_BYTES);
-            wgmma_fence();
+            if constexpr (kInt8QK) {
+                // s32 accumulator started at the bits of 1.5 * 2^23: |S| < 2^22 keeps the sum inside [2^23, 2^24), where the
+                // bits read as the float 1.5 * 2^23 + S exactly, so one exact FADD converts it (no I2F)
+                uint32_t si[ATT_BKV / 2];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) wgmma_ss_e4m3<ATT_BKV>(sc, q_desc + 2 * k, k_desc + 2 * k, k != 0);
-            wgmma_commit();
-            wgmma_wait<0>();
-            fence_regs(sc);
+                for (int i = 0; i < ATT_BKV / 2; ++i) si[i] = 0x4B400000u;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_ss_s8<ATT_BKV>(si, q_desc + 2 * k, k_desc + 2 * k);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(si);
+#pragma unroll
+                for (int i = 0; i < ATT_BKV / 2; ++i) sc[i] = __fsub_rn(__uint_as_float(si[i]), 12582912.0f);
+            } else {
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_ss_e4m3<ATT_BKV>(sc, q_desc + 2 * k, k_desc + 2 * k, k != 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(sc);
+            }
             // K scales of this thread's columns 8c + 2 quad + {0, 1}
             const uint32_t ksa = ks_smem + s * ATT8_KS_BYTES + 8 * quad;
 #pragma unroll

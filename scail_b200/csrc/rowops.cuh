@@ -63,6 +63,35 @@ __device__ __forceinline__ uint2 quant_bf16x8(const uint4 v, float s) {
     return make_uint2(h[0] | (h[1] << 16), h[2] | (h[3] << 16));
 }
 
+// ---- INT8 row format of fp8_attention="int8_qk" (Q and smoothed K): s = amax(|row|) / 127 (IEEE division),
+// q = cvt.rni.sat.s8(x / s) in [-127, 127]; an all-zero row gets s = 1 and q = 0.
+// torch: torch.round(x.float() / s[:, None]).clamp(-127, 127).to(torch.int8)  (round-half-even, as cvt.rni)
+constexpr float INT8_QMAX = 127.0f;
+
+__device__ __forceinline__ float int8_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, INT8_QMAX) : 1.0f; }
+// 8 fp32 -> 8 int8 codes
+__device__ __forceinline__ uint2 quant_f32x8_s8(const float (&f)[8], float s) {
+    uint32_t w[2] = {0u, 0u};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int q = max(-127, min(127, __float2int_rn(__fdiv_rn(f[i], s))));
+        w[i >> 2] |= (static_cast<uint32_t>(q) & 0xffu) << (8 * (i & 3));
+    }
+    return make_uint2(w[0], w[1]);
+}
+// 8 bf16 -> 8 int8 codes
+__device__ __forceinline__ uint2 quant_bf16x8_s8(const uint4 v, float s) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    float f[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float2 x = unpack_bf16(w[k]);
+        f[2 * k] = x.x;
+        f[2 * k + 1] = x.y;
+    }
+    return quant_f32x8_s8(f, s);
+}
+
 // One 128-thread block per row of a row-strided bf16 [M, K] (K % 16 == 0, K <= 8 * ROW_THREADS * V): the row stays in registers
 // between the amax reduction and the quantisation, so it is read once.
 template <int V>
@@ -251,7 +280,9 @@ struct RmsRopeParams {
 // FP8: the bf16 row the bf16 form would write is quantised per 128-wide head (the e4m3 row format above, one row = one head of
 // one token), so the result equals quant_rows_fp8 of the bf16 form's heads bit for bit.  A head's 16 vectors are held by 16
 // consecutive lanes (D % 128 == 0), so its amax is four shuffles.
-template <bool FP8>
+// INT8Q (FP8 false): slab 0 (Q) is quantised the same way in the INT8 row format; slab 1 (K) is written back in bf16 in place,
+// exactly as the bf16 form writes it, because its smoothing (quant_k_int8) needs the mean over all keys first.
+template <bool FP8, bool INT8Q = false>
 __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_rope_kernel(const RmsRopeParams p) {
     __shared__ float red[4];
     const int row = blockIdx.x;
@@ -309,10 +340,14 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_rope_kernel(const RmsRope
                 ow[k] = f32x2_to_bf16x2(y);
             }
             if constexpr (FP8) ob[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-            else xin[i] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+            else if constexpr (INT8Q) {
+                if (slab == 0) ob[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+                else xin[i] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+            } else xin[i] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
         }
     }
-    if constexpr (FP8) {
+    if constexpr (FP8 || INT8Q) {
+        if (INT8Q && slab == 1) return;  // the whole block: K went back in bf16
         uint8_t* q8 = (slab ? p.q8[1] : p.q8[0]) + static_cast<int64_t>(row) * p.ld8;
         float* s8 = slab ? p.s8[1] : p.s8[0];
         const int b = row / p.rows_per_batch, tok = row - b * p.rows_per_batch;
@@ -326,13 +361,97 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_rope_kernel(const RmsRope
 #pragma unroll
             for (int o = 1; o < 16; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
             if (i < nvec) {
-                const float s = fp8_row_scale(amax);
-                reinterpret_cast<uint2*>(q8)[i] = quant_bf16x8(ob[j], s);
+                const float s = INT8Q ? int8_row_scale(amax) : fp8_row_scale(amax);
+                reinterpret_cast<uint2*>(q8)[i] = INT8Q ? quant_bf16x8_s8(ob[j], s) : quant_bf16x8(ob[j], s);
                 if ((i & 15) == 0) {
                     float* sh = s8 + (static_cast<int64_t>(b) * heads + (i >> 4)) * p.L_pad;
                     sh[tok] = s;
                     for (int pad = p.rows_per_batch + tok; pad < p.L_pad; pad += p.rows_per_batch) sh[pad] = 0.f;
                 }
+            }
+        }
+    }
+}
+
+// ---- K of fp8_attention="int8_qk": smoothing + INT8 quantisation (scail_quant_k_int8), three launches, no atomics:
+//   k_mean_partial_kernel : per (batch, 256-key chunk, channel) the fp64 sum of the chunk's bf16 keys, in ascending key order;
+//   k_mean_finish_kernel  : k-bar[b, c] = f32((sum of the chunks' partials in ascending chunk order) / L), fp64 throughout;
+//   quant_k_int8_kernel   : K'[row] = __fsub_rn(f32(k), k-bar) in registers, quantised per 128-wide head in the INT8 row
+//                           format: codes [B*L, ld8], scales head-major [B, H, L_pad] with zeros past L.
+// The partition is fixed by the shape, so every launch writes the same bits.
+constexpr int KMEAN_ROWS = 256;  // keys per chunk of the partial sums
+
+// grid (ceil(L / 256), B, ceil(D / 1024)), 128 threads: 8 channels per thread
+__global__ void __launch_bounds__(128) k_mean_partial_kernel(const __nv_bfloat16* k, int64_t ldk, double* partial, int L, int D) {
+    const int b = blockIdx.y;
+    const int col = (blockIdx.z * 128 + threadIdx.x) * 8;
+    if (col >= D) return;
+    const int r0 = blockIdx.x * KMEAN_ROWS, r1 = min(L, r0 + KMEAN_ROWS);
+    double acc[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    const __nv_bfloat16* src = k + (static_cast<int64_t>(b) * L) * ldk + col;
+#pragma unroll 8
+    for (int r = r0; r < r1; ++r) {
+        const uint4 x = *reinterpret_cast<const uint4*>(src + static_cast<int64_t>(r) * ldk);
+        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float2 f = unpack_bf16(w[i]);
+            acc[2 * i] += static_cast<double>(f.x);
+            acc[2 * i + 1] += static_cast<double>(f.y);
+        }
+    }
+    double* dst = partial + (static_cast<int64_t>(b) * gridDim.x + blockIdx.x) * D + col;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) dst[i] = acc[i];
+}
+
+// grid (ceil(D / 128), B), one thread per channel
+__global__ void __launch_bounds__(128) k_mean_finish_kernel(const double* partial, float* kbar, int n_chunks, int L, int D) {
+    const int b = blockIdx.y, c = blockIdx.x * 128 + threadIdx.x;
+    if (c >= D) return;
+    const double* src = partial + static_cast<int64_t>(b) * n_chunks * D + c;
+    double acc = 0.0;
+    for (int i = 0; i < n_chunks; ++i) acc += src[static_cast<int64_t>(i) * D];
+    kbar[static_cast<int64_t>(b) * D + c] = static_cast<float>(acc / static_cast<double>(L));
+}
+
+// One 128-thread block per key row (rows = B * L), D = H * 128 <= ROW_MAXV * 1024
+__global__ void __launch_bounds__(ROW_THREADS) quant_k_int8_kernel(const __nv_bfloat16* k, int64_t ldk, const float* kbar,
+                                                                    int8_t* k8, int64_t ld8, float* scale, int L, int L_pad,
+                                                                    int D) {
+    const int row = blockIdx.x;
+    const int b = row / L, tok = row - b * L;
+    const int heads = D >> 7, nvec = D >> 3;
+    const uint4* xin = reinterpret_cast<const uint4*>(k + static_cast<int64_t>(row) * ldk);
+    const float* kb = kbar + static_cast<int64_t>(b) * D;
+#pragma unroll
+    for (int j = 0; j < ROW_MAXV; ++j) {
+        const int i = j * ROW_THREADS + threadIdx.x;
+        float f[8];
+        float amax = 0.f;  // all lanes shuffle (a lane past the row contributes 0); a head's 16 lanes are all in or all out
+        if (i < nvec) {
+            const uint4 v = xin[i];
+            const float4 m0 = reinterpret_cast<const float4*>(kb)[2 * i], m1 = reinterpret_cast<const float4*>(kb)[2 * i + 1];
+            const float m[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const float2 x = unpack_bf16(w[c]);
+                f[2 * c] = __fsub_rn(x.x, m[2 * c]);
+                f[2 * c + 1] = __fsub_rn(x.y, m[2 * c + 1]);
+            }
+#pragma unroll
+            for (int c = 0; c < 8; ++c) amax = fmaxf(amax, fabsf(f[c]));
+        }
+#pragma unroll
+        for (int o = 1; o < 16; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+        if (i < nvec) {
+            const float s = int8_row_scale(amax);
+            reinterpret_cast<uint2*>(k8 + static_cast<int64_t>(row) * ld8)[i] = quant_f32x8_s8(f, s);
+            if ((i & 15) == 0) {
+                float* sh = scale + (static_cast<int64_t>(b) * heads + (i >> 4)) * L_pad;
+                sh[tok] = s;
+                for (int pad = L + tok; pad < L_pad; pad += L) sh[pad] = 0.f;
             }
         }
     }

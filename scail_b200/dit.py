@@ -148,6 +148,16 @@ class _Workspace:
 
 _WS = _Workspace()
 
+FP8_ATTENTION_INT8_QK = "int8_qk"
+
+
+def check_fp8_attention(mode):
+    """The fp8_attention setting: False / True (any non-string value, by its truth, as it has always been read), or the string
+    "int8_qk" (INT8 Q and smoothed K, e4m3 V and P).  Any other string raises ValueError."""
+    if isinstance(mode, str) and mode != FP8_ATTENTION_INT8_QK:
+        raise ValueError(f"fp8_attention must be False, True or {FP8_ATTENTION_INT8_QK!r}, got {mode!r}")
+    return mode
+
 
 class Conditioning:
     """Step-invariant conditioning of one sample (SURVEY §8f rank 1): text / CLIP embeddings and every layer's
@@ -359,7 +369,8 @@ class AdaLNMixin(BaseMixin):
         self.fp8_linear = fp8_linear
         # Opt-in, independent of fp8_linear: the self-attention runs on e4m3 Q, K (one scale per token and head) and V (one
         # scale per channel) through attention_fp8_kernel; cross-attention stays bf16.  A plain attribute, like fp8_linear.
-        self.fp8_attention = fp8_attention
+        # "int8_qk": Q and K in INT8 instead, K smoothed by its per-(batch, channel) mean first (DESIGN §3.2.1).
+        self.fp8_attention = check_fp8_attention(fp8_attention)
         # Opt-in block-sparse self-attention (scail_b200.sparse): None is dense; an int w >= 0 restricts every query to the
         # keys within w frames of its own (the ref rows and the ref keys stay dense), through the sparse forms of whichever
         # self-attention kernel runs (bf16 or fp8_attention).  A plain attribute, toggled between forwards like fp8_attention.
@@ -554,22 +565,39 @@ class AdaLNMixin(BaseMixin):
 
     def _self_attention_fp8(self, qkv, B, N, d, H, wq, wk, cos, sin, ctx, tiles=None, n_ref=None):
         """Self-attention of the fused QKV buffer in e4m3: RMSNorm+RoPE writes quantised Q and K, the V slab is transposed and
-        quantised per channel, then attention_fp8 writes the merged-head context into ctx.  Buffers: per-stream workspace."""
+        quantised per channel, then attention_fp8 writes the merged-head context into ctx.  Buffers: per-stream workspace.
+        fp8_attention="int8_qk": Q in INT8 from RMSNorm+RoPE, K normalised in place and then smoothed and quantised to INT8
+        (quant_k_int8), and attention_int8qk."""
         dev, f32 = qkv.device, torch.float32
         Lp = ops.fp8_pad(N)
-        q8 = (_WS.get("q8", (B * N, d), dev, ops.FP8), _WS.get("q8_scale", (B, H, Lp), dev, f32))
-        k8 = (_WS.get("k8", (B * N, d), dev, ops.FP8), _WS.get("k8_scale", (B, H, Lp), dev, f32))
-        ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon, out_fp8=[q8, k8])
+        int8 = check_fp8_attention(self.fp8_attention) == FP8_ATTENTION_INT8_QK
+        if int8:
+            q8 = (_WS.get("q8i", (B * N, d), dev, ops.INT8), _WS.get("q8_scale", (B, H, Lp), dev, f32))
+            k8 = (_WS.get("k8i", (B * N, d), dev, ops.INT8), _WS.get("k8_scale", (B, H, Lp), dev, f32))
+            ops.rmsnorm_rope_int8q(qkv, N, d, [(0, wq), (d, wk)], q8[0], q8[1], cos, sin, eps=self.layernorm_epsilon)
+            ops.quant_k_int8(qkv[:, d:2 * d], B, H, N, k8[0], k8[1], _WS.get("k8_mean", (B, d), dev, f32),
+                             _WS.get("k8_partial", (ops.quant_k_int8_partial_len(B, H, N),), dev, torch.float64))
+        else:
+            q8 = (_WS.get("q8", (B * N, d), dev, ops.FP8), _WS.get("q8_scale", (B, H, Lp), dev, f32))
+            k8 = (_WS.get("k8", (B * N, d), dev, ops.FP8), _WS.get("k8_scale", (B, H, Lp), dev, f32))
+            ops.rmsnorm_rope(qkv, N, d, [(0, wq), (d, wk)], cos, sin, eps=self.layernorm_epsilon, out_fp8=[q8, k8])
         vt, vs = ops.quant_vt_fp8(qkv[:, 2 * d:], B, H, N, _WS.get("vt8", (B, H, 128, Lp), dev, ops.FP8),
                                   _WS.get("vt8_scale", (B, H, 128), dev, f32), _WS.get("vt8_amax", (B, d), dev, torch.int32))
         if self.attention_adaptive is not None:
+            # with int8_qk the pooled K is the smoothed K': every s_k of a query tile shifts by the same amount (DESIGN §3.2.1)
             ptr, idx = self.attention_adaptive.select(q8[0], k8[0], B, H, N, self._n_ref(N, {"ref_length": n_ref}), self._ws(dev),
                                                       q_scale=q8[1], k_scale=k8[1])
-            ops.attention_fp8_sparse_bh(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, ptr, idx)
+            if int8:
+                ops.attention_int8qk(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, bh_maps=(ptr, idx))
+            else:
+                ops.attention_fp8_sparse_bh(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, ptr, idx)
+        elif int8:
+            ops.attention_int8qk(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, tiles=tiles)
         else:
             ops.attention_fp8(q8[0], q8[1], k8[0], k8[1], vt, vs, ctx, B, H, N, tiles=tiles)
 
     def _refuse_fp8_attention_cp(self):
+        check_fp8_attention(self.fp8_attention)  # an attribute set to an unknown mode since construction
         if self.fp8_attention and self.cp is not None and self.cp.size > 1:
             raise NotImplementedError("fp8_attention is not implemented under context parallelism (a ContextParallel of size "
                                       f"{self.cp.size}); turn fp8_attention off or run without context parallelism")

@@ -161,6 +161,101 @@ def rmsnorm_rope(buf, rows_per_batch, D, slabs, cos=None, sin=None, eps=1e-6, ou
     return buf
 
 
+INT8 = torch.int8
+
+
+def rmsnorm_rope_int8q(buf, rows_per_batch, D, slabs, q8, q_scale, cos=None, sin=None, eps=1e-6):
+    """fp8_attention="int8_qk" form of rmsnorm_rope over the two slabs [(q_offset, wq), (k_offset, wk)] of the 2-D bf16 buf:
+    Q goes to INT8 rows q8 [rows, D] (2-D, stride(1)==1) with scales q_scale fp32 [B, D/128, L_pad] (s = amax / 127, q =
+    round-half-even(x / s) clamped to [-127, 127], one per token and 128-wide head, zeros past rows_per_batch), bit for bit
+    the quantised bf16 result; K is normalised in place in bf16 exactly as rmsnorm_rope writes it.  Returns (q8, q_scale)."""
+    _req(buf), _req(q8, INT8), _req(q_scale, torch.float32)
+    assert buf.dim() == 2 and buf.stride(1) == 1 and len(slabs) == 2
+    (o0, w0), (o1, w1) = slabs
+    rows = buf.shape[0]
+    assert q8.dim() == 2 and q8.shape == (rows, D) and q8.stride(1) == 1
+    assert q_scale.is_contiguous() and q_scale.shape == (rows // rows_per_batch, D // 128, q_scale.shape[-1])
+    _lib.check(_lib.lib().scail_rmsnorm_rope_int8q(
+        _ptr(buf), buf.stride(0), rows, rows_per_batch, D, 2, o0, _ptr(w0), o1, _ptr(w1), _ptr(cos), _ptr(sin), eps,
+        _ptr(q8), _ptr(q_scale), q8.stride(0), q_scale.shape[-1], _stream()), "scail_rmsnorm_rope_int8q")
+    _count()
+    return q8, q_scale
+
+
+KMEAN_ROWS = 256  # keys per fp64 partial sum of quant_k_int8
+
+
+def quant_k_int8_partial_len(B, H, L):
+    """fp64 entries of quant_k_int8's partial-sum workspace: B ceil(L / 256) H 128."""
+    return B * -(-int(L) // KMEAN_ROWS) * H * 128
+
+
+def quant_k_int8(k, B, H, L, k8=None, scale=None, kbar=None, partial=None):
+    """K operand of attention_int8qk: k bf16 [B*L, H*128] (2-D row-strided view) -> (k8 int8 [B*L, H*128], scale fp32
+    [B, H, L_pad], kbar fp32 [B, H*128]).  kbar is the per-(batch, channel) mean over the L keys (fp64 sums over fixed
+    256-key chunks, added in order, divided by L in fp64, rounded once); k8 and scale quantise K' = f32(k) - kbar (one fp32
+    rounding) per token and head in the INT8 row format of rmsnorm_rope_int8q.  partial: fp64 workspace of
+    quant_k_int8_partial_len(B, H, L) entries (allocated when None).  Bit-reproducible, no host reads."""
+    _req(k)
+    assert k.dim() == 2 and k.stride(1) == 1 and k.shape == (B * L, H * 128)
+    Lp = fp8_pad(L)
+    dev = k.device
+    k8 = torch.empty(B * L, H * 128, device=dev, dtype=INT8) if k8 is None else k8
+    scale = torch.empty(B, H, Lp, device=dev, dtype=torch.float32) if scale is None else scale
+    kbar = torch.empty(B, H * 128, device=dev, dtype=torch.float32) if kbar is None else kbar
+    n = quant_k_int8_partial_len(B, H, L)
+    partial = torch.empty(n, device=dev, dtype=torch.float64) if partial is None else partial
+    _req(k8, INT8), _req(scale, torch.float32), _req(kbar, torch.float32), _req(partial, torch.float64)
+    assert k8.dim() == 2 and k8.shape == (B * L, H * 128) and k8.stride(1) == 1
+    assert scale.is_contiguous() and scale.shape == (B, H, Lp) and kbar.is_contiguous() and kbar.shape == (B, H * 128)
+    assert partial.is_contiguous()
+    _lib.check(_lib.lib().scail_quant_k_int8(_ptr(k), k.stride(0), _ptr(k8), k8.stride(0), _ptr(scale), _ptr(kbar),
+                                             _ptr(partial), partial.numel(), B, H, L, Lp, _stream()), "scail_quant_k_int8")
+    _count(3)
+    return k8, scale, kbar
+
+
+def attention_int8qk(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L, scale=None, tiles=None, bh_maps=None):
+    """Self-attention with INT8 Q and K (q_len == kv_len == L): q8 and its scales from rmsnorm_rope_int8q, k8 and its scales
+    from quant_k_int8 (smoothed K), (vt, v_scale) from quant_vt_fp8; out bf16 [B*L, H*128] merged heads.  S = Q K^T is
+    exact in s32; V, P and the softmax are attention_fp8's.  tiles: one block-sparse map for every (batch, head), as for
+    attention_sparse; bh_maps=(ptr, idx): per-(batch, head) maps as for attention_sparse_bh.  At most one of the two."""
+    if tiles is not None and bh_maps is not None:
+        raise ValueError("attention_int8qk: give tiles or bh_maps, not both")
+    m = _tile_map(tiles, L) if tiles is not None else None
+    for t in (q8, k8):
+        _req(t, INT8)
+        assert t.dim() == 2 and t.stride(1) == 1 and t.shape == (B * L, H * 128)
+    Lp = fp8_pad(L)
+    for s in (q_scale, k_scale):
+        _req(s, torch.float32)
+        assert s.is_contiguous() and s.shape == (B, H, Lp)
+    _req(vt, FP8), _req(v_scale, torch.float32), _req(out)
+    assert vt.is_contiguous() and vt.shape == (B, H, 128, Lp) and v_scale.is_contiguous() and v_scale.shape == (B, H, 128)
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape == (B * L, H * 128)
+    ptr = idx = None
+    ps = ids = 0
+    if m is not None:
+        m._check_for(L, q8.device)
+        ptr, idx = m.ptr, m.idx
+    elif bh_maps is not None:
+        ptr, idx = bh_maps
+        ps, ids = _bh_maps(ptr, idx, B, H, L, q8.device)
+    scale = 1.0 / math.sqrt(128) if scale is None else scale
+    ev = None
+    if ATTN_EVENTS is not None and L > 1024:
+        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+        ev[0].record()
+    _lib.check(_lib.lib().scail_attention_int8qk(_ptr(q8), q8.stride(0), _ptr(q_scale), _ptr(k8), k8.stride(0), _ptr(k_scale),
+                                                 _ptr(vt), _ptr(v_scale), _ptr(out), out.stride(0), B, H, 128, L, Lp, scale,
+                                                 _ptr(ptr), ps, _ptr(idx), ids, _stream()), "scail_attention_int8qk")
+    if ev is not None:
+        ev[1].record()
+        ATTN_EVENTS.append(ev)
+    _count()
+    return out
+
+
 def attention(q, k, v, out, B, H, q_len, kv_len, q_batch_rows=None, kv_batch_rows=None, scale=None, accumulate=False):
     """q/k/v/out: 2-D row-strided bf16 views [rows, H*128] (stride(1)==1); head h = columns h*128..h*128+127."""
     for t in (q, k, v, out):
@@ -410,11 +505,12 @@ def attention_fp8_sparse_bh(q8, q_scale, k8, k_scale, vt, v_scale, out, B, H, L,
 
 
 def tile_pool(x, B, H, L, out=None, x_scale=None):
-    """Tile means of one self-attention operand: x [B*L, H*128] (2-D row-strided view) bf16, or e4m3 with its per-token
-    scales x_scale [B, H, L_pad] -> out fp32 [B, H, ceil(L/128), 128], the mean of each 128-row tile's valid rows (of x *
-    scale for e4m3).  Bit-reproducible."""
+    """Tile means of one self-attention operand: x [B*L, H*128] (2-D row-strided view) bf16, or e4m3 or int8 with its
+    per-token scales x_scale [B, H, L_pad] -> out fp32 [B, H, ceil(L/128), 128], the mean of each 128-row tile's valid rows
+    (of x * scale for e4m3 and int8).  Bit-reproducible."""
     fp8 = x_scale is not None
-    _req(x, FP8 if fp8 else torch.bfloat16)
+    int8 = fp8 and x.dtype == INT8
+    _req(x, (INT8 if int8 else FP8) if fp8 else torch.bfloat16)
     assert x.dim() == 2 and x.stride(1) == 1 and x.shape == (B * L, H * 128)
     n = -(-L // ATT_TILE)
     Lp = fp8_pad(L)
@@ -425,8 +521,12 @@ def tile_pool(x, B, H, L, out=None, x_scale=None):
         out = torch.empty(B, H, n, 128, device=x.device, dtype=torch.float32)
     _req(out, torch.float32)
     assert out.is_contiguous() and out.shape == (B, H, n, 128)
-    _lib.check(_lib.lib().scail_attention_tile_pool(_ptr(x), x.stride(0), _ptr(x_scale), 1 if fp8 else 0, _ptr(out), B, H, L,
-                                                    Lp if fp8 else 0, _stream()), "scail_attention_tile_pool")
+    if int8:
+        _lib.check(_lib.lib().scail_attention_tile_pool_int8(_ptr(x), x.stride(0), _ptr(x_scale), _ptr(out), B, H, L, Lp,
+                                                             _stream()), "scail_attention_tile_pool_int8")
+    else:
+        _lib.check(_lib.lib().scail_attention_tile_pool(_ptr(x), x.stride(0), _ptr(x_scale), 1 if fp8 else 0, _ptr(out), B, H,
+                                                        L, Lp if fp8 else 0, _stream()), "scail_attention_tile_pool")
     _count()
     return out
 

@@ -34,6 +34,14 @@ timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$O
     > "$OUT/memcheck_fp8_attention_pytest.log" 2>&1
 echo "sanitizer exit code $?" >> "$OUT/memcheck_fp8_attention_pytest.log"
 tail -3 "$OUT/memcheck_fp8_attention_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_fp8_attention.log" | head -5
+# int8_qk self-attention at small shapes: RMSNorm+RoPE INT8 form, K smoothing and quantisation (ragged last chunk), the
+# INT8 tile pooling, attention_int8qk dense and sparse (partial last tile)
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 99 --log-file "$OUT/memcheck_int8qk_attention.log" \
+    python -m pytest tests/test_int8qk_attention_gpu.py -q -x --timeout 600 \
+    -k "quantisers and 129 or quantisers and 1000 or dense and 1-2-129 or sparse_forms or tile_pool or small_model or abi" \
+    > "$OUT/memcheck_int8qk_attention_pytest.log" 2>&1
+echo "sanitizer exit code $?" >> "$OUT/memcheck_int8qk_attention_pytest.log"
+tail -3 "$OUT/memcheck_int8qk_attention_pytest.log"; grep -E "ERROR SUMMARY|Invalid|out of bounds" "$OUT/memcheck_int8qk_attention.log" | head -5
 # adaptive tile selection at small shapes: tile pooling (bf16, e4m3 + scales, ragged last tile), device selection and
 # compaction, and the per-(batch, head) sparse attention kernels; memcheck, then racecheck for the shared-memory selection
 for tool in memcheck racecheck; do
