@@ -126,14 +126,18 @@ def _view(t):
 
 
 def _rope_geometry(cos):
-    """(T, H, W) of the RoPE tables `cos` (rope.build_tables keeps one pair per geometry), or None without RoPE."""
+    """(T, H, W, h_shift, w_shift, first row) of the RoPE tables `cos`, or None without RoPE.  rope.build_tables keeps one
+    pair per geometry and shift; `cos` is one of them or, under context parallelism, a row slice of one (first row: the
+    slice's offset into its base table)."""
     from scail_b200 import rope
     if cos is None:
         return None
     for key, (c, _) in rope._DEV_CACHE.items():
-        if c is cos:
-            assert key[5:] == (0, 0, 0, 120, 10000.0), key  # no context-parallel shifts on one GPU
-            return key[2:5]
+        if cos.untyped_storage().data_ptr() == c.untyped_storage().data_ptr():
+            assert key[7:] == (0, 120, 10000.0), key  # the model's global_rope_H / W and theta
+            row, rem = divmod(cos.storage_offset() - c.storage_offset(), c.stride(0))
+            assert rem == 0 and cos.stride() == c.stride() and row + cos.shape[0] <= c.shape[0], "not a row slice of its table"
+            return key[2:7] + (row,)
     raise AssertionError("RoPE tables that rope.build_tables did not make")
 
 
@@ -468,9 +472,11 @@ def check_rmsnorm_rope(ops, f, g):
     weights = [1 + _rand(g, D, scale=0.1) for _ in f["slabs"]]
     slabs = list(zip(f["slabs"], weights))
     cos = sin = None
-    if f["rope"] is not None:  # the geometry's real tables
-        cos, sin = rope.build_tables("cuda", 128, *f["rope"])
-        assert cos.shape[0] == rpb
+    if f["rope"] is not None:  # the geometry's real tables (shifted, and the recorded row slice of them)
+        *geo, row = f["rope"]
+        cos, sin = rope.build_tables("cuda", 128, *geo)
+        assert row + rpb <= cos.shape[0]
+        cos, sin = cos[row:row + rpb], sin[row:row + rpb]
     buf = Slab(data, f["buf"])
     ops.rmsnorm_rope(buf.v, rpb, D, slabs, cos, sin, eps=eps)
     torch.cuda.synchronize()
@@ -481,7 +487,7 @@ def check_rmsnorm_rope(ops, f, g):
         other[o:o + D] = False
         x = data[:, o:o + D].float()
         y = wgt.float() * (x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps))  # oracle rmsnorm: g * (x * rstd)
-        if cos is not None:  # oracle RoPE on interleaved pairs, token = row % rows_per_batch
+        if cos is not None:  # oracle RoPE on interleaved pairs, token = first row + row % rows_per_batch of the base table
             tok = torch.arange(rows, device="cuda") % rpb
             yh = y.view(rows, D // 128, 128)
             y = (yh * cos[tok][:, None] + _rotate_half(yh) * sin[tok][:, None]).view(rows, D)
@@ -562,6 +568,10 @@ def _attention_data(g, f, tiles=None):
     plants = [(3, kv_len - 1, 0.5), (q_len - 2, 0, 0.5), (q_len // 2, edge - 1, 0.5), (q_len // 2 + 1, edge, 0.5)]
     if B > 1 and kv_len % 128:  # batch 0's last key tile overhangs into batch 1: its key 5 is inside that TMA box
         plants.append((q_len - 1, kv_len + 5, 1.0))
+    if kv_len > q_len and kv_len % q_len == 0:  # context parallelism: local queries against P = kv_len / q_len gathered shards
+        # the first and last key of every shard; where a shard boundary falls inside a 128-key tile, those are its two sides
+        keys = sorted({key for p in range(kv_len // q_len) for key in (p * q_len, (p + 1) * q_len - 1)})
+        plants += [(10 + 17 * j, key, 0.5) for j, key in enumerate(keys)]
     if tiles is not None:  # a key in a tile the row's map does not list (no effect), and one in a listed tile
         t = tiles.shape[0] // 2
         listed = torch.nonzero(tiles[t]).flatten().tolist()
@@ -1084,10 +1094,10 @@ def test_recorded_launches_cover_the_production_cases(launches):
         "final-layer ln_modulate with row_offset = n_ref at every geometry":
             all(has("ln_modulate", n_in=Ns[geo], row_offset=n_ref[geo], rows_out=n_seq[geo]) for geo in GEOMETRIES),
         "two-slab rmsnorm_rope with RoPE at every geometry":
-            all(has("rmsnorm_rope", slabs=(0, 5120), rope=grid(geo), fp8=None) for geo in GEOMETRIES),
+            all(has("rmsnorm_rope", slabs=(0, 5120), rope=grid(geo) + (0, 0, 0), fp8=None) for geo in GEOMETRIES),
         "fp8 forms: GEMM, quantisers, LN, RMSNorm+RoPE and dense attention at every geometry":
             has("gemm_fp8") and has("quant_rows_fp8") and has("ln_modulate", fp8=True) and
-            all(has("rmsnorm_rope", rope=grid(geo), fp8=lambda v: v is not None) and has("quant_vt_fp8", L=N) and
+            all(has("rmsnorm_rope", rope=grid(geo) + (0, 0, 0), fp8=lambda v: v is not None) and has("quant_vt_fp8", L=N) and
                 has("attention_fp8", B=2, L=N, tiles=None) for geo, N in Ns.items()),
         "window-2 sparse maps, bf16 and fp8, at every geometry":
             all(has("attention_sparse", B=2, q_len=Ns[geo], tiles=window(geo)) and

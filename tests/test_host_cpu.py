@@ -67,6 +67,61 @@ def test_rope_tables_bit_identical_to_oracle():
     assert torch.equal(c, c2) and torch.equal(s, s2)
 
 
+# the pre-chunked context-parallel forms the CP launch-shape test runs: (token grid T, H, W of the latent, chunk_dim, P).
+# 512x896 -> 21x32x56, 480x832 -> 21x30x52; chunk_dim 3 at 480x832 would leave a 15-row pose latent per rank, which does
+# not patchify
+CHUNK_CASES = [((21, 32, 56), 3, 2), ((21, 32, 56), 3, 4), ((21, 32, 56), 4, 2), ((21, 32, 56), 4, 4), ((21, 30, 52), 4, 2)]
+
+
+def chunk_shifts(T, H, W, chunk_dim, P, p):
+    """(rope_H, rope_W, rope_H_shift, rope_W_shift) of rank p when the latents are chunked on H (chunk_dim 3) or W (4)."""
+    if chunk_dim == 3:
+        return H // P, W, p * (H // P), 0
+    return H, W // P, 0, p * (W // P)
+
+
+def chunk_tokens(T, H, W, chunk_dim, P, p):
+    """The global token indices (into the one-GPU ref || noise || pose sequence of a T x H x W token grid) of rank p's
+    local sequence when the latent, the reference and the pose are each chunked on H (chunk_dim 3) or W (4) into P parts,
+    in local order."""
+    def part(t, h, w, base):
+        idx = torch.arange(t * h * w).view(t, h, w) + base
+        return (idx[:, p * h // P:(p + 1) * h // P] if chunk_dim == 3 else idx[:, :, p * w // P:(p + 1) * w // P]).reshape(-1)
+    n_ref, n_seq = H * W, T * H * W
+    return torch.cat([part(1, H, W, 0), part(T, H, W, n_ref), part(T, H // 2, W // 2, n_ref + n_seq)])
+
+
+def test_shifted_rope_tables_at_production_chunks_bit_identical_to_oracle():
+    from oracle import dit_oracle as O
+    from scail_b200 import rope
+    for (T, H, W), cd, P in CHUNK_CASES:
+        for p in range(P):
+            h, w, hs, ws = chunk_shifts(T, H, W, cd, P, p)
+            c, s = rope.build_tables_cpu(128, T, h, w, hs, ws)
+            c2, s2 = O.rope_tables(128, T, h, w, 21, 150, 150, h_shift=hs, w_shift=ws)
+            assert torch.equal(c, c2) and torch.equal(s, s2), ((T, H, W), cd, P, p)
+
+
+def test_each_ranks_shifted_tables_are_the_one_gpu_rows_of_its_tokens():
+    """Rank p's shifted tables equal the one-GPU tables at chunk_tokens(p), bit for bit.  Every shift here is even, so the 2x2
+    average pooling of the pose rows pairs the same grid rows and columns locally as on one GPU (an odd shift would pool
+    across the pairs and give other values)."""
+    from scail_b200 import rope
+    for (T, H, W), cd, P in CHUNK_CASES:
+        c, s = rope.build_tables_cpu(128, T, H, W)
+        for p in range(P):
+            h, w, hs, ws = chunk_shifts(T, H, W, cd, P, p)
+            assert hs % 2 == 0 and ws % 2 == 0
+            idx = chunk_tokens(T, H, W, cd, P, p)
+            assert idx.numel() * P == c.shape[0]
+            cl, sl = rope.build_tables_cpu(128, T, h, w, hs, ws)
+            assert torch.equal(cl, c[idx]) and torch.equal(sl, s[idx]), ((T, H, W), cd, P, p)
+    # the ranks' tokens partition the sequence
+    for (T, H, W), cd, P in CHUNK_CASES:
+        allidx = torch.cat([chunk_tokens(T, H, W, cd, P, p) for p in range(P)])
+        assert torch.equal(allidx.sort().values, torch.arange(allidx.numel()))
+
+
 def test_state_dict_names_match_reference_golden():
     from scail_b200.dit import DiffusionTransformer
     from scail_b200.wan_vae import WanVAE
