@@ -18,6 +18,7 @@ Everything is computed on the tensors' own device (no copy to the host), in fp32
 `recording` finds the launches to check: it wraps entry points of a module while a real workload runs and keeps one entry per
 distinct launch, so that each can be re-run on fresh data against a reference."""
 import contextlib
+import functools
 import inspect
 from collections import namedtuple
 
@@ -67,13 +68,14 @@ def recording(module, names, fields):
 
     fields(name, arguments) -> (key, value) for one call, where `arguments` maps every parameter to its value (defaults
     applied): `key` is a dict of what makes two calls the same launch, `value` a number kept as the maximum over the calls
-    with that key.  Yields `seen`, a dict {(name, tuple(key.items())): value} in first-call order."""
+    with that key.  Recordings nest: an inner one sees the calls an outer one sees.  Yields `seen`, a dict {(name, tuple(key.items())): value} in first-call order."""
     seen = {}
     originals = {name: getattr(module, name) for name in names}
 
     def recorder(name, fn):
-        sig = inspect.signature(fn)
+        sig = inspect.signature(fn)  # through functools.wraps: recordings nest, each binding the entry point's own parameters
 
+        @functools.wraps(fn)
         def rec(*args, **kwargs):
             b = sig.bind(*args, **kwargs)
             b.apply_defaults()

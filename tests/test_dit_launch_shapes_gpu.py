@@ -23,7 +23,11 @@ Attention data can fail: q, k give scaled logits with std ~3, and planted keys d
 last valid key, keys on both sides of a 128-key tile edge, and for sparse maps a key in an unlisted tile, which must have no
 effect, and one in a listed tile).  Where batch 0's last key tile overhangs into batch 1 (kv_len % 128 != 0), batch 0's last
 query row gets a winning key among batch 1's first rows: the TMA box of that tile reads it and only the mask keeps it out.
-A leaked mask or a skipped tile moves such a row by the scale of V, not by a rounding.  The per-(batch, head) kernels run
+A leaked mask or a skipped tile moves such a row by the scale of V, not by a rounding.  The last batch's last key tile has
+nothing after it (TMA zero-fills the overhang, and a zero key's logit 0 is far below an ordinary row's max of ~ +13), so
+where kv_len % 128 != 0 the last query row of batch B - 1 gets logits <= -40 at heads 0 and H - 1 (_plant_last_tile): a
+leaked key past the end then takes the whole row.  Every view has 128 sentinel rows after it, so a whole tile read or
+stored past its last row lands on sentinels.  The per-(batch, head) kernels run
 under maps from a real select_tiles run that differ across heads and batch elements; in both batch elements, at heads 0,
 H/2 and H - 1, a row gets a key in a tile its own map omits but the next head's map lists (no effect), and one in a tile
 its map lists.
@@ -209,7 +213,7 @@ def _fields(name, a):
         return dict(shape=tuple(a["h"].shape), n_ref=a["n_ref"], n_seq=a["R"].shape[1]), 1
     if name == "tile_pool":
         xs = a["x_scale"]
-        return dict(B=a["B"], H=a["H"], L=a["L"], x=_view(a["x"]), fp8=xs is not None,
+        return dict(B=a["B"], H=a["H"], L=a["L"], x=_view(a["x"]), fp8=xs is not None, int8=a["x"].dtype == torch.int8,
                     L_pad=None if xs is None else xs.shape[-1]), 1
     if name == "select_tiles":
         return dict(B=a["B"], H=a["H"], L=a["L"], n_ref=a["n_ref"], mass=float(a["mass"]), max_tiles=a["max_tiles"],
@@ -285,8 +289,9 @@ def launches():
 
 
 # ---------------------------------------------------------------- buffers with sentinels
-_SENTINEL_BITS = {1: 0x7E, 2: 0x4680, 4: 0x46800000}  # e4m3 448, bf16 16384, fp32 16384
-_INT = {1: torch.uint8, 2: torch.int16, 4: torch.int32}
+_SENTINEL_BITS = {1: 0x7E, 2: 0x4680, 4: 0x46800000, 8: 0x40D0000000000000}  # e4m3 448 / int8 126, bf16, fp32, fp64 16384
+_INT = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
+TRAILING = 128  # sentinel rows after a Slab's view: a whole 128-row tile read or stored past its last row lands on them
 
 
 def _bits(t):
@@ -295,13 +300,13 @@ def _bits(t):
 
 class Slab:
     """`data` [rows, cols] placed as a view at a recorded place (row stride, first column, rows before) of a wider buffer
-    with two rows after it; every other element of the buffer is a sentinel, which check() asserts is unchanged."""
+    with TRAILING rows after it; every other element of the buffer is a sentinel, which check() asserts is unchanged."""
 
     def __init__(self, data, view):
         ld, c0, before = view
         rows, cols = data.shape
         self.r0, self.c0, self.rows, self.cols = (2 if before else 0), c0, rows, cols
-        self.parent = torch.empty(self.r0 + rows + 2, ld, device=data.device, dtype=data.dtype)
+        self.parent = torch.empty(self.r0 + rows + TRAILING, ld, device=data.device, dtype=data.dtype)
         _bits(self.parent).fill_(_SENTINEL_BITS[data.element_size()])
         self.v = self.parent[self.r0:self.r0 + rows, c0:c0 + cols]
         _bits(self.v).copy_(_bits(data))
@@ -530,15 +535,23 @@ def _attention_ref(q, k, v, B, H, q_len, kv_len, scale, tiles=None, chain=False)
     """fp32 softmax(scale q k^T) v per batch and head over [B * len, H * 128] operands, queries chunked; tiles: the key tiles
     each 128-query tile may see, bool [n_q_tiles, n_kv_tiles] for every (batch, head) or [B, H, n_q_tiles, n_kv_tiles] per
     (batch, head).  chain: the restated fp8 chain of test_fp8_attention_gpu.chain_fp8 (dequantised per-token Q, K and
-    per-channel V, P^ = e4m3(2^8 p) against the row max over the allowed keys, l the sum of the unquantised 2^8 p)."""
+    per-channel V, P^ = e4m3(2^8 p) against the row max over the allowed keys, l the sum of the unquantised 2^8 p); chain=
+    "int8": the int8-QK chain of test_int8qk_attention_gpu.chain_int8 (Q and K' = K - its fp64 per-(batch, channel) mean
+    over the kv_len keys in the INT8 row format, V and P as in the fp8 chain)."""
+    from test_int8qk_attention_gpu import int8_ref
     out = torch.empty(B * q_len, H * 128, device="cuda")
     chunk = min(4096, max(128, (2 ** 29 // (H * kv_len)) // 128 * 128))
     for b in range(B):
         heads = lambda x, n: x[b * n:(b + 1) * n].float().view(n, H, 128).transpose(0, 1)
         qh, kh, vh = heads(q, q_len), heads(k, kv_len), heads(v, kv_len)
-        if chain:
+        if chain == "int8":
+            qh = deq(*int8_ref(qh.reshape(-1, 128))).view(H, q_len, 128)
+            kh = kh - kh.double().mean(1, keepdim=True).float()
+            kh = deq(*int8_ref(kh.reshape(-1, 128))).view(H, kv_len, 128)
+        elif chain:
             qh = deq(*quant_ref(qh.reshape(-1, 128))).view(H, q_len, 128)
             kh = deq(*quant_ref(kh.reshape(-1, 128))).view(H, kv_len, 128)
+        if chain:
             vh = deq(*quant_ref(vh.transpose(1, 2).reshape(-1, kv_len))).view(H, 128, kv_len).transpose(1, 2)
         kt = kh.transpose(1, 2)
         for i in range(0, q_len, chunk):
@@ -558,8 +571,9 @@ def _attention_ref(q, k, v, B, H, q_len, kv_len, scale, tiles=None, chain=False)
 
 
 def _attention_data(g, f, tiles=None):
-    """q, k, v bf16 [B * len, H * 128] with scaled logits of std ~3 and planted keys (module docstring).  -> (q, k, v,
-    [(query row, head, whether the row may see its planted key)] of batch 0)."""
+    """q, k, v bf16 [B * len, H * 128] with scaled logits of std ~3 and planted keys (module docstring), and where kv_len %
+    128 != 0 the last-tile plant of _plant_last_tile.  -> (q, k, v, [(global query row, head, whether the row may see its
+    planted key)])."""
     B, H, q_len, kv_len = f["B"], f["H"], f["q_len"], f["kv_len"]
     s = LOGIT_STD ** 0.5
     q, k, v = _rand(g, B * q_len, H * 128, scale=s), _rand(g, B * kv_len, H * 128, scale=s), _rand(g, B * kv_len, H * 128)
@@ -585,7 +599,37 @@ def _attention_data(g, f, tiles=None):
             c = slice(h * 128, h * 128 + 128)
             q[row, c] = (alpha * k[key, c].float()).to(BF)
             rows.append((row, h, visible))
+    if kv_len % 128:
+        rows += _plant_last_tile(g, q, k, B, H, q_len, kv_len, f.get("scale") or 128 ** -0.5, B > 1)
     return q, k, v, rows
+
+
+def _plant_last_tile(g, q, k, B, H, q_len, kv_len, scale, overhang):
+    """The last query row of batch B - 1, at heads 0 and H - 1, sees only logits <= -40: one common vector u is added to
+    every key of that (batch, head) and the row's q = -gamma u.  Softmax is shift-invariant per row, so only that row's
+    expected output changes, and it stays an ordinary row (its logits still spread by ~3).  The key tile past batch B - 1's
+    last key overhangs the end of the operand: TMA zero-fills it, and a zero key gets logit 0.  Without the mask those keys
+    take practically all of the row's weight and move it by its whole norm; with ordinary logits (max ~ +13) they would
+    carry ~1e-4 of it, below one bf16 rounding.  INT8 smoothing subtracts u again (mean-centred logits of a row cannot all
+    be negative), so for attention_int8qk this row is ordinary; there batch 0's overhang plant and the K scales past L
+    (check_attention_int8qk) test the mask.  overhang: batch 0's last row was planted with batch 1's key 5, so u is kept
+    orthogonal to that key (its winning logit stays as it was).  -> [(global row, head, False)]."""
+    row, rows = (B - 1) * q_len + q_len - 1, []
+    for h in (0, H - 1):
+        c = slice(h * 128, h * 128 + 128)
+        keys = k[(B - 1) * kv_len:B * kv_len, c]
+        u = torch.randn(128, device="cuda", generator=g) * 4.0
+        if overhang:
+            w = k[kv_len + 5, c].float()
+            u -= (u @ w) / (w @ w) * w
+        keys.copy_((keys.float() + u).to(BF))
+        ub = u.to(BF).float()
+        least = float((keys.float() @ ub).min())  # min over the keys of u . k, > 0: |u|^2 ~ 2048 against |u . k| ~ 80
+        assert least > 0, least
+        gamma = 2.0 ** math.ceil(math.log2(40.0 / (scale * least)))  # a power of two: q = -gamma u is exact in bf16
+        q[row, c] = (-gamma * ub).to(BF)
+        rows.append((row, h, False))
+    return rows
 
 
 def _block_rel(got, want, B, H, L):
@@ -670,21 +714,23 @@ def _fp8_verdict(got, want, chain, B, H, L, planted, what):
 
 # ---------------------------------------------------------------- content-adaptive attention
 def _flat(data):
-    """A Slab of a contiguous tensor taken as rows of its last dimension: two sentinel rows before and after it, and a view
-    that is contiguous again.  -> (slab, the view in data's shape)."""
+    """A Slab of a contiguous tensor taken as rows of its last dimension: two sentinel rows before it and TRAILING after it,
+    and a view that is contiguous again.  -> (slab, the view in data's shape)."""
     s = Slab(data.reshape(-1, data.shape[-1]), (data.shape[-1], 0, True))
     return s, s.v.view(data.shape)
 
 
 def check_tile_pool(ops, f, g):
     """Tile means against float64 within 1e-6 relative (as test_adaptive_attention_gpu), the ragged last tile included; in
-    e4m3 the codes times per-(token, head) scales that differ from token to token, with NaN past L (never read)."""
+    e4m3 or INT8 (the row format of test_int8qk_attention_gpu.heads_ref) the codes times per-(token, head) scales that
+    differ from token to token, with NaN past L (never read)."""
+    from test_int8qk_attention_gpu import heads_ref
     B, H, L = f["B"], f["H"], f["L"]
     n = -(-L // 128)
     x = _rand(g, B * L, H * 128, scale=2.0) + _rand(g, B * L, 1)  # rows with a mean of their own
     slabs = []
     if f["fp8"]:
-        codes, sc = qk_ref(x, B, H, L)
+        codes, sc = (heads_ref if f["int8"] else qk_ref)(x, B, H, L)
         assert sc.shape[-1] == f["L_pad"]
         sc[:, :, L:] = math.nan
         X = Slab(codes, f["x"])
@@ -758,7 +804,7 @@ def check_select_tiles(ops, f, g):
 def _adaptive_data(ops, g, f):
     """q, k, v bf16 [B * L, H * 128] (logit std ~3), per-(b, h) maps tm (bool [B, H, n, n] on the host) from a real
     select_tiles run on q, k at the adaptive mode's settings, and planted keys -> (q, k, v, tm, [(global query row, head,
-    whether the row may see its planted key)]).  In both batch elements, at heads 0, H/2 and H - 1, a query tile gets a key
+    whether the row may see its planted key)]).  In every batch element, at heads 0, H/2 and H - 1, a query tile gets a key
     in a tile its own map omits but the next head's map lists (no effect), and one in a listed tile (batch 0: the last
     valid key, in the ragged last tile); where batch 0's last key tile overhangs into batch 1, batch 0's last query row gets
     a winning key among batch 1's first rows (as _attention_data)."""
@@ -769,7 +815,7 @@ def _adaptive_data(ops, g, f):
     sel = dict(B=B, H=H, L=L, n_ref=N_REF[L], mass=ADAPTIVE[0], max_tiles=ADAPTIVE[1], ptr_stride=n + 1, idx_stride=n * n)
     _, ptr, idx = _select(ops, sel, ops.tile_pool(q, B, H, L), ops.tile_pool(k, B, H, L))
     tm = bh_dense(ptr, idx)
-    assert not torch.equal(tm[0, 0], tm[0, 1]) and not torch.equal(tm[0, 0], tm[1, 0]), "maps that do not differ"
+    assert not torch.equal(tm[0, 0], tm[0, 1]) and (B == 1 or not torch.equal(tm[0, 0], tm[1, 0])), "maps that do not differ"
     plants = []
     for b in range(B):
         for j, h in enumerate((0, H // 2, H - 1)):

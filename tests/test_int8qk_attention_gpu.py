@@ -10,14 +10,14 @@
    bounds against the masked fp32 softmax; the INT8 tile pooling bit for bit.
 4. Smoothing against a planted per-(batch, head) channel offset in K.
 5. The model against the fp32 oracle, toggling off, CUDA graphs and the cross-K/V cache.
-6. The mode's launches at 512x512 and 480x832 re-run inside wider buffers whose sentinels must not change.
+The mode's launches of the 14B step at every geometry, b = 2 and b = 1, are checked against fp32 in
+tests/test_dit_int8_b1_launch_shapes_gpu.py.
 TF32 is off throughout."""
 import math
 
 import pytest
 import torch
 
-from kernel_check import recording
 from test_fp8_attention_gpu import oracle_fp32, pad, qk_ref, small_model
 from test_fp8_gpu import SIX, lib_fp8_linear, rel, rnd, small_inputs
 from test_scale_gpu import sdpa_fp32_chunked
@@ -449,153 +449,6 @@ def test_adaptive_graphed_step_bit_identical():
             gs(sig[i], sig[i + 1])
     torch.cuda.synchronize()
     assert torch.equal(xe, xg)
-
-
-# ---------------------------------------------------------------- 6. launch shapes
-GEOMETRIES = {"512x512": (21, 64, 64), "480x832": (21, 60, 104)}
-OPS = ("rmsnorm_rope_int8q", "quant_k_int8", "attention_int8qk")
-
-
-def _view(t):
-    ld, off = t.stride(0), t.storage_offset()
-    return (ld, off % ld, off >= ld)
-
-
-def _fields(name, a):
-    if name == "rmsnorm_rope_int8q":
-        return dict(rows=a["buf"].shape[0], L=a["rows_per_batch"], D=a["D"], buf=_view(a["buf"]),
-                    slabs=tuple(o for o, _ in a["slabs"]), q8=_view(a["q8"]), L_pad=a["q_scale"].shape[-1]), 1
-    if name == "quant_k_int8":
-        return dict(B=a["B"], H=a["H"], L=a["L"], k=_view(a["k"]), k8=_view(a["k8"])), 1
-    return dict(B=a["B"], H=a["H"], L=a["L"], q=_view(a["q8"]), k=_view(a["k8"]), out=_view(a["out"]),
-                tiles=a["tiles"] is not None, bh=a["bh_maps"] is not None), 1
-
-
-@pytest.fixture(scope="module")
-def launches():
-    from scail_b200 import dit, ops, sampler, sparse
-    from test_dit_launch_shapes_gpu import step_inputs
-    m = full_width_model(1)
-    ad = m.mixins["adaln_layer"]
-    ad.fp8_attention = "int8_qk"
-    sig = sampler.make_flow_timesteps(50, 5.0)
-    with torch.no_grad(), recording(ops, OPS, _fields) as seen:
-        for i, (t, h, w) in enumerate(GEOMETRIES.values()):
-            x0, cond, uc = step_inputs(10 + i, t, h, w)
-            for window, adaptive in ((None, None), (2, None), (None, sparse.AdaptiveTiles(0.9, 40))):
-                ad.attention_window, ad.attention_adaptive = window, adaptive
-                sampler.sampler_step(m, x0.clone(), sig[0], sig[1], cond, uc, 4.0)
-    torch.cuda.synchronize()
-    del m, ad
-    dit._WS.bufs.clear()
-    torch.cuda.empty_cache()
-    return [(name, dict(k)) for (name, k) in seen]
-
-
-_SENT = {1: 0x7E, 2: 0x4680, 4: 0x46800000}
-_INT = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
-
-
-def _bits(t):
-    return t.view(_INT[t.element_size()])
-
-
-class Slab:
-    """`data` [rows, cols] at a recorded place (row stride, first column, rows before) of a wider buffer with two rows after
-    it; every other element is a sentinel that check() asserts is unchanged."""
-
-    def __init__(self, data, view):
-        ld, c0, before = view
-        rows, cols = data.shape
-        self.r0, self.c0, self.rows, self.cols = (2 if before else 0), c0, rows, cols
-        self.parent = torch.empty(self.r0 + rows + 2, max(ld, c0 + cols), device=data.device, dtype=data.dtype)
-        _bits(self.parent).fill_(_SENT[data.element_size()])
-        self.v = self.parent[self.r0:self.r0 + rows, c0:c0 + cols]
-        _bits(self.v).copy_(_bits(data))
-        self.snap = _bits(self.parent).clone()
-
-    def check(self, what):
-        changed = _bits(self.parent) != self.snap
-        changed[self.r0:self.r0 + self.rows, self.c0:self.c0 + self.cols] = False
-        assert not changed.any(), f"{what}: {int(changed.sum())} sentinel elements beside the view were written"
-
-
-def _guarded(*shape, dtype=torch.float32, fill=7.0):
-    """A contiguous output with a sentinel tail: (view, check)."""
-    n = math.prod(shape)
-    buf = torch.full((n + 64,), fill, device="cuda", dtype=dtype)
-    return buf[:n].view(*shape), lambda what: None if torch.equal(buf[n:], torch.full_like(buf[n:], fill)) else \
-        pytest.fail(f"{what}: the sentinel tail was written")
-
-
-def test_every_int8qk_launch_in_wider_buffers(launches):
-    from scail_b200 import ops, sparse
-    g = torch.Generator(device="cuda").manual_seed(9)
-    names = {n for n, _ in launches}
-    assert names == set(OPS), names
-    geoms = {f["L"] for n, f in launches if n == "quant_k_int8"}
-    assert len(geoms) == 2 and any(L % 128 for L in geoms), geoms  # 480x832 ends in a ragged key tile
-    for name, f in launches:
-        what = f"{name} {f}"
-        if name == "rmsnorm_rope_int8q":
-            rows, L, D = f["rows"], f["L"], f["D"]
-            data = (torch.randn(rows, f["buf"][0], device="cuda", generator=g)).to(BF)
-            wq, wk = (torch.randn(D, device="cuda", generator=g) + 1).to(BF), (torch.randn(D, device="cuda", generator=g) + 1).to(BF)
-            buf = Slab(data, f["buf"])
-            q8 = Slab(torch.zeros(rows, D, device="cuda", dtype=torch.int8), f["q8"])
-            qs, chk = _guarded(rows // L, D // 128, f["L_pad"])
-            ops.rmsnorm_rope_int8q(buf.v, L, D, [(f["slabs"][0], wq), (f["slabs"][1], wk)], q8.v, qs)
-            ref = data.clone()
-            ops.rmsnorm_rope(ref, L, D, [(f["slabs"][0], wq), (f["slabs"][1], wk)])
-            qr, sr = heads_ref(ref[:, f["slabs"][0]:f["slabs"][0] + D], rows // L, D // 128, L)
-            assert torch.equal(q8.v, qr) and torch.equal(qs, sr), what
-            assert torch.equal(buf.v, torch.cat([data[:, :f["slabs"][1]], ref[:, f["slabs"][1]:]], 1)), what
-            buf.check(what), q8.check(what), chk(what)
-        elif name == "quant_k_int8":
-            B, H, L = f["B"], f["H"], f["L"]
-            d = H * 128
-            k = Slab(torch.randn(B * L, d, device="cuda", generator=g).to(BF), f["k"])
-            k8 = Slab(torch.zeros(B * L, d, device="cuda", dtype=torch.int8), f["k8"])
-            ks, c1 = _guarded(B, H, pad(L))
-            kb, c2 = _guarded(B, d)
-            part, c3 = _guarded(ops.quant_k_int8_partial_len(B, H, L), dtype=torch.float64)
-            ops.quant_k_int8(k.v, B, H, L, k8.v, ks, kb, part)
-            kp = (k.v.float().view(B, L, d) - kb[:, None, :]).view(B * L, d)
-            kr, ksr = heads_ref(kp, B, H, L)
-            want_bar = kbar_fp64(k.v, B, L)
-            assert ((kb - want_bar).abs() <= ulp_f32(want_bar)).all(), what
-            assert torch.equal(k8.v, kr) and torch.equal(ks, ksr), what
-            for c in (k.check, k8.check, c1, c2, c3):
-                c(what)
-        else:
-            B, H, L = f["B"], f["H"], f["L"]
-            d = H * 128
-            qkv = (torch.randn(B * L, 3 * d, device="cuda", generator=g)).to(BF)
-            o = operands(qkv, B, H, L)
-            qi, qis, ki, kis = o["i8"]
-            q = Slab(qi, f["q"])
-            k = Slab(ki, f["k"])
-            out = Slab(torch.zeros(B * L, d, device="cuda", dtype=BF), f["out"])
-            compact = torch.empty(B * L, d, device="cuda", dtype=BF)
-            kw = {}
-            if f["bh"]:
-                ws = {}
-                kw["bh_maps"] = sparse.AdaptiveTiles(0.9, 40).select(qi, ki, B, H, L, 100, lambda nm, sh, dt: ws.setdefault(
-                    nm, torch.empty(sh, device="cuda", dtype=dt)), q_scale=qis, k_scale=kis)
-            elif f["tiles"]:
-                n = -(-L // 128)
-                ptr, idx = [0], []
-                for t in range(n):
-                    idx += sorted({0} | {j for j in (t - 2, t - 1, t, t + 1, t + 2) if 0 <= j < n})
-                    ptr.append(len(idx))
-                kw["tiles"] = ops.TileMap(ptr, idx, L, L, device="cuda")
-            ops.attention_int8qk(q.v, qis, k.v, kis, *o["v"], out.v, B, H, L, **kw)
-            ops.attention_int8qk(qi, qis, ki, kis, *o["v"], compact, B, H, L, **kw)
-            assert torch.equal(out.v, compact), what
-            assert torch.isfinite(compact.float()).all(), what
-            for c in (q.check, k.check, out.check):
-                c(what)
-        print(f"{what}: exact, sentinels intact")
 
 
 # ---------------------------------------------------------------- the ABI refuses bad arguments

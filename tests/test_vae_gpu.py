@@ -96,6 +96,21 @@ def test_vae_elementwise():
     assert rel(ops.vae_latent_to_cl(z, mean, inv), want) < 4e-3
 
 
+@pytest.mark.parametrize("h,w", [(64, 64), (60, 104), (64, 112)])
+def test_latent_to_cl_at_the_production_latents(h, w):
+    """The decoder's first launch at the 21-frame latents of 512x512, 480x832 and 512x896: bit for bit one IEEE division
+    and one addition in fp32, rounded once to bf16, at every (channel, frame, row, column)."""
+    from scail_b200 import ops
+    z = rnd(16, 21, h, w, seed=h + w, scale=3.0)
+    g = torch.Generator(device="cuda").manual_seed(w)
+    mean = torch.randn(16, device="cuda", generator=g)
+    inv = torch.rand(16, device="cuda", generator=g) + 0.5
+    want = (z.float() / inv.view(16, 1, 1, 1) + mean.view(16, 1, 1, 1)).permute(1, 2, 3, 0).to(torch.bfloat16)
+    got = ops.vae_latent_to_cl(z, mean, inv)
+    assert got.shape == (21, h, w, 16)
+    assert torch.equal(got.view(torch.int16), want.view(torch.int16)), int((got != want).sum())
+
+
 def test_vae_decode_against_reference_golden():
     from scail_b200.wan_vae import WanVAE
     g = torch.load(os.path.join(GOLD, "vae_small.pt"))
