@@ -64,6 +64,22 @@ int scail_gemm_fp8(const void* A, int64_t lda, const void* W, int64_t ldw, const
  * ldx % 8 == 0; x and q 16-byte aligned. */
 int scail_quant_rows_fp8(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream);
 
+/* fp8_linear="int8": the linears' INT8 row format is the one of fp8_attention="int8_qk" (see scail_rmsnorm_rope_int8q),
+ * one scale per row: scale[m] = amax(|x[m, :K]|) / 127 (IEEE division; 1 for an all-zero row), q[m, k] =
+ * round-half-even(x[m, k] / scale[m]) saturated to [-127, 127].
+ *
+ * INT8 GEMM: C[M,N] = epilogue((float(A_q[M,K] @ W_q[N,K]^T) * scale_a[m]) * scale_w[n]).  The product is accumulated
+ * exactly in s32 and converted once (round to nearest); then the same epilogues, in the same order, as scail_gemm_bf16.
+ * A_q, W_q are int8 codes with leading dims lda/ldw in elements; K, lda, ldw must be multiples of 16 and K <= 131072
+ * (K * 127^2 < 2^31).  Scales, C, bias, gate, residual and the bf16-only output as for scail_gemm_fp8. */
+int scail_gemm_int8(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
+                    int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
+                    int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, const float* scale_a,
+                    const float* scale_w, scail_stream_t stream);
+
+/* Row-wise INT8 quantisation in the format above: x, q, scale and the limits as for scail_quant_rows_fp8, q int8 [M, K]. */
+int scail_quant_rows_int8(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream);
+
 /* out = modulate(LayerNorm(x)) per row.  gamma/beta (bf16 [D]) and shift/scale (bf16 [B, mod_stride])
  * are optional (NULL).  Reads rows [in_row_offset, in_row_offset+rows_out) of each batch of
  * in_batch_rows rows; writes [B*rows_out, D] densely.  D % 8 == 0, D <= 5120.
@@ -77,6 +93,11 @@ int scail_ln_modulate(const void* x, void* out, const void* gamma, const void* b
 int scail_ln_modulate_fp8(const void* x, void* out_q, float* out_scale, const void* gamma, const void* beta, const void* shift,
                           const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
                           int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream);
+/* The same rows quantised for scail_gemm_int8: out_q int8 [B*rows_out, D], out_scale as for scail_ln_modulate_fp8, equal
+ * bit for bit to scail_quant_rows_int8 of what scail_ln_modulate writes.  D % 16 == 0. */
+int scail_ln_modulate_int8(const void* x, void* out_q, float* out_scale, const void* gamma, const void* beta, const void* shift,
+                           const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
+                           int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream);
 
 /* In-place RMSNorm over D columns (fp32 math, affine weight) of 1 or 2 column slabs of a
  * [rows, ld] bf16 matrix, optionally followed by interleaved-pair RoPE with per-token fp32

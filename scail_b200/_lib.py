@@ -27,8 +27,12 @@ SIGNATURES = {
     "scail_gemm_fp8": [c_p, c_i64, c_p, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_p, c_i64, c_i64, c_p,
                        c_i64, c_int, c_p, c_p, c_p],
     "scail_quant_rows_fp8": [c_p, c_i64, c_p, c_p, c_i64, c_i64, c_p],
+    "scail_gemm_int8": [c_p, c_i64, c_p, c_i64, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_p, c_i64, c_i64, c_p,
+                        c_i64, c_int, c_p, c_p, c_p],
+    "scail_quant_rows_int8": [c_p, c_i64, c_p, c_p, c_i64, c_i64, c_p],
     "scail_ln_modulate": [c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
     "scail_ln_modulate_fp8": [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
+    "scail_ln_modulate_int8": [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f, c_p],
     "scail_rmsnorm_rope": [c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_f, c_p],
     "scail_rmsnorm_rope_fp8": [c_p, c_i64, c_i64, c_i64, c_i64, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_f, c_p, c_p, c_p,
                                c_p, c_i64, c_i64, c_p],

@@ -260,7 +260,7 @@ class CFGCache:
     def cond_forward(self, model, x, timesteps, context, kw):
         """The conditional-only forward, model(x, timesteps=timesteps, context=context, **kw) with x [1, ...] and context
         the cond row, on stream() after everything enqueued on the current stream; the current stream then waits for it.
-        With fp8_linear the e4m3 weights are brought up to date on the current stream first.  -> v bf16 [1, ...]."""
+        With fp8_linear the 8-bit weights of its mode are brought up to date on the current stream first.  -> v bf16 [1, ...]."""
         dev = x.device
         main = torch.cuda.current_stream(dev)
         side = self.stream(dev)

@@ -236,14 +236,16 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tw, const CUten
     return 0;
 }
 
-template <int EPI>
-static int launch_gemm_fp8(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const CUtensorMap& tr,
-                           const scail::GemmParams& p, int grid, cudaStream_t st) {
+// OP: GEMM_OP_E4M3 (gemm_fp8_kernel) or GEMM_OP_INT8 (gemm_int8_kernel)
+template <int OP, int EPI>
+static int launch_gemm_scaled(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tc, const CUtensorMap& tr,
+                              const scail::GemmParams& p, int grid, cudaStream_t st) {
     using namespace scail;
-    constexpr int smem = GemmCfg<true>::SMEM_BYTES;
+    constexpr int smem = GemmCfg<OP>::SMEM_BYTES;
+    auto kernel = OP == GEMM_OP_INT8 ? gemm_int8_kernel<EPI> : gemm_fp8_kernel<EPI>;
     int rc;
-    if ((rc = set_smem(gemm_fp8_kernel<EPI>, smem))) return rc;
-    gemm_fp8_kernel<EPI><<<grid, GEMM_THREADS, smem, st>>>(ta, tw, tc, tr, p);
+    if ((rc = set_smem(kernel, smem))) return rc;
+    kernel<<<grid, GEMM_THREADS, smem, st>>>(ta, tw, tc, tr, p);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -333,26 +335,32 @@ int scail_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, cons
     }
 }
 
-int scail_gemm_fp8(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
-                   int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
-                   int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, const float* scale_a,
-                   const float* scale_w, scail_stream_t stream) {
+}  // extern "C"
+
+// scail_gemm_fp8 and scail_gemm_int8: the same checks and launch on 1-byte operands; `what` names the entry point
+template <int OP>
+static int gemm_scaled_impl(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
+                            int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
+                            int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, const float* scale_a,
+                            const float* scale_w, scail_stream_t stream, const char* what) {
     using namespace scail;
-    using Cfg = GemmCfg<true>;
-    SCAIL_REQUIRE(A && W && C && scale_a && scale_w, "gemm_fp8: null operand");
-    SCAIL_REQUIRE(!c_fp32, "gemm_fp8: the output is bf16 (c_fp32 must be 0)");
-    SCAIL_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
+    using Cfg = GemmCfg<OP>;
+    SCAIL_REQUIRE(A && W && C && scale_a && scale_w, "%s: null operand", what);
+    SCAIL_REQUIRE(!c_fp32, "%s: the output is bf16 (c_fp32 must be 0)", what);
+    SCAIL_REQUIRE(M > 0 && N > 0 && K > 0, "%s: bad shape M=%lld N=%lld K=%lld", what, (long long)M, (long long)N, (long long)K);
     SCAIL_REQUIRE(K % 16 == 0 && lda % 16 == 0 && ldw % 16 == 0,
-                  "gemm_fp8: K, lda and ldw must be multiples of 16 (16-byte e4m3 row pitch)");
-    SCAIL_REQUIRE(N % 8 == 0 && ldc % 8 == 0, "gemm_fp8: N and ldc must be multiples of 8");
+                  "%s: K, lda and ldw must be multiples of 16 (16-byte %s row pitch)", what, OP == GEMM_OP_INT8 ? "int8" : "e4m3");
+    // int8: the s32 accumulator is exact while K * 127^2 < 2^31
+    if (OP == GEMM_OP_INT8) SCAIL_REQUIRE(K <= 131072, "%s: K=%lld exceeds 131072 (s32 accumulator range)", what, (long long)K);
+    SCAIL_REQUIRE(N % 8 == 0 && ldc % 8 == 0, "%s: N and ldc must be multiples of 8", what);
     SCAIL_REQUIRE(aligned16(C) && aligned16(bias) && aligned16(gate) && aligned16(residual),
-                  "gemm_fp8: C, bias, gate and residual must be 16-byte aligned (the epilogue uses 16-byte accesses)");
+                  "%s: C, bias, gate and residual must be 16-byte aligned (the epilogue uses 16-byte accesses)", what);
     SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(scale_a) & 3) == 0 && (reinterpret_cast<uintptr_t>(scale_w) & 3) == 0,
-                  "gemm_fp8: scales must be 4-byte aligned float32");
-    SCAIL_REQUIRE(epilogue >= 0 && epilogue <= 5, "gemm_fp8: unknown epilogue %d", epilogue);
-    if (epilogue == EPI_BIAS_GATE_RES) SCAIL_REQUIRE(gate && residual && gate_stride % 8 == 0, "gemm_fp8: gate/residual required");
-    if (epilogue == EPI_BIAS_RES) SCAIL_REQUIRE(residual, "gemm_fp8: residual required");
-    if (residual) SCAIL_REQUIRE(ldr % 8 == 0, "gemm_fp8: ldr must be a multiple of 8");
+                  "%s: scales must be 4-byte aligned float32", what);
+    SCAIL_REQUIRE(epilogue >= 0 && epilogue <= 5, "%s: unknown epilogue %d", what, epilogue);
+    if (epilogue == EPI_BIAS_GATE_RES) SCAIL_REQUIRE(gate && residual && gate_stride % 8 == 0, "%s: gate/residual required", what);
+    if (epilogue == EPI_BIAS_RES) SCAIL_REQUIRE(residual, "%s: residual required", what);
+    if (residual) SCAIL_REQUIRE(ldr % 8 == 0, "%s: ldr must be a multiple of 8", what);
     const bool res_epi = epilogue == EPI_BIAS_GATE_RES || epilogue == EPI_BIAS_RES;
     CUtensorMap ta, tw, tc, tr;
     int rc;
@@ -366,7 +374,7 @@ int scail_gemm_fp8(const void* A, int64_t lda, const void* W, int64_t ldw, const
     p.scale_a = scale_a;
     p.scale_w = scale_w;
     const int sms = sm_count();
-    SCAIL_REQUIRE(sms > 0, "gemm_fp8: no CUDA device");
+    SCAIL_REQUIRE(sms > 0, "%s: no CUDA device", what);
     if ((rc = make_tmap_2d(A, M, K, lda, Cfg::BM, Cfg::BK, &ta, 1))) return rc;
     if ((rc = make_tmap_2d(W, N, K, ldw, Cfg::BN, Cfg::BK, &tw, 1))) return rc;
     if ((rc = make_tmap_2d(C, M, N, ldc, 64, 64, &tc))) return rc;
@@ -379,36 +387,69 @@ int scail_gemm_fp8(const void* A, int64_t lda, const void* W, int64_t ldw, const
     const int grid = num_tiles < sms ? num_tiles : sms;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     switch (epilogue) {
-        case EPI_BIAS: return launch_gemm_fp8<EPI_BIAS>(ta, tw, tc, tr, p, grid, st);
-        case EPI_BIAS_GELU: return launch_gemm_fp8<EPI_BIAS_GELU>(ta, tw, tc, tr, p, grid, st);
-        case EPI_BIAS_SILU: return launch_gemm_fp8<EPI_BIAS_SILU>(ta, tw, tc, tr, p, grid, st);
-        case EPI_BIAS_GELU_ERF: return launch_gemm_fp8<EPI_BIAS_GELU_ERF>(ta, tw, tc, tr, p, grid, st);
-        case EPI_BIAS_GATE_RES: return launch_gemm_fp8<EPI_BIAS_GATE_RES>(ta, tw, tc, tr, p, grid, st);
-        default: return launch_gemm_fp8<EPI_BIAS_RES>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS: return launch_gemm_scaled<OP, EPI_BIAS>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GELU: return launch_gemm_scaled<OP, EPI_BIAS_GELU>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_SILU: return launch_gemm_scaled<OP, EPI_BIAS_SILU>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GELU_ERF: return launch_gemm_scaled<OP, EPI_BIAS_GELU_ERF>(ta, tw, tc, tr, p, grid, st);
+        case EPI_BIAS_GATE_RES: return launch_gemm_scaled<OP, EPI_BIAS_GATE_RES>(ta, tw, tc, tr, p, grid, st);
+        default: return launch_gemm_scaled<OP, EPI_BIAS_RES>(ta, tw, tc, tr, p, grid, st);
     }
 }
 
-int scail_quant_rows_fp8(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream) {
+template <bool INT8>
+static int quant_rows_impl(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream,
+                           const char* what) {
     using namespace scail;
-    SCAIL_REQUIRE(x && q && scale, "quant_rows_fp8: null operand");
+    SCAIL_REQUIRE(x && q && scale, "%s: null operand", what);
     SCAIL_REQUIRE(M > 0 && K > 0 && K % 16 == 0 && ldx % 8 == 0 && aligned16(x) && aligned16(q),
-                  "quant_rows_fp8: K must be a multiple of 16, ldx of 8, x and q 16-byte aligned");
-    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(scale) & 3) == 0, "quant_rows_fp8: scale must be 4-byte aligned float32");
+                  "%s: K must be a multiple of 16, ldx of 8, x and q 16-byte aligned", what);
+    SCAIL_REQUIRE((reinterpret_cast<uintptr_t>(scale) & 3) == 0, "%s: scale must be 4-byte aligned float32", what);
     auto xp = static_cast<const __nv_bfloat16*>(x);
     auto qp = static_cast<uint8_t*>(q);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int vpt = blocks_for(K / 8, ROW_THREADS);  // 16-byte vectors per thread
-    if (vpt <= 4) quant_rows_fp8_kernel<4><<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
-    else if (vpt <= 8) quant_rows_fp8_kernel<8><<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
-    else if (vpt <= 16) quant_rows_fp8_kernel<16><<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
-    else return fail(-1, "quant_rows_fp8: K=%lld exceeds %d", (long long)K, 16 * ROW_THREADS * 8);
+    auto k4 = INT8 ? quant_rows_int8_kernel<4> : quant_rows_fp8_kernel<4>;
+    auto k8 = INT8 ? quant_rows_int8_kernel<8> : quant_rows_fp8_kernel<8>;
+    auto k16 = INT8 ? quant_rows_int8_kernel<16> : quant_rows_fp8_kernel<16>;
+    if (vpt <= 4) k4<<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
+    else if (vpt <= 8) k8<<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
+    else if (vpt <= 16) k16<<<(unsigned)M, ROW_THREADS, 0, st>>>(xp, ldx, qp, scale, (int)K);
+    else return fail(-1, "%s: K=%lld exceeds %d", what, (long long)K, 16 * ROW_THREADS * 8);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
+extern "C" {
+
+int scail_gemm_fp8(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
+                   int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
+                   int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, const float* scale_a,
+                   const float* scale_w, scail_stream_t stream) {
+    return gemm_scaled_impl<scail::GEMM_OP_E4M3>(A, lda, W, ldw, bias, C, ldc, M, N, K, epilogue, gate, gate_stride,
+                                                 rows_per_batch, residual, ldr, c_fp32, scale_a, scale_w, stream, "gemm_fp8");
+}
+
+int scail_gemm_int8(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, void* C, int64_t ldc,
+                    int64_t M, int64_t N, int64_t K, int epilogue, const void* gate, int64_t gate_stride,
+                    int64_t rows_per_batch, const void* residual, int64_t ldr, int c_fp32, const float* scale_a,
+                    const float* scale_w, scail_stream_t stream) {
+    return gemm_scaled_impl<scail::GEMM_OP_INT8>(A, lda, W, ldw, bias, C, ldc, M, N, K, epilogue, gate, gate_stride,
+                                                 rows_per_batch, residual, ldr, c_fp32, scale_a, scale_w, stream, "gemm_int8");
+}
+
+int scail_quant_rows_fp8(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream) {
+    return quant_rows_impl<false>(x, ldx, q, scale, M, K, stream, "quant_rows_fp8");
+}
+
+int scail_quant_rows_int8(const void* x, int64_t ldx, void* q, float* scale, int64_t M, int64_t K, scail_stream_t stream) {
+    return quant_rows_impl<true>(x, ldx, q, scale, M, K, stream, "quant_rows_int8");
+}
+
+// int8: out_q takes INT8 rows instead of e4m3 ones
 static int ln_modulate_impl(const void* x, void* out, void* out_q, float* out_scale, const void* gamma, const void* beta,
                             const void* shift, const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out,
-                            int64_t in_batch_rows, int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream) {
+                            int64_t in_batch_rows, int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream,
+                            bool int8 = false) {
     using namespace scail;
     SCAIL_REQUIRE(D % 8 == 0 && D <= ROW_MAXV * ROW_THREADS * 8, "ln_modulate: D=%lld must be a multiple of 8 and <= %d", (long long)D, ROW_MAXV * ROW_THREADS * 8);
     SCAIL_REQUIRE((gamma == nullptr) == (beta == nullptr) && (shift == nullptr) == (scale == nullptr), "ln_modulate: gamma/beta and shift/scale come in pairs");
@@ -419,7 +460,8 @@ static int ln_modulate_impl(const void* x, void* out, void* out_q, float* out_sc
     p.shift = static_cast<const __nv_bfloat16*>(shift); p.scale = static_cast<const __nv_bfloat16*>(scale);
     p.mod_stride = mod_stride; p.D = (int)D; p.rows_out = (int)rows_out; p.in_batch_rows = (int)in_batch_rows;
     p.in_row_offset = (int)in_row_offset; p.total_rows = (int)(B * rows_out); p.eps = eps;
-    if (out_q) ln_modulate_kernel<true><<<p.total_rows, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    if (out_q && int8) ln_modulate_kernel<false, true><<<p.total_rows, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    else if (out_q) ln_modulate_kernel<true><<<p.total_rows, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
     else ln_modulate_kernel<false><<<p.total_rows, ROW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(p);
     SCAIL_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -441,6 +483,16 @@ int scail_ln_modulate_fp8(const void* x, void* out_q, float* out_scale, const vo
                   "ln_modulate_fp8: D must be a multiple of 16, out_q 16-byte aligned, out_scale 4-byte aligned");
     return ln_modulate_impl(x, nullptr, out_q, out_scale, gamma, beta, shift, scale, mod_stride, B, rows_out, in_batch_rows,
                             in_row_offset, D, eps, stream);
+}
+
+int scail_ln_modulate_int8(const void* x, void* out_q, float* out_scale, const void* gamma, const void* beta, const void* shift,
+                           const void* scale, int64_t mod_stride, int64_t B, int64_t rows_out, int64_t in_batch_rows,
+                           int64_t in_row_offset, int64_t D, float eps, scail_stream_t stream) {
+    SCAIL_REQUIRE(x && out_q && out_scale, "ln_modulate_int8: null operand");
+    SCAIL_REQUIRE(D % 16 == 0 && aligned16(out_q) && (reinterpret_cast<uintptr_t>(out_scale) & 3) == 0,
+                  "ln_modulate_int8: D must be a multiple of 16, out_q 16-byte aligned, out_scale 4-byte aligned");
+    return ln_modulate_impl(x, nullptr, out_q, out_scale, gamma, beta, shift, scale, mod_stride, B, rows_out, in_batch_rows,
+                            in_row_offset, D, eps, stream, true);
 }
 
 int scail_rmsnorm_rope(void* buf, int64_t ld, int64_t rows, int64_t rows_per_batch, int64_t D, int nslabs,

@@ -19,7 +19,15 @@
 //   allocates every warp against the 168 registers of the 384-thread launch bound (setmaxnreg only moves the budget at run
 //   time), so the two accumulators fit at 64 x 128 per warpgroup (64 x 192 spills): the fp8 tile is 128 x 128.  The loader warp also brings the tile's
 //   s_w columns and s_a rows; the scales multiply the accumulator first, then the epilogue runs exactly as for bf16.
+//
+// gemm_int8_kernel is the same again on int8 operands (fp8_linear="int8"): C = epi(f32(sum_k A_q W_q) * s_a[m] * s_w[n]).
+//   The s32 wgmma accumulator is exact (|q| <= 127 and K <= 2^17: |acc| <= 2^17 * 127^2 < 2^31), so there is no promotion: one s32
+//   accumulator lives in registers for the whole K, the same 128 registers per thread as the bf16 kernel's fp32 one, and the
+//   tile, the 3-deep ring of 48 KB stages and the 64 KB staging buffer are the bf16 kernel's.  The epilogue converts with
+//   cvt.rn.f32.s32, applies (acc * s_a) * s_w and continues as the fp8 one.
 #pragma once
+#include <type_traits>
+
 #include "sm90.cuh"
 
 namespace scail {
@@ -41,8 +49,8 @@ struct GemmParams {
     int64_t gate_stride;
     int rows_per_batch;
     int group_m;  // rasterisation: m-blocks per L2 group
-    const float* scale_a;  // fp8 only: [M] scale of each row of A
-    const float* scale_w;  // fp8 only: [N] scale of each row of W
+    const float* scale_a;  // fp8 / int8 only: [M] scale of each row of A
+    const float* scale_w;  // fp8 / int8 only: [N] scale of each row of W
 };
 
 constexpr int GEMM_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: consumers
@@ -50,13 +58,17 @@ constexpr int GEMM_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: co
 // Warpgroup w owns rows [64 w, 64 w + 64) of every chunk, so each warpgroup stores 64-row boxes of its own.
 constexpr int GEMM_OUT_CHUNK_BYTES = 128 * 128;  // 16 KB
 
-// Every k-block row is 128 bytes (64 bf16 or 128 e4m3 elements).
-template <bool FP8>
+// Operand formats of gemm_body.  Every k-block row is 128 bytes (64 bf16, or 128 e4m3 or int8 elements).
+enum GemmOperand : int { GEMM_OP_BF16 = 0, GEMM_OP_E4M3 = 1, GEMM_OP_INT8 = 2 };
+
+template <int OP>
 struct GemmCfg {
+    static constexpr bool FP8 = OP == GEMM_OP_E4M3;
+    static constexpr bool SCALED = OP != GEMM_OP_BF16;  // per-row fp32 scales of A and W
     static constexpr int BM = 128;
     static constexpr int BN = FP8 ? 128 : 256;
-    static constexpr int BK = FP8 ? 128 : 64;
-    // bf16: 3 stages, the 64 KB output staging tile does not fit beside a 4th 48 KB stage in 227 KB.
+    static constexpr int BK = OP == GEMM_OP_BF16 ? 64 : 128;
+    // bf16 and int8: 3 stages, the 64 KB output staging tile does not fit beside a 4th 48 KB stage in 227 KB.
     // fp8: 5 stages of 32 KB beside a 32 KB staging tile.
     static constexpr int STAGES = FP8 ? 5 : 3;
     static constexpr int A_BYTES = BM * 128;
@@ -66,17 +78,17 @@ struct GemmCfg {
     static constexpr int OUT_OFF = STAGES * STAGE_BYTES;
     static constexpr int BIAS_OFF = OUT_OFF + OUT_CHUNKS * GEMM_OUT_CHUNK_BYTES;  // fp32 [BN], zeros without a bias
     static constexpr int GATE_OFF = BIAS_OFF + BN * 4;           // bf16 [2][BN]: the gate rows of the tile's first two batches
-    static constexpr int SCALE_OFF = GATE_OFF + 2 * BN * 2;      // fp8: fp32 s_w [BN], then s_a [BM]
-    static constexpr int BAR_OFF = SCALE_OFF + (FP8 ? (BN + BM) * 4 : 0);
+    static constexpr int SCALE_OFF = GATE_OFF + 2 * BN * 2;      // fp8 / int8: fp32 s_w [BN], then s_a [BM]
+    static constexpr int BAR_OFF = SCALE_OFF + (SCALED ? (BN + BM) * 4 : 0);
     static constexpr int SMEM_BYTES = BAR_OFF + 128 /*barriers*/ + 1024 /*align*/;
     static_assert(SMEM_BYTES <= 232448, "gemm: shared memory budget");
     static_assert(OUT_OFF % 1024 == 0 && A_BYTES % 1024 == 0 && STAGE_BYTES % 1024 == 0,
                   "gemm: TMA SWIZZLE_128B destinations must be 1024-B aligned");
 };
-constexpr int GEMM_BM = GemmCfg<false>::BM;
-constexpr int GEMM_BN = GemmCfg<false>::BN;
-constexpr int GEMM_BK = GemmCfg<false>::BK;
-constexpr int GEMM_SMEM_BYTES = GemmCfg<false>::SMEM_BYTES;
+constexpr int GEMM_BM = GemmCfg<GEMM_OP_BF16>::BM;
+constexpr int GEMM_BN = GemmCfg<GEMM_OP_BF16>::BN;
+constexpr int GEMM_BK = GemmCfg<GEMM_OP_BF16>::BK;
+constexpr int GEMM_SMEM_BYTES = GemmCfg<GEMM_OP_BF16>::SMEM_BYTES;
 
 __device__ __forceinline__ void gemm_tile_coords(int tile, int num_m, int num_n, int group_m, int& m_blk, int& n_blk) {
     int per_group = group_m * num_n;
@@ -97,23 +109,24 @@ __device__ __forceinline__ float epi_act(float v) {
 }
 
 // F32: fp32 output (no residual epilogues, bf16 only).  The fp32 tile is twice the staging buffer, so it is stored in two
-// 128-column passes.  FP8: e4m3 operands with per-row scales (gemm_fp8_kernel).
-template <int EPI, bool F32, bool FP8>
+// 128-column passes.  OP: the operand format; e4m3 (gemm_fp8_kernel) and int8 (gemm_int8_kernel) carry per-row scales.
+template <int EPI, bool F32, int OP>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w, const CUtensorMap& tmap_c,
                                           const CUtensorMap& tmap_r, const GemmParams& p) {
-    using C = GemmCfg<FP8>;
+    using C = GemmCfg<OP>;
+    constexpr bool FP8 = C::FP8, INT8 = OP == GEMM_OP_INT8, SCALED = C::SCALED;
     constexpr int GEMM_BN = C::BN, GEMM_BK = C::BK, GEMM_STAGES = C::STAGES;
     constexpr int GEMM_A_BYTES = C::A_BYTES, GEMM_STAGE_BYTES = C::STAGE_BYTES;
     constexpr bool RES = EPI == EPI_BIAS_GATE_RES || EPI == EPI_BIAS_RES;
     constexpr bool GATE = EPI == EPI_BIAS_GATE_RES;
     static_assert(!(F32 && RES), "gemm: the residual epilogues write bf16");
-    static_assert(!(F32 && FP8), "gemm: the fp8 GEMM writes bf16");
+    static_assert(!(F32 && SCALED), "gemm: the fp8 and int8 GEMMs write bf16");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
     const uint32_t out_base = smem_base + C::OUT_OFF;
     const uint32_t bias_base = smem_base + C::BIAS_OFF;
-    const uint32_t scale_base = smem_base + C::SCALE_OFF;  // fp8: s_w [BN] then s_a [BM]
+    const uint32_t scale_base = smem_base + C::SCALE_OFF;  // fp8 / int8: s_w [BN] then s_a [BM]
     const uint32_t bar_base = smem_base + C::BAR_OFF;
     // barrier layout (8 B each): full[S], empty[S], epi_full, epi_empty, res_full, out_free
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
@@ -195,7 +208,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                         }
                     }
                 }
-                if constexpr (FP8) {  // zeros outside [M, N]: those rows and columns are clipped by the store anyway
+                if constexpr (SCALED) {  // zeros outside [M, N]: those rows and columns are clipped by the store anyway
                     float* sw_s = reinterpret_cast<float*>(smem + C::SCALE_OFF);
                     float* sa_s = sw_s + GEMM_BN;
                     for (int i = lane; i < GEMM_BN; i += 32) sw_s[i] = n0 + i < p.N ? p.scale_w[n0 + i] : 0.f;
@@ -242,7 +255,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         };
         int stage = 0;
         uint32_t phase = 0;
-        float acc[GEMM_BN / 2];
+        // int8: s32 accumulator bits
+        std::conditional_t<INT8, uint32_t, float> acc[GEMM_BN / 2];
         [[maybe_unused]] float part[FP8 ? GEMM_BN / 2 : 1];  // fp8: one k-block's wgmma accumulator
         int it = 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
@@ -272,8 +286,13 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                 } else {
                     fence_regs(acc);
                     wgmma_fence();
+                    if constexpr (INT8) {
 #pragma unroll
-                    for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<GEMM_BN>(acc, da + 2 * k, db + 2 * k, 1);
+                        for (int k = 0; k < GEMM_BK / 32; ++k) wgmma_ss_s8<GEMM_BN>(acc, da + 2 * k, db + 2 * k);
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<GEMM_BN>(acc, da + 2 * k, db + 2 * k, 1);
+                    }
                     wgmma_commit();
                     wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
                     fence_regs(acc);
@@ -314,8 +333,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                     }
                 }
             }
-            [[maybe_unused]] float srow[2];  // fp8: s_a of rows r0 and r0 + 8
-            if constexpr (FP8) {
+            [[maybe_unused]] float srow[2];  // fp8 / int8: s_a of rows r0 and r0 + 8
+            if constexpr (SCALED) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h) srow[h] = lds_f1(scale_base + 4 * (GEMM_BN + wg * 64 + r0 + 8 * h));
             }
@@ -335,7 +354,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                 }
             };
             // G accumulator column groups (8 G columns) at a time: their shared-memory loads are issued together
-            constexpr int G = F32 ? 4 : 8;  // fewer live registers where the fp32 stores need them (no spills)
+            // fewer live registers where the fp32 stores or the int8 scales beside the 128 accumulators need them (no spills)
+            constexpr int G = F32 || INT8 ? 4 : 8;
 #pragma unroll
             for (int cc = 0; cc < GEMM_BN / 8 / G; ++cc) {
                 if constexpr (F32) {
@@ -352,7 +372,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                 for (int jj = 0; jj < G; ++jj) {
                     const int j = G * cc + jj;
                     bb[jj] = lds_f2(bias_base + 4 * (8 * j + 2 * q));
-                    if constexpr (FP8) ss[jj] = lds_f2(scale_base + 4 * (8 * j + 2 * q));
+                    if constexpr (SCALED) ss[jj] = lds_f2(scale_base + 4 * (8 * j + 2 * q));
                     if constexpr (GATE) {
 #pragma unroll
                         for (int h = 0; h < 2; ++h)
@@ -368,8 +388,15 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                     const int j = G * cc + jj;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
-                        float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
-                        if constexpr (FP8) {  // (acc * s_a) * s_w, then the bf16 kernel's epilogue
+                        float a0, a1;
+                        if constexpr (INT8) {  // cvt.rn.f32.s32
+                            a0 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h]));
+                            a1 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h + 1]));
+                        } else {
+                            a0 = acc[4 * j + 2 * h];
+                            a1 = acc[4 * j + 2 * h + 1];
+                        }
+                        if constexpr (SCALED) {  // (acc * s_a) * s_w, then the bf16 kernel's epilogue
                             a0 = __fmul_rn(__fmul_rn(a0, srow[h]), ss[jj].x);
                             a1 = __fmul_rn(__fmul_rn(a1, srow[h]), ss[jj].y);
                         }
@@ -404,7 +431,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                  const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r,
                  const GemmParams p) {
-    gemm_body<EPI, F32, false>(tmap_a, tmap_w, tmap_c, tmap_r, p);
+    gemm_body<EPI, F32, GEMM_OP_BF16>(tmap_a, tmap_w, tmap_c, tmap_r, p);
 }
 
 template <int EPI>
@@ -412,7 +439,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                 const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r,
                 const GemmParams p) {
-    gemm_body<EPI, false, true>(tmap_a, tmap_w, tmap_c, tmap_r, p);
+    gemm_body<EPI, false, GEMM_OP_E4M3>(tmap_a, tmap_w, tmap_c, tmap_r, p);
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_int8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+                 const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r,
+                 const GemmParams p) {
+    gemm_body<EPI, false, GEMM_OP_INT8>(tmap_a, tmap_w, tmap_c, tmap_r, p);
 }
 
 }  // namespace scail

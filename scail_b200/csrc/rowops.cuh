@@ -63,7 +63,8 @@ __device__ __forceinline__ uint2 quant_bf16x8(const uint4 v, float s) {
     return make_uint2(h[0] | (h[1] << 16), h[2] | (h[3] << 16));
 }
 
-// ---- INT8 row format of fp8_attention="int8_qk" (Q and smoothed K): s = amax(|row|) / 127 (IEEE division),
+// ---- INT8 row format of fp8_attention="int8_qk" (Q and smoothed K) and of fp8_linear="int8" (both GEMM operands):
+// s = amax(|row|) / 127 (IEEE division),
 // q = cvt.rni.sat.s8(x / s) in [-127, 127]; an all-zero row gets s = 1 and q = 0.
 // torch: torch.round(x.float() / s[:, None]).clamp(-127, 127).to(torch.int8)  (round-half-even, as cvt.rni)
 constexpr float INT8_QMAX = 127.0f;
@@ -93,10 +94,9 @@ __device__ __forceinline__ uint2 quant_bf16x8_s8(const uint4 v, float s) {
 }
 
 // One 128-thread block per row of a row-strided bf16 [M, K] (K % 16 == 0, K <= 8 * ROW_THREADS * V): the row stays in registers
-// between the amax reduction and the quantisation, so it is read once.
-template <int V>
-__global__ void __launch_bounds__(ROW_THREADS) quant_rows_fp8_kernel(const __nv_bfloat16* x, int64_t ldx, uint8_t* q,
-                                                                      float* scale, int K) {
+// between the amax reduction and the quantisation, so it is read once.  INT8: the INT8 row format instead of e4m3.
+template <int V, bool INT8>
+__device__ __forceinline__ void quant_rows_body(const __nv_bfloat16* x, int64_t ldx, uint8_t* q, float* scale, int K) {
     __shared__ float red[4];
     const int64_t row = blockIdx.x;
     const uint4* xin = reinterpret_cast<const uint4*>(x + row * ldx);
@@ -111,20 +111,32 @@ __global__ void __launch_bounds__(ROW_THREADS) quant_rows_fp8_kernel(const __nv_
             amax = absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(amax, v[j].x), v[j].y), v[j].z), v[j].w);
         }
     }
-    const float s = fp8_row_scale(row_block_max(amax, red));
+    const float s = INT8 ? int8_row_scale(row_block_max(amax, red)) : fp8_row_scale(row_block_max(amax, red));
     if (threadIdx.x == 0) scale[row] = s;
     uint2* o = reinterpret_cast<uint2*>(q + row * K);
 #pragma unroll
     for (int j = 0; j < V; ++j) {
         const int i = j * ROW_THREADS + threadIdx.x;
-        if (i < nvec) o[i] = quant_bf16x8(v[j], s);
+        if (i < nvec) o[i] = INT8 ? quant_bf16x8_s8(v[j], s) : quant_bf16x8(v[j], s);
     }
+}
+
+template <int V>
+__global__ void __launch_bounds__(ROW_THREADS) quant_rows_fp8_kernel(const __nv_bfloat16* x, int64_t ldx, uint8_t* q,
+                                                                      float* scale, int K) {
+    quant_rows_body<V, false>(x, ldx, q, scale, K);
+}
+
+template <int V>
+__global__ void __launch_bounds__(ROW_THREADS) quant_rows_int8_kernel(const __nv_bfloat16* x, int64_t ldx, uint8_t* q,
+                                                                       float* scale, int K) {
+    quant_rows_body<V, true>(x, ldx, q, scale, K);
 }
 
 struct LnModParams {
     const __nv_bfloat16* x;      // input rows
     __nv_bfloat16* out;          // output rows [B*rows_out, D] (bf16 form)
-    uint8_t* out_q;              // fp8 form: e4m3 rows [B*rows_out, D] and their fp32 scales [B*rows_out]
+    uint8_t* out_q;              // fp8 / int8 form: e4m3 or int8 rows [B*rows_out, D] and their fp32 scales [B*rows_out]
     float* out_scale;
     const __nv_bfloat16* gamma;  // optional affine
     const __nv_bfloat16* beta;
@@ -164,8 +176,9 @@ __device__ __forceinline__ float hsum_f32x2(uint64_t v) {
 // Restates F.layer_norm + modulate (dit_video_crossattn_sc_xc.py:760-761, :1031-1032, :1045-1046, :825).
 // The row is unpacked to fp32 pairs once and stays in registers (4 x ROW_MAXV packed f32x2 per thread) for all three passes.
 // FP8: the bf16 row the bf16 form would write is quantised to e4m3 in registers (one more block reduction for its amax),
-// so the result equals quant_rows_fp8 of the bf16 form bit for bit.
-template <bool FP8>
+// so the result equals quant_rows_fp8 of the bf16 form bit for bit.  INT8 (FP8 false): the same in the INT8 row format,
+// equal to quant_rows_int8 of the bf16 form.
+template <bool FP8, bool INT8 = false>
 __global__ void __launch_bounds__(ROW_THREADS) ln_modulate_kernel(const LnModParams p) {
     __shared__ float red[4];
     const int row = blockIdx.x;
@@ -205,7 +218,8 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_modulate_kernel(const LnModPar
     const float rstd = rsqrtf(row_block_sum(hsum_f32x2(acc), red) / p.D + p.eps);
     const uint64_t rstd2 = pack_f32x2(rstd, rstd), one2 = pack_f32x2(1.0f, 1.0f);
     uint4* o = reinterpret_cast<uint4*>(p.out + static_cast<int64_t>(row) * p.D);
-    [[maybe_unused]] uint4 ob[ROW_MAXV];  // fp8: the bf16 row, kept for the quantisation
+    constexpr bool QUANT = FP8 || INT8;
+    [[maybe_unused]] uint4 ob[ROW_MAXV];  // fp8 / int8: the bf16 row, kept for the quantisation
     [[maybe_unused]] float amax = 0.f;
 #pragma unroll
     for (int j = 0; j < ROW_MAXV; ++j) {
@@ -235,7 +249,7 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_modulate_kernel(const LnModPar
             ov.y = f32x2_to_bf16x2(y[1]);
             ov.z = f32x2_to_bf16x2(y[2]);
             ov.w = f32x2_to_bf16x2(y[3]);
-            if constexpr (FP8) {
+            if constexpr (QUANT) {
                 ob[j] = ov;
                 amax = absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(absmax_bf16x2(amax, ov.x), ov.y), ov.z), ov.w);
             } else {
@@ -243,14 +257,14 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_modulate_kernel(const LnModPar
             }
         }
     }
-    if constexpr (FP8) {
-        const float s = fp8_row_scale(row_block_max(amax, red));
+    if constexpr (QUANT) {
+        const float s = INT8 ? int8_row_scale(row_block_max(amax, red)) : fp8_row_scale(row_block_max(amax, red));
         if (threadIdx.x == 0) p.out_scale[row] = s;
         uint2* oq = reinterpret_cast<uint2*>(p.out_q + static_cast<int64_t>(row) * p.D);
 #pragma unroll
         for (int j = 0; j < ROW_MAXV; ++j) {
             const int i = j * ROW_THREADS + threadIdx.x;
-            if (i < nvec) oq[i] = quant_bf16x8(ob[j], s);
+            if (i < nvec) oq[i] = INT8 ? quant_bf16x8_s8(ob[j], s) : quant_bf16x8(ob[j], s);
         }
     }
 }

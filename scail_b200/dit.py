@@ -66,9 +66,10 @@ class _Linear(nn.Module):
         self.weight = nn.Parameter(torch.randn(out_features, in_features) * std)
         self.bias = nn.Parameter(torch.zeros(out_features)) if bias else None
 
-    def __getstate__(self):  # the e4m3 copy (AdaLNMixin.fp8_weight) is derived data holding a weakref: not pickled
+    def __getstate__(self):  # the e4m3 and int8 copies (AdaLNMixin.weight8) are derived data holding a weakref: not pickled
         state = self.__dict__.copy()
         state.pop("_fp8_cache", None)
+        state.pop("_int8_cache", None)
         return state
 
 
@@ -157,6 +158,17 @@ def check_fp8_attention(mode):
     if isinstance(mode, str) and mode != FP8_ATTENTION_INT8_QK:
         raise ValueError(f"fp8_attention must be False, True or {FP8_ATTENTION_INT8_QK!r}, got {mode!r}")
     return mode
+
+
+FP8_LINEAR_INT8 = "int8"
+
+
+def linear_format(mode):
+    """The operand dtype of the six per-block linears for an fp8_linear setting: None (bf16) when it is falsy, torch.int8 for
+    exactly the string "int8" (INT8 codes, DESIGN §3.1.1), and e4m3 for any other truthy value, as it has always been read."""
+    if not mode:
+        return None
+    return ops.INT8 if isinstance(mode, str) and mode == FP8_LINEAR_INT8 else ops.FP8
 
 
 class Conditioning:
@@ -365,7 +377,8 @@ class AdaLNMixin(BaseMixin):
         # Opt-in: the six per-block linears over all tokens (QKV, self-attention out, cross q, cross-attention out, fc1, fc2) run
         # as e4m3 GEMMs with one scale per token and per output channel (scail_gemm_fp8); everything else stays bf16.  The
         # e4m3 weights are derived on the GPU on first use and are not part of the state_dict.  A plain attribute: it can be
-        # toggled between forwards.
+        # toggled between forwards.  "int8": the same six linears as INT8 GEMMs with the same scale layout (scail_gemm_int8,
+        # DESIGN §3.1.1); any other truthy value is e4m3 (linear_format).
         self.fp8_linear = fp8_linear
         # Opt-in, independent of fp8_linear: the self-attention runs on e4m3 Q, K (one scale per token and head) and V (one
         # scale per channel) through attention_fp8_kernel; cross-attention stays bf16.  A plain attribute, like fp8_linear.
@@ -387,54 +400,74 @@ class AdaLNMixin(BaseMixin):
     FP8_LINEARS = ("attention.query_key_value", "attention.dense", "cross_attention.query", "cross_attention.dense",
                    "mlp.dense_h_to_4h", "mlp.dense_4h_to_h")
 
-    def fp8_weight(self, lin, streams=()):
-        """(q e4m3 [out, in], scale fp32 [out]) of `lin.weight`, quantised on the current stream on first use and again
-        whenever the parameter object, its storage or its version has changed (a checkpoint loaded after construction, an
-        in-place edit), so a stale copy is never used.  The copy lives on `lin` (not in the state_dict) with only a weak
-        reference to the weight: a replaced parameter is neither kept alive nor served.  A changed weight of the same shape
-        is re-derived into the same buffers, so the pointers a CUDA graph captured stay valid.  Newly allocated buffers are
-        recorded on `streams`, the other streams that will read them."""
+    def weight8(self, lin, dtype, streams=()):
+        """(q [out, in], scale fp32 [out]) of `lin.weight` in the 8-bit row format of `dtype` (ops.FP8: e4m3, ops.INT8: int8),
+        quantised on the current stream on first use and again whenever the parameter object, its storage or its version has
+        changed (a checkpoint loaded after construction, an in-place edit), so a stale copy is never used.  The copy lives on
+        `lin` (not in the state_dict; one cache per format, so switching modes never frees the other format's buffers) with
+        only a weak reference to the weight: a replaced parameter is neither kept alive nor served.  A changed weight of the
+        same shape is re-derived into the same buffers, so the pointers a CUDA graph captured stay valid.  Newly allocated
+        buffers are recorded on `streams`, the other streams that will read them."""
+        attr = "_int8_cache" if dtype == ops.INT8 else "_fp8_cache"
         w = lin.weight
         tag = (w.data_ptr(), w._version)
-        c = getattr(lin, "_fp8_cache", None)
+        c = getattr(lin, attr, None)
         if c is not None and c[0]() is w and c[1] == tag:
             return c[2], c[3]
         if c is not None and c[2].shape == w.shape and c[2].device == w.device:
             q, sc = ops.quant_rows_fp8(w.detach(), c[2], c[3])
         else:
-            lin._fp8_cache = None  # free the old copy before allocating the new one
-            q, sc = ops.quant_rows_fp8(w.detach())
+            setattr(lin, attr, None)  # free the old copy before allocating the new one
+            if dtype == ops.INT8:
+                q, sc = ops.quant_rows_fp8(w.detach(), torch.empty(w.shape, device=w.device, dtype=ops.INT8),
+                                           torch.empty(w.shape[0], device=w.device, dtype=torch.float32))
+            else:
+                q, sc = ops.quant_rows_fp8(w.detach())
             for st in streams:
                 q.record_stream(st)
                 sc.record_stream(st)
-        lin._fp8_cache = (weakref.ref(w), tag, q, sc)
+        setattr(lin, attr, (weakref.ref(w), tag, q, sc))
         return q, sc
 
-    def prepare_fp8_weights(self, num_layers=None, streams=()):
-        """Bring the e4m3 copies of the first `num_layers` blocks' six linears up to date on the current stream.  Work that
-        reads them on other streams must be ordered after this (DiffusionTransformer.forward does it before the context-parallel
-        branch streams fork).  Returns the copies."""
+    def fp8_weight(self, lin, streams=()):
+        """The e4m3 copy of `lin.weight` (weight8)."""
+        return self.weight8(lin, ops.FP8, streams)
+
+    def prepare_fp8_weights(self, num_layers=None, streams=(), dtype=None):
+        """Bring the 8-bit copies of the first `num_layers` blocks' six linears up to date on the current stream: int8 copies
+        when `dtype` is ops.INT8 (by default: when fp8_linear is "int8"), e4m3 copies otherwise.  Work that reads them on other
+        streams must be ordered after this (DiffusionTransformer.forward does it before the context-parallel branch streams
+        fork).  Returns the copies."""
+        if dtype is None:
+            dtype = ops.INT8 if linear_format(self.fp8_linear) == ops.INT8 else ops.FP8
         out = []
         for layer in list(self.transformer.layers)[:num_layers]:
             for name in self.FP8_LINEARS:
-                out.extend(self.fp8_weight(layer.get_submodule(name), streams))
+                out.extend(self.weight8(layer.get_submodule(name), dtype, streams))
         return out
 
-    def _fp8_act(self, x2, name):
-        """x2 bf16 [M, K] -> its e4m3 rows and scales, in the per-stream workspace `name`."""
+    @staticmethod
+    def _ws8(name, dtype):
+        """Workspace name of 8-bit activations: the int8 buffers have names of their own, so they never alias e4m3 ones."""
+        return name + "_int8" if dtype == ops.INT8 else name
+
+    def _fp8_act(self, x2, name, dtype=ops.FP8):
+        """x2 bf16 [M, K] -> its e4m3 (or int8) rows and scales, in the per-stream workspace `name`."""
         M, K = x2.shape
-        q = _WS.get(name, (M, K), x2.device, ops.FP8)
+        name = self._ws8(name, dtype)
+        q = _WS.get(name, (M, K), x2.device, dtype)
         sc = _WS.get(name + "_scale", (M,), x2.device, torch.float32)
         return ops.quant_rows_fp8(x2, q, sc)
 
     def _linear(self, x2, lin, x_scale=None, out=None, name="act8", **kw):
-        """epilogue(x2 @ lin.weight^T + lin.bias) into `out`.  bf16 GEMM unless fp8_linear; then the e4m3 GEMM, on x2 itself when
-        it is already e4m3 (with its row scales x_scale), else on x2 quantised into workspace `name`."""
-        if not self.fp8_linear:
+        """epilogue(x2 @ lin.weight^T + lin.bias) into `out`.  bf16 GEMM unless fp8_linear; then the e4m3 (or int8) GEMM, on
+        x2 itself when it is already in that format (with its row scales x_scale), else on x2 quantised into workspace `name`."""
+        dt = linear_format(self.fp8_linear)
+        if dt is None:
             return ops.gemm(x2, lin.weight, lin.bias, out=out, **kw)
-        if x2.dtype != ops.FP8:
-            x2, x_scale = self._fp8_act(x2, name)
-        wq, ws = self.fp8_weight(lin)
+        if x2.dtype != dt:
+            x2, x_scale = self._fp8_act(x2, name, dt)
+        wq, ws = self.weight8(lin, dt)
         return ops.gemm_fp8(x2, x_scale, wq, ws, lin.bias, out=out, **kw)
 
     # -- hooks ---------------------------------------------------------------------------------
@@ -456,15 +489,17 @@ class AdaLNMixin(BaseMixin):
         eps = self.layernorm_epsilon
         x2 = x.view(B * N, d)
         mod = ops.adaln_modulation(kwargs["emb"], self.adaLN_modulations[l].view(-1)).view(B, 6, d)  # :1025-1028
-        fp8 = self.fp8_linear
-        if fp8:
-            ln8 = (_WS.get("ln8", (B * N, d), dev, ops.FP8), _WS.get("ln8_scale", (B * N,), dev, torch.float32))
+        dt8 = linear_format(self.fp8_linear)
+        if dt8 is not None:
+            n8 = self._ws8("ln8", dt8)
+            ln8 = (_WS.get(n8, (B * N, d), dev, dt8), _WS.get(n8 + "_scale", (B * N,), dev, torch.float32))
         else:
             lnb = _WS.get("ln", (B, N, d), dev)
 
         def ln(**kw):
-            """The block's LNs feed linears only: with fp8_linear they write e4m3 rows + scales.  -> (rows [B, N, d], scales)"""
-            if fp8:
+            """The block's LNs feed linears only: with fp8_linear they write e4m3 (or int8) rows + scales.
+            -> (rows [B, N, d], scales)"""
+            if dt8 is not None:
                 ops.ln_modulate(x, eps=eps, out_fp8=ln8, **kw)
                 return ln8[0].view(B, N, d), ln8[1]
             return ops.ln_modulate(x, out=lnb, eps=eps, **kw), None
@@ -499,8 +534,8 @@ class AdaLNMixin(BaseMixin):
 
     def attention_forward(self, hidden_states, mask, _ctx_out=None, _fp8_scale=None, **kw_args):
         """:1058-1105.  Returns the out-projected attention output unless `_ctx_out` is given (then the
-        merged-head context is left there for the fused out-proj epilogue of layer_forward).  hidden_states may be e4m3 rows
-        with their scales in `_fp8_scale` (fp8_linear)."""
+        merged-head context is left there for the fused out-proj epilogue of layer_forward).  hidden_states may be e4m3 (or
+        int8) rows with their scales in `_fp8_scale` (fp8_linear)."""
         l = int(kw_args["layer_id"])
         a = self.transformer.layers[l].attention
         B, N, d = hidden_states.shape
@@ -508,8 +543,9 @@ class AdaLNMixin(BaseMixin):
         H = self.num_attention_heads
         cos, sin = self._rope_tables(dev, **kw_args)
         h2 = hidden_states.view(B * N, d)
-        if self.fp8_linear and h2.dtype != ops.FP8:
-            h2, _fp8_scale = self._fp8_act(h2, "ln8")
+        dt8 = linear_format(self.fp8_linear)
+        if dt8 is not None and h2.dtype != dt8:
+            h2, _fp8_scale = self._fp8_act(h2, "ln8", dt8)
         ctx = _ctx_out if _ctx_out is not None else torch.empty(B * N, d, device=dev, dtype=torch.bfloat16)
         wq, wk = self.query_layernorm_list[l].weight, self.key_layernorm_list[l].weight
         if self.cp is None or self.cp.size == 1:
@@ -611,7 +647,7 @@ class AdaLNMixin(BaseMixin):
     def cross_attention_forward(self, hidden_states, cross_attention_mask, encoder_outputs, _ctx_out=None, _fp8_scale=None,
                                 **kw_args):
         """:1107-1203: text K/V and CLIP K/V are two separate softmaxes whose outputs are summed (F4).  hidden_states may be
-        e4m3 rows with their scales in `_fp8_scale` (fp8_linear)."""
+        e4m3 (or int8) rows with their scales in `_fp8_scale` (fp8_linear)."""
         l = int(kw_args["layer_id"])
         c = self.transformer.layers[l].cross_attention
         B, N, d = hidden_states.shape
@@ -816,7 +852,7 @@ class DiffusionTransformer(nn.Module):
         local = hidden if chunk_dim is not None else cp.shard_tokens(hidden)
         main = torch.cuda.current_stream()
         streams = cp.branch_streams(b, x.device)
-        if ad.fp8_linear:  # every branch reads the same e4m3 weights: derive them here, before the branch streams wait on main
+        if ad.fp8_linear:  # every branch reads the same 8-bit weights: derive them here, before the branch streams wait on main
             ad.prepare_fp8_weights(n_layers, streams)
         per = []
         for i in range(b):

@@ -53,12 +53,18 @@ def gemm(a, w, bias=None, out=None, epilogue=EPI_BIAS, gate=None, residual=None,
 
 
 FP8 = torch.float8_e4m3fn
+INT8 = torch.int8
 
 
 def gemm_fp8(a, a_scale, w, w_scale, bias=None, out=None, epilogue=EPI_BIAS, gate=None, residual=None, rows_per_batch=0):
     """out[M,N] (bf16) = epilogue((a[M,K] @ w[N,K]^T) * a_scale[m] * w_scale[n]); a, w e4m3 with fp32 per-row scales (as
-    quant_rows_fp8 makes them).  a/out may be row-strided 2-D views (stride(1)==1), K % 16 == 0."""
-    _req(a, FP8), _req(w, FP8), _req(a_scale, torch.float32), _req(w_scale, torch.float32)
+    quant_rows_fp8 makes them).  a/out may be row-strided 2-D views (stride(1)==1), K % 16 == 0.
+    a and w both int8 (torch.int8 codes in the INT8 row format, quant_rows_fp8 with an int8 q): the INT8 GEMM
+    (scail_gemm_int8), the product exact in s32, K <= 131072.  Mixed operand dtypes raise TypeError."""
+    int8 = a.dtype == INT8
+    if int8 != (w.dtype == INT8):
+        raise TypeError(f"gemm_fp8: a and w must both be e4m3 or both be int8, got {a.dtype} and {w.dtype}")
+    _req(a, INT8 if int8 else FP8), _req(w, INT8 if int8 else FP8), _req(a_scale, torch.float32), _req(w_scale, torch.float32)
     M, K = a.shape
     N = w.shape[0]
     assert w.shape[1] == K and a.stride(1) == 1 and w.stride(1) == 1
@@ -68,17 +74,19 @@ def gemm_fp8(a, a_scale, w, w_scale, bias=None, out=None, epilogue=EPI_BIAS, gat
     _req(out)
     assert out.shape == (M, N) and out.stride(1) == 1
     gs = gate.stride(0) if gate is not None else 0
-    _lib.check(_lib.lib().scail_gemm_fp8(
+    name = "scail_gemm_int8" if int8 else "scail_gemm_fp8"
+    _lib.check(getattr(_lib.lib(), name)(
         _ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(bias), _ptr(out), out.stride(0), M, N, K, epilogue,
         _ptr(gate), gs, rows_per_batch, _ptr(residual), residual.stride(0) if residual is not None else 0, 0,
-        _ptr(a_scale), _ptr(w_scale), _stream()), "scail_gemm_fp8")
+        _ptr(a_scale), _ptr(w_scale), _stream()), name)
     _count()
     return out
 
 
 def quant_rows_fp8(x, q=None, scale=None):
     """Row-wise e4m3: x bf16 [M, K] (row-strided 2-D view) -> (q e4m3 [M, K], scale fp32 [M]) with scale = amax(|row|) / 448
-    (1 for an all-zero row) and q = satfinite_rn(x / scale)."""
+    (1 for an all-zero row) and q = satfinite_rn(x / scale).  An int8 q selects the INT8 row format (scail_quant_rows_int8):
+    scale = amax(|row|) / 127 (1 for an all-zero row) and q = round-half-even(x / scale) saturated to [-127, 127]."""
     _req(x)
     assert x.dim() == 2 and x.stride(1) == 1
     M, K = x.shape
@@ -86,10 +94,11 @@ def quant_rows_fp8(x, q=None, scale=None):
         q = torch.empty(M, K, device=x.device, dtype=FP8)
     if scale is None:
         scale = torch.empty(M, device=x.device, dtype=torch.float32)
-    _req(q, FP8), _req(scale, torch.float32)
+    int8 = q.dtype == INT8
+    _req(q, INT8 if int8 else FP8), _req(scale, torch.float32)
     assert q.shape == (M, K) and q.is_contiguous() and scale.shape == (M,) and scale.is_contiguous()
-    _lib.check(_lib.lib().scail_quant_rows_fp8(_ptr(x), x.stride(0), _ptr(q), _ptr(scale), M, K, _stream()),
-               "scail_quant_rows_fp8")
+    name = "scail_quant_rows_int8" if int8 else "scail_quant_rows_fp8"
+    _lib.check(getattr(_lib.lib(), name)(_ptr(x), x.stride(0), _ptr(q), _ptr(scale), M, K, _stream()), name)
     _count()
     return q, scale
 
@@ -98,7 +107,8 @@ def ln_modulate(x, out=None, gamma=None, beta=None, shift=None, scale=None, eps=
                 out_fp8=None):
     """x [B, Nin, D] -> out [B, rows_out, D] = modulate(LN(x[:, row_offset:row_offset+rows_out])).
     out_fp8=(q, s): write that result quantised instead, q e4m3 [B*rows_out, D] and s fp32 [B*rows_out] (bit for bit
-    quant_rows_fp8 of the bf16 result), and return (q, s)."""
+    quant_rows_fp8 of the bf16 result), and return (q, s).  An int8 q writes the INT8 row format instead
+    (scail_ln_modulate_int8, bit for bit quant_rows_fp8 of the bf16 result into an int8 q)."""
     _req(x)
     B, n_in, D = x.shape
     rows_out = n_in if rows_out is None else rows_out
@@ -109,11 +119,12 @@ def ln_modulate(x, out=None, gamma=None, beta=None, shift=None, scale=None, eps=
     if out_fp8 is not None:
         assert out is None
         q, s = out_fp8
-        _req(q, FP8), _req(s, torch.float32)
+        int8 = q.dtype == INT8
+        _req(q, INT8 if int8 else FP8), _req(s, torch.float32)
         assert q.is_contiguous() and q.numel() == B * rows_out * D and s.is_contiguous() and s.numel() == B * rows_out
-        _lib.check(_lib.lib().scail_ln_modulate_fp8(_ptr(x), _ptr(q), _ptr(s), _ptr(gamma), _ptr(beta), _ptr(shift),
-                                                    _ptr(scale), ms, B, rows_out, n_in, row_offset, D, eps, _stream()),
-                   "scail_ln_modulate_fp8")
+        name = "scail_ln_modulate_int8" if int8 else "scail_ln_modulate_fp8"
+        _lib.check(getattr(_lib.lib(), name)(_ptr(x), _ptr(q), _ptr(s), _ptr(gamma), _ptr(beta), _ptr(shift),
+                                             _ptr(scale), ms, B, rows_out, n_in, row_offset, D, eps, _stream()), name)
         _count()
         return out_fp8
     if out is None:
@@ -159,9 +170,6 @@ def rmsnorm_rope(buf, rows_per_batch, D, slabs, cos=None, sin=None, eps=1e-6, ou
                "scail_rmsnorm_rope")
     _count()
     return buf
-
-
-INT8 = torch.int8
 
 
 def rmsnorm_rope_int8q(buf, rows_per_batch, D, slabs, q8, q_scale, cos=None, sin=None, eps=1e-6):

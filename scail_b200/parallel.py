@@ -126,8 +126,8 @@ class ContextParallel:
     def self_attention(self, mixin, attn, h2, B, n_local, d, H, wq, wk, cos, sin, ctx, tables_local=False, h_scale=None):
         """tables_local: cos/sin already describe this rank's tokens (engine-style pre-chunked latents whose RoPE offsets
         come from rope_H/W_shift); otherwise they cover the full sequence and this rank's contiguous slice is taken.
-        Keys/values are gathered in rank order either way (softmax is order-free).  h2 e4m3 with row scales h_scale
-        (mixin.fp8_linear): the K, V and Q projections are fp8 GEMMs on row slices of the e4m3 QKV weight."""
+        Keys/values are gathered in rank order either way (softmax is order-free).  h2 e4m3 (or int8) with row scales h_scale
+        (mixin.fp8_linear): the K, V and Q projections are 8-bit GEMMs on row slices of the QKV weight's copy in that format."""
         dev = h2.device
         P = self.size
         eps = mixin.layernorm_epsilon
@@ -141,11 +141,12 @@ class ContextParallel:
                                  "tokens must be sharded with shard_tokens() (or pass chunk_dim for pre-chunked latents)")
             cos_l, sin_l = self.rope_slice(cos, sin, n_local)
         w, bias = attn.query_key_value.weight, attn.query_key_value.bias
-        if h2.dtype == ops.FP8:
-            w8, ws8 = mixin.fp8_weight(attn.query_key_value)
+        q8 = h2.dtype in (ops.FP8, ops.INT8)
+        if q8:
+            w8, ws8 = mixin.weight8(attn.query_key_value, h2.dtype)
 
         def proj(rows, cols, out):  # out = h2[rows] @ w[cols]^T + bias[cols]; per-row scales slice with the rows
-            if h2.dtype == ops.FP8:
+            if q8:
                 return ops.gemm_fp8(h2[rows], h_scale[rows], w8[cols], ws8[cols], bias[cols], out=out)
             return ops.gemm(h2[rows], w[cols], bias[cols], out=out)
         # K and V travel separately so that the K gather is already in flight during the V (and Q) projection and the V gather

@@ -237,8 +237,9 @@ class GraphedStep:
     The graph runs in the `fp8_linear`, `fp8_attention`, `attention_window` and `attention_adaptive` modes of construction
     time; a window's tile map is held by scail_b200.sparse for the life of the process, so the graph reads it at a fixed
     address.  attention_adaptive selects its maps on the device on every replay (tile pooling and selection are captured
-    kernels writing the per-stream workspace), so they follow the replayed step's Q and K.  With fp8 it reads the e4m3 weight copies in place: every
-    call first re-derives, into the same buffers, the copies of weights that changed since (e.g. after load_state_dict).
+    kernels writing the per-stream workspace), so they follow the replayed step's Q and K.  With fp8 it reads the e4m3 weight copies in place
+    (the int8 ones with fp8_linear="int8"): every call first re-derives, into the same buffers, the copies of weights that
+    changed since (e.g. after load_state_dict).
     step_cache (a scail_b200.step_cache.FirstBlockCache): the step runs as three graphs with the host's skip decision between
     them (bit-identical to sampler_step with the same cache and thresholds).  The cache is reset at construction; when its
     buffers are dropped or replaced later (reset(), another geometry) the graphs are captured again, and the next step
@@ -274,8 +275,10 @@ class GraphedStep:
         assert ops.ATTN_EVENTS is None, "event timing of individual launches cannot be captured"
         self.adaln = model.mixins["adaln_layer"]
         self.fp8 = getattr(self.adaln, "fp8_linear", False)
-        # the e4m3 weights are derived on this stream and held here: the graph replays against these very buffers
-        self._fp8_weights = self.adaln.prepare_fp8_weights() if self.fp8 else []
+        # the 8-bit weights (e4m3, or int8 for fp8_linear="int8") are derived on this stream and held here: the graph replays
+        # against these very buffers
+        self._w8_dtype = ops.INT8 if dit.linear_format(self.fp8) == ops.INT8 else ops.FP8
+        self._fp8_weights = self.adaln.prepare_fp8_weights(dtype=self._w8_dtype) if self.fp8 else []
         self.step_cache, self.cfg_cache, self.guidance = step_cache, cfg_cache, guidance
         if guidance is not None:
             guidance.reset()
@@ -372,7 +375,7 @@ class GraphedStep:
         if g is not None and g.begin_step():
             return g.zero_step(self.x, self.scale, sigma, next_sigma, self.solver)
         if self.fp8:
-            self.adaln.prepare_fp8_weights()
+            self.adaln.prepare_fp8_weights(dtype=self._w8_dtype)
         cc = self.cfg_cache
         if cc is not None and cc.begin_step(self.x, sigma):
             self.ts1.fill_(float(sigma) * 1000.0)
